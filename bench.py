@@ -2,6 +2,7 @@
 
   python bench.py [--gpus N] [--steps K] [--warmup W]                (N>1: launched under torchrun, one rank per GPU)
   python bench.py --impl reference [--gpus N] [--steps K] [--warmup W]
+  python bench.py ... --dump-outputs DIR      (rank 0 writes what the last timed step computed as DIR/<name>.npy)
 
 Workload (BASELINE.json metric, configs[1]): 3-layer GraphSAGE (hidden 256, --use-pp, LayerNorm, dropout 0.5,
 lr 0.01, sampling rate 0.1) on the Reddit-shape synthetic power-law graph (232,965 nodes, ~114.6M edges, 602
@@ -10,7 +11,7 @@ boundary sampling -> id exchange -> forward (feature exchange + SpMM + dense) ->
 gradient exchange) -> weight-gradient all-reduce -> Adam.  The graph is fixed, so more GPUs = less work per GPU
 ("scaling": "strong").  value = epochs/sec of the whole job (max over ranks of the device-timed region).
 Besides the contract keys the line carries `roofline` (the SpMM, the dominant kernel: algorithmic bytes / CUDA-event
-time per launch, measured in an eager pass of the same step), `dense_roofline` (the tcgen05 GEMM family), `e2e`
+time per launch, measured in an eager pass of the same step), `dense_roofline` (the wgmma GEMM family), `e2e`
 (inputs copied from pinned host memory every epoch, loss read back), `cpu_baseline` (N=1), `exchange`, `clocks`.
 
 `--impl reference` times the CPU restatement of the reference (oracle/: torch CPU fp32 + C/OpenMP SpMM, P in-process
@@ -58,11 +59,11 @@ def load_peaks():
         with open(p) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -201,6 +202,7 @@ def run_ours(a):
 
     from bns_gcn_b200.module import dense as dense_mod
     dense_prof = []
+    last = {}                                            # what the last timed step returned (its loss)
 
     def timed(step_fn, n_steps, profile_spmm):
         """n_steps of step_fn between barriers; device time by CUDA events, max over ranks."""
@@ -214,7 +216,7 @@ def run_ours(a):
         e0.record(torch.cuda.current_stream(dev))
         torch.cuda.nvtx.range_push("bns_timed")          # ncu --nvtx --nvtx-include "bns_timed/" lists the steps
         for _ in range(n_steps):
-            step_fn()
+            last["loss"] = step_fn()
         torch.cuda.nvtx.range_pop()
         e1.record(torch.cuda.current_stream(dev))
         barrier()
@@ -228,11 +230,12 @@ def run_ours(a):
 
     def eager_step():
         nonlocal epoch
-        train.train_epoch(st, epoch)
+        loss = train.train_epoch(st, epoch)
         epoch += 1
         if world > 1:                                    # Comm(s) / Reduce(s) of EVERY eager epoch (train.py:415-418)
             comm_log.append(comm_timer.tot_time())
             reduce_log.append(ctx.reducer.last_reduce_seconds())
+        return loss
 
     # ---------------- eager pass: per-kernel CUDA events (roofline), Comm(s)/Reduce(s) -----------------------
     clocks = ClockSampler(local)
@@ -264,6 +267,8 @@ def run_ours(a):
             if a.strict:
                 raise
             dev_ms, n_launch, _ = timed(eager_step, K, False)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, st, last["loss"])
     n0, n1 = 0, n_launch
     clk = clocks.stop() if rank == 0 else None
     spmm_ms = sum(s.elapsed_time(e) for s, e, *_ in prof)
@@ -370,15 +375,9 @@ def run_ours(a):
     # boundary exchange (per rank, per epoch): rows sent forward + gradient rows returned, on every communicating layer
     n_comm_layers = max(WORKLOAD["n_layers"] - 1, 0)
     ex_bytes = 4 * WORKLOAD["n_hidden"] * (sum(st.send_size) + sum(st.recv_size)) * n_comm_layers if world > 1 else 0
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "spmm_traffic.json")
-    if os.path.exists(tp) and WORKLOAD["shape"] == "reddit":
-        # not measurable inside this run (ncu replays kernels): the per-launch DRAM bytes of the F = 256 inner SpMM from
-        # the committed capture of the same kernel on the same shape (tools/ncu_spmm_traffic.sh; world 1 and 4)
-        with open(tp) as f:
-            tj = json.load(f)
-        ent = tj.get(str(world)) or (tj if world == 1 else {})
-        traffic, traffic_src = ent.get("dram_bytes_per_launch"), ent.get("source")
+    # DRAM bytes per launch are not measurable inside this run (a hardware counter profiler replays kernels)
+    traffic, traffic_src = None, "not measured"
+    l2_mb = torch.cuda.get_device_properties(dev).L2_cache_size / 2 ** 20
     ach = spmm_alg / (spmm_ms * 1e-3) / 1e9 if spmm_ms > 0 else 0.0
     out = {
         "metric": METRIC(), "value": K / (dev_ms * 1e-3),
@@ -386,7 +385,7 @@ def run_ours(a):
         "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload_string(gstats, world),
                    "l2": f"no flush between timed epochs: one epoch of rank 0 streams {ws_mb:.0f} MB (features "
-                         f"{feat_mb:.0f} MB + CSR and transposes {csr_mb:.0f} MB + activations), L2 is 126 MB",
+                         f"{feat_mb:.0f} MB + CSR and transposes {csr_mb:.0f} MB + activations), L2 is {l2_mb:.0f} MB",
                    "parallelism": f"partition-parallel x{world}", "exchange": a.backend, "execution": mode,
                    "n_in_rank0": part.graph.n_in, "n_halo_rank0": part.graph.n_halo,
                    "local_edges_rank0": part.graph.num_edges()},
@@ -415,7 +414,7 @@ def run_ours(a):
                              "binding resource on this degree-492 graph, see DESIGN.md"},
     }
     if dense_prof and gemm_ms > 0:
-        # second kernel family of the step: the dense layers on tcgen05 (csrc/dense_tc.cuh).  3xTF32 issues three
+        # second kernel family of the step: the dense layers on wgmma (csrc/dense_tc.cuh).  3xTF32 issues three
         # tensor-core products per useful f32 one; TF32 dense peak is taken as half the measured bf16 cuBLAS rate
         # (MEASURED_PEAKS.json holds no TF32 figure; sustained, because the kernel runs inside a long step)
         try:
@@ -423,7 +422,7 @@ def run_ours(a):
                 pk = json.load(f)
             tf32_peak, tf32_src = 0.5 * float(pk.get("bf16_tflops_sustained") or pk["bf16_tflops"]), "0.5 x measured sustained bf16 (MEASURED_PEAKS.json)"
         except Exception:   # noqa: BLE001
-            tf32_peak, tf32_src = 0.5 * 1400.0, "0.5 x fallback sustained bf16 (B200_PROFILING.md)"
+            tf32_peak, tf32_src = 495.0, "H100 SXM data sheet, dense TF32 (not measured)"
         useful = gemm_flops / (gemm_ms * 1e-3) / 1e12
         out["dense_roofline"] = {"bound": "tensor", "kernel": "gemm3x_kernel (bns_dense_tn_3xtf32 / bns_dense_nt_3xtf32)",
                                  "achieved": 3.0 * useful, "peak": tf32_peak, "unit": "TFLOP/s", "frac": 3.0 * useful / tf32_peak,
@@ -431,9 +430,7 @@ def run_ours(a):
                                  "share_of_step": gemm_ms / eager_ms if eager_ms else None,
                                  "algorithmic_GBs": gemm_bytes / (gemm_ms * 1e-3) / 1e9,
                                  "note": "achieved = 3 x useful f32 FLOPs (hi*hi + hi*lo + lo*hi) / CUDA-event time of the "
-                                         "launches in the eager pass; the kernel is shared-memory-bandwidth bound (ncu: tensor "
-                                         "pipe 46 %, LSU + tensor-core shared-memory wavefronts 53 % + 51 %), see "
-                                         "profiles/ncu_gemm3x_r01.md"}
+                                         "launches in the eager pass"}
     if world == 1 and not a.no_cpu_baseline:
         out["cpu_baseline"] = cpu_epochs_per_sec(a.shape, 1, steps=1, warmup=1, probe=probe is not None)
         out["cpu_baseline"].pop("gstats", None)
@@ -447,6 +444,31 @@ def run_ours(a):
         out["parity_probe"] = probe
     emit(out)
     _leave(world)
+
+
+DUMP_LOGIT_ROWS = 65536      # a fixed, seeded sample of the logits rows keeps the dump far below 64 MB
+
+
+def dump_outputs(out_dir: str, st, loss) -> None:
+    """What the last timed step handed its caller, as float32 ``out_dir/<name>.npy``: the loss, the logits (at most
+    DUMP_LOGIT_ROWS rows, a sample drawn with a fixed seed) and every parameter after the optimizer step.  The inputs
+    are generated from fixed seeds, so two builds run with the same arguments can be compared file by file."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"loss": loss.detach().reshape(-1)}
+    logits = st.last_logits.detach()
+    if logits.shape[0] > DUMP_LOGIT_ROWS:
+        rows = torch.randperm(logits.shape[0], generator=torch.Generator().manual_seed(0))[:DUMP_LOGIT_ROWS].sort().values
+        logits = logits[rows.to(logits.device)]
+    arrays["logits"] = logits
+    for name, p in st.model.named_parameters():
+        arrays["param." + name] = p.detach()
+    total = 0
+    for name, t in arrays.items():
+        a_ = t.float().cpu().numpy()
+        total += a_.nbytes
+        np.save(os.path.join(out_dir, name + ".npy"), a_)
+    assert total <= 64 << 20, f"dump of {total} bytes exceeds 64 MB"
 
 
 def _leave(world: int) -> None:
@@ -682,6 +704,8 @@ def main():
                          "(post-mortem of a hang on a box nobody can attach to); 0 = off")
     ap.add_argument("--strict", action="store_true", help="fail instead of falling back to eager when capture fails")
     ap.add_argument("--profile", default="", help="write a torch.profiler kernel table of 3 epochs (rank 0) to this file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the loss, logits (sampled) and parameters of the last timed step (rank 0) to DIR/<name>.npy")
     # non-default workloads (the other BASELINE.json configs); the driver's contract run uses the defaults above
     ap.add_argument("--model", default=None, choices=["graphsage", "gcn", "gat"])
     ap.add_argument("--n-layers", type=int, default=None)

@@ -1,8 +1,8 @@
-"""bns-gcn_b200: the B200-native hot path of BNS-GCN (partition-parallel GCN training with
+"""bns-gcn_b200: the H100-native hot path of BNS-GCN (partition-parallel GCN training with
 random boundary-node sampling) behind the reference's own Python surface.
 
 Layout (mirrors the reference's tree so call sites read the same):
-  csrc/      sm_100a CUDA kernels + the C-ABI (``include/bnsgcn.h``) -> ``libbnsgcn.so``
+  csrc/      sm_90a CUDA kernels + the C-ABI (``include/bnsgcn.h``) -> ``libbnsgcn.so``
   _lib.py    ctypes binding of that library (fails loudly when it is missing)
   ops.py     ``torch.autograd.Function`` wrappers over the C-ABI calls
   module/    ``layer.py`` ``model.py``      (reference: module/layer.py, module/model.py)

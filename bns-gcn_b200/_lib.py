@@ -157,7 +157,7 @@ def _load() -> ctypes.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: the CUDA extension has not been built. Run `python __graft_entry__.py` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         try:

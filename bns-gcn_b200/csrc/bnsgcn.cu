@@ -1,4 +1,4 @@
-// bnsgcn.cu -- sm_100a kernels + the C ABI of include/bnsgcn.h.
+// bnsgcn.cu -- sm_90a kernels + the C ABI of include/bnsgcn.h.
 //
 // Hot kernels (all HBM/L2-bound f32 gather / scatter work; no tensor-core shaped math here):
 //   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers
@@ -7,7 +7,7 @@
 //   philox_key / take  K6         counter-based exactly-k sampling (with cub radix sort)
 //   p2p_put_rows       K3+C1      pack straight into the peer's receive slab over NVLink + flag
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 --shared -Xcompiler -fPIC
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 --shared -Xcompiler -fPIC
 #include "bnsgcn.h"
 
 #include <cuda_runtime.h>
@@ -50,7 +50,7 @@ inline cudaStream_t as_stream(void *s) { return reinterpret_cast<cudaStream_t>(s
 
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
-constexpr int kDefaultChunk = 256;   // B200 sweep (profiles/spmm_chunk_sweep_r1.txt): 256 -> 7.39 ms, 512 -> 7.58, 1024 -> 8.34, 2048 -> 9.27
+constexpr int kDefaultChunk = 256;   // nnz per work item; larger chunks were slower in a sweep of 256..2048 on the previous GPU
 
 std::atomic<unsigned long long> g_launches{0};   // kernels of this library enqueued so far (bench.py gpu_launches)
 
@@ -72,7 +72,7 @@ int sm_count() {
     const int dev = current_device();
     int n = g_dev[dev].sms.load(std::memory_order_relaxed);
     if (n == 0) {
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;   // H100 SXM
         g_dev[dev].sms.store(n, std::memory_order_relaxed);
     }
     return n;
@@ -461,9 +461,8 @@ __device__ __forceinline__ int32_t ld_stream_i32(const int32_t *p) {
 // slab row, -1 = skip), compacted through shared memory and then consumed UNROLL at a time so that
 // UNROLL*NV independent 16-byte gathers are in flight per lane.
 //
-// Cache blocking (the ncu capture of round 1 showed why: with the whole F = 256 row per gather the 238 MB
-// source matrix of the Reddit-shape graph misses the 126 MB L2 58 % of the time and the kernel moves 53 GB
-// of DRAM per launch for 0.9 GB of algorithmic bytes).  The feature dimension is cut into column slabs of
+// Cache blocking (with the whole F = 256 row per gather the 238 MB source matrix of the Reddit-shape graph is
+// several times the size of the L2, so most gathers miss it and go to DRAM).  The feature dimension is cut into column slabs of
 // SLAB = G*W*NV floats chosen so that (source rows x SLAB x 4 B) stays L2-resident; work items are ordered
 // slab-major, so at any moment all resident warps gather from the same slab.  For narrow slabs a warp is
 // split into 32/G row groups of G lanes that walk different entries of the chunk concurrently (every lane
@@ -702,7 +701,7 @@ int64_t l2_bytes() {
     long long v = g_dev[dev].l2.load(std::memory_order_relaxed);
     if (v == 0) {
         int b = 0;
-        v = (cudaDeviceGetAttribute(&b, cudaDevAttrL2CacheSize, dev) == cudaSuccess && b > 0) ? b : (126ll << 20);
+        v = (cudaDeviceGetAttribute(&b, cudaDevAttrL2CacheSize, dev) == cudaSuccess && b > 0) ? b : (50ll << 20);   // H100 SXM
         g_dev[dev].l2.store(v, std::memory_order_relaxed);
     }
     return v;
@@ -716,9 +715,7 @@ int pick_slab(int64_t F, int64_t x_rows, int32_t forced) {
         int v = atoi(env);
         if (v == 256 || v == 128 || v == 64 || v == 32) return v;
     }
-    // Measured on B200 (profiles/spmm_slab_sweep_r1.md, Reddit-shape, F = 256, 238 MB of sources): slab 256 ->
-    // 10.2 ms, 128 -> 8.1 ms, 64 -> 8.5 ms, 32 -> 14.1 ms; a 51 MB source matrix is fastest unblocked.  So: full
-    // rows while they fit comfortably, else 128 floats (a slab about the size of L2 still wins: the slab-major
+    // Full rows while they fit comfortably, else 128 floats (a slab about the size of L2 still wins: the slab-major
     // order keeps the hot part resident and halves the index re-reads of 64), else 64; never 32.  When even a
     // 64-float slab cannot be L2-resident the gather is a pure HBM stream and the widest slab is best.
     const double l2 = (double)l2_bytes(), bytes_per_col = (double)x_rows * 4.0;
@@ -956,7 +953,7 @@ extern "C" int bns_sddmm_dot_f32(const bns_graph_t *g, const float *A, int64_t l
     unsigned gx = (unsigned)(want < cap ? (want > 0 ? want : 1) : cap);
     cudaStream_t st = as_stream(stream);
     const int nv = (int)((F + 127) / 128);
-    // gathered rows in flight per lane, measured on the Yelp shape (profiles/gat_r02.md): F = 256: 8 (3.2 ms) beats 4 (3.9 ms);
+    // gathered rows in flight per lane, measured on the Yelp shape: F = 256: 8 beats 4;
     // F = 100: 4 (1.46 ms) beats 8 (1.76 ms)
     if (nv <= 1) sddmm_dot_kernel<1, 4><<<gx, kThreads, 0, st>>>(a);
     else if (nv == 2) sddmm_dot_kernel<2, 8><<<gx, kThreads, 0, st>>>(a);
@@ -1837,6 +1834,6 @@ extern "C" int bns_p2p_wait_flag(bns_p2p_t *p, int32_t flag_index, uint64_t flag
 #include "comm.cuh"
 
 // =================================================================================================
-// K8: dense layers on tcgen05 (3xTF32 with the operand split fused into the pipeline)
+// K8: dense layers on wgmma (3xTF32 with the operand split fused into the pipeline)
 // =================================================================================================
 #include "dense_tc.cuh"

@@ -1,32 +1,31 @@
 // dense_tc.cuh -- K8, the dense layers of the path (nn.Linear at module/layer.py:30, 38, 83, 92 of the reference)
-// on the 5th-generation tensor cores: tcgen05.mma kind::tf32, accumulator in TMEM, operands staged by TMA.
+// on the Hopper tensor cores: wgmma.mma_async .tf32 with f32 register accumulators, operands staged by TMA.
 // Included at the end of bnsgcn.cu (same translation unit: shares fail(), BNS_CUDA, the launch counter).
 //
 // Why not one TF32 GEMM: the parity bar is 1e-4 on layer outputs (f32 in the reference: torch 1.12 has
 // allow_tf32 = False for matmul); a 10-bit mantissa misses it.  The kernel therefore computes the error-compensated
-// 3xTF32 product  A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (hi = the TF32 part of x, lo = x - hi, exact in f32; the
-// dropped lo*lo term is ~2^-20 relative) with the operand split done INSIDE the pipeline: TMA lands the raw f32 tile
-// in shared memory, four "split" warps write lo beside it (element-wise, so the 128-byte swizzle pattern is
-// untouched; hi is the raw tile itself, see kTrunc below), then one thread issues the three MMAs per 8-wide k-step.
-// HBM/L2 see every operand once; the library-composed variant (module/dense.py "3xtf32") needs a split pass plus
-// three GEMMs.
+// 3xTF32 product  A*B ~= A_hi*B_hi + A_hi*B_lo + A_lo*B_hi  (hi = x with its 13 low mantissa bits cleared, lo = x - hi,
+// exact in f32; the dropped lo*lo term is ~2^-20 relative) with the operand split done INSIDE the pipeline: TMA lands
+// the raw f32 tile in shared memory, the consumer warpgroups write hi and lo into a K-major 128-byte-swizzled operand
+// buffer (transposing on the way for the MN-major layout: wgmma takes .tf32 operands K-major only), then issue the
+// three products per 8-wide k-step.  HBM/L2 see every operand once; the library-composed variant (module/dense.py
+// "3xtf32") needs a split pass plus three GEMMs.
 //
 // A work item = one 128 x 128 output tile (x one slice of the contraction for the weight-gradient shape); persistent CTAs
-// of 320 threads walk the items:
-//   warp 0      TMA producer (one lane)
-//   warp 1      TMEM allocator + MMA issuer (one lane)
-//   warps 2..5  split stage
-//   warps 6..9  epilogue (tcgen05.ld -> sum of the chains -> +bias -> global), overlapped with the next item's main loop
-// Pipeline barriers per stage: full (TMA -> split, transaction bytes), split (4 warps -> MMA), empty (tcgen05.commit
-// -> TMA); per TMEM buffer: acc_full (last commit -> epilogue), acc_empty (epilogue -> MMA).
+// of 288 threads walk the items:
+//   warps 0..3  consumer warpgroup 0: output rows [0, 64) of the tile
+//   warps 4..7  consumer warpgroup 1: output rows [64, 128)
+//   warp 8      TMA producer (one lane)
+// Each consumer warpgroup splits half of the A and half of the B tile, so both halves of B are complete only after a
+// named barrier of the 256 consumer threads.  The split of k-block i+1 runs on the CUDA cores while the wgmmas of
+// k-block i run on the tensor cores; two operand buffers alternate between them.  Barriers: full[s] (TMA -> consumers,
+// transaction bytes) and empty[s] (consumers -> TMA) per stage of the raw ring.
 //
-// Accumulation chains.  The tensor core adds into the TMEM accumulator with truncation, so the error of one long
-// chain grows linearly (measured on B200: ~2.5e-7 of max|C| per 32-wide k-block, 2.6e-4 after 1040 k-blocks).  Two
-// counter-measures keep the result at cuBLAS-f32 level: k-blocks go round-robin into kAcc accumulators that the epilogue
-// adds in f32 (shorter chains), and the weight-gradient contraction is cut into slices of <= kMaxChainKb k-blocks whose
-// partial tiles are summed by splitk_reduce_kernel in slice order (round-to-nearest f32, deterministic).
+// Accumulation chains.  k-blocks go round-robin into kAcc register accumulators that the epilogue adds in f32 (shorter
+// chains of tensor-core additions), and the weight-gradient contraction is cut into slices of <= kMaxChainKb k-blocks
+// whose partial tiles are summed by splitk_reduce_kernel in slice order (round-to-nearest f32, deterministic).
 //
-// Two operand layouts, through SWIZZLE_128B (K-major) / SWIZZLE_128B_ATOM_32B (MN-major) tensor maps:
+// Two operand layouts, both loaded through SWIZZLE_128B tensor maps:
 //   kMN = false  A [M, K], B [N, K] row-major: contraction contiguous ("K-major").  forward  Y = X W^T + b  and the
 //                input gradient  dX = dY (W^T)^T  (the caller passes a transposed copy of the small weight).
 //   kMN = true   A [R, M], B [R, N] row-major: contraction over the R rows ("MN-major").  weight gradient
@@ -36,21 +35,21 @@
 namespace tc {
 
 constexpr int BM = 128, BN = 128, BK = 32;     // BK f32 = 128 bytes = one swizzle row
-constexpr int UMMA_K = 8;                       // kind::tf32: 8 elements (32 bytes) of contraction per instruction
-constexpr int kStages = 3;
+constexpr int WG_K = 8;                         // wgmma .tf32: 8 elements (32 bytes) of contraction per instruction
+constexpr int kStages = 3;                      // raw ring (TMA destination)
 constexpr int A_BYTES = BM * BK * 4;            // 16 KB
 constexpr int B_BYTES = BN * BK * 4;            // 16 KB
-constexpr int RAW_BYTES = A_BYTES + B_BYTES;    // TMA lands here: the hi parts (the tensor core drops the low bits)
-constexpr int STAGE_BYTES = 2 * RAW_BYTES;      // [A_hi | B_hi | A_lo | B_lo]
-constexpr int kThreadsTc = 320;                 // warp 0 TMA, warp 1 MMA, warps 2-5 split, warps 6-9 epilogue
-constexpr int kSplitThreads = 128;
-constexpr int kEpiThreads = 128;
-constexpr int kAcc = 2;                         // round-robin TMEM accumulators per item (see "accumulation chains" above)
-constexpr int kTmemCols = 2 * kAcc * BN;        // 2 buffers x kAcc chains x one f32 column per output column = all 512
+constexpr int RAW_BYTES = A_BYTES + B_BYTES;
+constexpr int OP_BYTES = 2 * RAW_BYTES;         // operand buffer [A_hi | B_hi | A_lo | B_lo], K-major, 128-byte swizzle
+constexpr int kOpBufs = 2;
+constexpr int kConsumerThreads = 256;           // two warpgroups
+constexpr int kThreadsTc = kConsumerThreads + 32;
+constexpr int kAcc = 2;                         // round-robin accumulators per item (see "accumulation chains" above)
 constexpr int kMaxChainKb = 48;                 // weight-gradient slices: at most this many k-blocks per item (24 per chain)
 constexpr int BAR_BYTES = 256;
-constexpr int SMEM_BYTES = kStages * STAGE_BYTES + BAR_BYTES + 1024;   // + slack to align the stages to 1024
+constexpr int SMEM_BYTES = kStages * RAW_BYTES + kOpBufs * OP_BYTES + BAR_BYTES + 1024;   // + slack to align to 1024
 constexpr int MN_BOX_BYTES = BK * 128;          // MN-major: one TMA box = BK rows x 32 floats
+static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the shared memory of one block");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -92,117 +91,137 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map
         : "memory");
 }
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
+// the 256 consumer threads (named barrier 1; 0 is __syncthreads)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumerThreads) : "memory"); }
+
+// wgmma shared-memory matrix descriptor, K-major with 128-byte swizzle (layout type 1): 8-row groups of 128-byte rows,
+// SBO = 1024 (next 8 rows), LBO unused (one swizzle atom along K).  Stepping k inside the atom adds 32 bytes to the start.
+__device__ __forceinline__ uint64_t smem_desc(uint32_t addr) {
+    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// d[64 x 128] += A[64 x 8] * B[128 x 8]^T  (one warpgroup; d in the wgmma accumulator fragment layout)
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1)
         : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// Shared-memory matrix descriptor (sm_100 "version 1").  Offsets are in 16-byte units.
-//   K-major  (layout 2 = SWIZZLE_128B, 16-byte chunks XOR row%8): 8-row groups of 128-byte rows, SBO = 1024 (next 8
-//            rows); LBO unused (one swizzle atom along K)
-//   MN-major (layout 1 = SWIZZLE_128B_BASE32B, 32-byte chunks XOR row%4 -- the only MN-major layout the hardware takes
-//            for 32-bit operands; TMA writes it with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): atoms of 32 elements x 4
-//            contraction rows; LBO = next 32 elements (one TMA box further), SBO = next 4 contraction rows (512 bytes)
-__device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
-    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) | ((uint64_t)layout << 61);
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// The 12 wgmmas of one BK-wide k-block for consumer warpgroup wg (its 64 A rows against all 128 B rows).
+__device__ __forceinline__ void mma_kblock(float (&d)[64], uint32_t op, uint32_t wg) {
+    const uint32_t a_hi = op + wg * (64 * 128), b_hi = op + A_BYTES;
+    const uint32_t a_lo = a_hi + RAW_BYTES, b_lo = b_hi + RAW_BYTES;
+#pragma unroll
+    for (int k = 0; k < BK / WG_K; ++k) {
+        const uint32_t ko = k * WG_K * 4;
+        const uint64_t dah = smem_desc(a_hi + ko), dbh = smem_desc(b_hi + ko);
+        const uint64_t dal = smem_desc(a_lo + ko), dbl = smem_desc(b_lo + ko);
+        wgmma_tf32(d, dal, dbh);        // small terms first
+        wgmma_tf32(d, dah, dbl);
+        wgmma_tf32(d, dah, dbh);
+    }
 }
 
-__device__ __forceinline__ float tf32_rna(float x) {
-    uint32_t u;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-    return __uint_as_float(u);
+// Consumer warpgroup wg's share of the split: rows [64 wg, 64 wg + 64) of the A and of the B tile of raw stage `raw`
+// -> hi / lo of operand buffer `op`, K-major with the 128-byte swizzle (16-byte chunk c of row r at chunk c ^ (r % 8)).
+// Lanes walk consecutive rows, which keeps every shared-memory access of a warp free of bank conflicts.
+template <bool kMN>
+__device__ __forceinline__ void split_stage(const uint8_t *raw, uint8_t *op, int wg, int t) {
+#pragma unroll
+    for (int part = 0; part < 2; ++part) {           // 0: A, 1: B (same geometry, B starts A_BYTES further)
+        const int region = part * A_BYTES;
+#pragma unroll
+        for (int j = 0; j < (64 * BK / 4) / 128; ++j) {
+            const int idx = t + 128 * j;
+            const int r = 64 * wg + (idx & 63), k4 = idx >> 6;
+            const int dst = region + r * 128 + ((k4 ^ (r & 7)) << 4);
+            float4 x;
+            if (!kMN) {
+                x = *reinterpret_cast<const float4 *>(raw + dst);
+            } else {
+                // MN-major box b = r / 32 holds BK contraction rows of 32 floats; element (k, m) at k * 128 + swizzled m
+                const uint8_t *box = raw + region + (r >> 5) * MN_BOX_BYTES;
+                const int mm = r & 31;
+                float e[4];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int k = 4 * k4 + q;
+                    e[q] = *reinterpret_cast<const float *>(box + k * 128 + ((((mm >> 2) ^ (k & 7))) << 4) + (mm & 3) * 4);
+                }
+                x = make_float4(e[0], e[1], e[2], e[3]);
+            }
+            float4 h, l;
+            h.x = __uint_as_float(__float_as_uint(x.x) & 0xffffe000u); h.y = __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
+            h.z = __uint_as_float(__float_as_uint(x.z) & 0xffffe000u); h.w = __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
+            l.x = x.x - h.x; l.y = x.y - h.y; l.z = x.z - h.z; l.w = x.w - h.w;
+            *reinterpret_cast<float4 *>(op + dst) = h;
+            *reinterpret_cast<float4 *>(op + RAW_BYTES + dst) = l;
+        }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> visible to wgmma's async reads
 }
 
-// kTrunc: hi = x with the 13 low mantissa bits ignored BY THE TENSOR CORE (kind::tf32 reads the raw f32 words and drops
-// them -- verified on B200: same accuracy as the rounded variant), lo = x - trunc(x); saves the hi write-back, a third of
-// the split stage's shared-memory traffic.  Off (BNS_TC_TRUNC=0): hi = round-to-nearest TF32, written back in place.
-//
 // Persistent: gridDim.x = min(work items, SMs); a work item = (output tile, contraction slice).  All roles walk the same
-// item sequence; the shared-memory ring and its phases run on across items, and the accumulators are double-buffered in
-// TMEM (2 buffers x kAcc chains x 128 columns = all 512) so the epilogue of item i overlaps the main loop of item i+1.
-template <bool kMN, bool kTrunc>
+// item sequence; the raw ring and its phases run on across items.
+template <bool kMN>
 __global__ void __launch_bounds__(kThreadsTc, 1)
 gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
               float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
               const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
               int tiles_n, int tiles, int splits) {
     extern __shared__ uint8_t smem_raw[];
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t bars = base + kStages * STAGE_BYTES;
-    // barrier slots (8 bytes each): full[s], split[s], empty[s], acc_full[2], acc_empty[2]; then the TMEM base address
+    const uint32_t ops = base + kStages * RAW_BYTES;
+    const uint32_t bars = ops + kOpBufs * OP_BYTES;
     auto full_bar = [&](int s) { return bars + 8u * s; };
-    auto split_bar = [&](int s) { return bars + 8u * (kStages + s); };
-    auto empty_bar = [&](int s) { return bars + 8u * (2 * kStages + s); };
-    auto acc_full_bar = [&](int b) { return bars + 8u * (3 * kStages + b); };
-    auto acc_empty_bar = [&](int b) { return bars + 8u * (3 * kStages + 2 + b); };
-    volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(base_ptr + kStages * STAGE_BYTES + 8 * (3 * kStages + 4));
+    auto empty_bar = [&](int s) { return bars + 8u * (kStages + s); };
 
     const int total_work = tiles * splits;
 
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+    if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(split_bar(s), kSplitThreads / 32);
             mbar_init(empty_bar(s), 1);
         }
-        for (int b = 0; b < 2; ++b) {
-            mbar_init(acc_full_bar(b), 1);
-            mbar_init(acc_empty_bar(b), kEpiThreads / 32);
-        }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void *)tmem_slot)),
-                     "r"((uint32_t)kTmemCols)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    // work item w -> tile (m_t, n_t), contraction slice [kb0, kb1)
+    // work item w -> tile (m_t, n_t), contraction slice [kb0, kb0 + nkb)
 #define BNS_TC_ITEM(w)                                                        \
     const int split_ = (w) / tiles, tile_ = (w) % tiles;                      \
     const int m_t = tile_ / tiles_n, n_t = tile_ % tiles_n;                   \
     const int kb0 = (int)(((int64_t)split_ * num_kb) / splits);               \
     const int nkb = (int)(((int64_t)(split_ + 1) * num_kb) / splits) - kb0;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    // warpgroup index, broadcast so that the compiler sees it warp-uniform (wgmma under a divergent branch is serialized)
+    const int wg = __shfl_sync(0xffffffffu, (int)threadIdx.x / 128, 0);
+    if (wg * 128 >= kConsumerThreads) {
+        if (threadIdx.x == kConsumerThreads) {
             // ===== TMA producer =====
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+            asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
             uint32_t g = 0;                                  // k-blocks issued so far (ring position)
             for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
                 BNS_TC_ITEM(w)
@@ -210,7 +229,7 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                     const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
                     mbar_wait(empty_bar(s), ph ^ 1u);
                     mbar_expect_tx(full_bar(s), RAW_BYTES);
-                    const uint32_t a_dst = base + s * STAGE_BYTES, b_dst = a_dst + A_BYTES;
+                    const uint32_t a_dst = base + s * RAW_BYTES, b_dst = a_dst + A_BYTES;
                     const int kc = (kb0 + i) * BK;
                     if (!kMN) {
                         tma_load_2d(a_dst, &map_a, full_bar(s), kc, m_t * BM);
@@ -224,398 +243,75 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
                 }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ===== MMA issuer =====
-            // instruction descriptor: D f32, A/B tf32, M = 128, N = 128, majorness per layout
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((kMN ? 1u : 0u) << 15) | ((kMN ? 1u : 0u) << 16) |
-                                   ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-            const uint32_t lbo = kMN ? (uint32_t)MN_BOX_BYTES : 0u, sbo = kMN ? 512u : 1024u, lay = kMN ? 1u : 2u;
-            const uint32_t kstep = kMN ? 1024u : (uint32_t)(UMMA_K * 4);
-            uint32_t g = 0, it = 0;
-            for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++it) {
-                BNS_TC_ITEM(w)
-                (void)m_t; (void)n_t; (void)kb0;
-                const uint32_t buf = it & 1u;
-                mbar_wait(acc_empty_bar(buf), ((it >> 1) & 1u) ^ 1u);      // epilogue has drained this buffer
-                tc_fence_after();
-                for (int i = 0; i < nkb; ++i, ++g) {
-                    const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
-                    mbar_wait(split_bar(s), ph);
-                    tc_fence_after();
-                    const uint32_t a_hi = base + s * STAGE_BYTES, b_hi = a_hi + A_BYTES;
-                    const uint32_t a_lo = a_hi + RAW_BYTES, b_lo = a_lo + A_BYTES;
-                    const uint32_t d = tmem_base + (buf * kAcc + (uint32_t)(i % kAcc)) * BN;
+        return;
+    }
+
+    // ===== consumer warpgroups: split -> wgmma -> epilogue =====
+    const int t = threadIdx.x % 128;
+    const int warp = t / 32, lane = t % 32;
+    // stage g: wait for its bytes, split it into operand buffer g % 2, release it to the producer once both
+    // warpgroups are done with it (the barrier also publishes both halves of the operand buffer)
+    auto split_kblock = [&](uint32_t g) {
+        const uint32_t s = g % kStages;
+        mbar_wait(full_bar(s), (g / kStages) & 1u);
+        split_stage<kMN>(base_ptr + s * RAW_BYTES, base_ptr + kStages * RAW_BYTES + (g & 1u) * OP_BYTES, wg, t);
+    };
+    auto publish_kblock = [&](uint32_t g) {
+        consumers_sync();
+        if (threadIdx.x == 0) mbar_arrive(empty_bar(g % kStages));
+    };
+    uint32_t g = 0;                                          // k-blocks consumed so far (ring position)
+    for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
+        BNS_TC_ITEM(w)
+        (void)kb0;
+        float acc0[64], acc1[64];
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t dah = smem_desc(a_hi + k * kstep, lbo, sbo, lay), dbh = smem_desc(b_hi + k * kstep, lbo, sbo, lay);
-                        const uint64_t dal = smem_desc(a_lo + k * kstep, lbo, sbo, lay), dbl = smem_desc(b_lo + k * kstep, lbo, sbo, lay);
-                        umma_tf32(d, dal, dbh, idesc, (i >= kAcc || k != 0) ? 1u : 0u);    // small terms first
-                        umma_tf32(d, dah, dbl, idesc, 1u);
-                        umma_tf32(d, dah, dbh, idesc, 1u);
-                    }
-                    umma_commit(empty_bar(s));       // stage free once these MMAs have read it
-                }
-                umma_commit(acc_full_bar(buf));      // this item's accumulators are complete
-            }
+        for (int e = 0; e < 64; ++e) acc0[e] = acc1[e] = 0.f;
+        split_kblock(g);
+        publish_kblock(g);
+        for (int i = 0; i < nkb; ++i, ++g) {
+            const uint32_t op = ops + (g & 1u) * OP_BYTES;
+            wgmma_fence();
+            if (i % kAcc == 0) mma_kblock(acc0, op, wg);
+            else mma_kblock(acc1, op, wg);
+            wgmma_commit();
+            if (i + 1 < nkb) split_kblock(g + 1);            // CUDA cores: next k-block while the tensor cores run
+            wgmma_wait_all();
+            if (i + 1 < nkb) publish_kblock(g + 1);          // after the wait: both warpgroups' reads of buffer g are done
         }
-    } else if (warp < 2 + kSplitThreads / 32) {
-        // ===== split warps =====
-        const int t = threadIdx.x - 64;
-        uint32_t g = 0;
-        for (int w = blockIdx.x; w < total_work; w += gridDim.x) {
-            BNS_TC_ITEM(w)
-            (void)m_t; (void)n_t; (void)kb0;
-            for (int i = 0; i < nkb; ++i, ++g) {
-                const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
-                mbar_wait(full_bar(s), ph);
-                float4 *raw = reinterpret_cast<float4 *>(base_ptr + s * STAGE_BYTES);
-                float4 *lo = reinterpret_cast<float4 *>(base_ptr + s * STAGE_BYTES + RAW_BYTES);
-#pragma unroll 4
-                for (int j = 0; j < RAW_BYTES / 16 / kSplitThreads; ++j) {
-                    const int idx = t + j * kSplitThreads;
-                    const float4 x = raw[idx];
-                    float4 h, l;
-                    if (kTrunc) {
-                        h.x = __uint_as_float(__float_as_uint(x.x) & 0xffffe000u); h.y = __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
-                        h.z = __uint_as_float(__float_as_uint(x.z) & 0xffffe000u); h.w = __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
-                    } else {
-                        h.x = tf32_rna(x.x); h.y = tf32_rna(x.y); h.z = tf32_rna(x.z); h.w = tf32_rna(x.w);
-                        raw[idx] = h;
-                    }
-                    l.x = x.x - h.x; l.y = x.y - h.y; l.z = x.z - h.z; l.w = x.w - h.w;
-                    lo[idx] = l;
-                }
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> visible to the MMA's async reads
-                __syncwarp();
-                if (lane == 0) mbar_arrive(split_bar(s));
-            }
-        }
-    } else {
-        // ===== epilogue warps: TMEM -> (+ other chains, + bias) -> global =====
-        const uint32_t q = warp & 3u;                    // TMEM lane quadrant this warp may read
-        uint32_t it = 0;
-        for (int w = blockIdx.x; w < total_work; w += gridDim.x, ++it) {
-            BNS_TC_ITEM(w)
-            (void)kb0;
-            const uint32_t buf = it & 1u;
-            mbar_wait(acc_full_bar(buf), (it >> 1) & 1u);
-            tc_fence_after();
-            const int nacc = nkb < kAcc ? nkb : kAcc;
-            const int row = m_t * BM + (int)(32 * q + lane);
-            float *Cout = C + (int64_t)split_ * split_stride + (int64_t)row * ldc;
+
+        // ===== epilogue: sum of the chains (fixed order) -> + bias -> + addend -> * row_scale -> global =====
+        // fragment: d[4j + 2h + e] = row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e
+        float *Cs = C + (int64_t)split_ * split_stride;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = m_t * BM + 64 * wg + 16 * warp + (lane >> 2) + 8 * h;
+            if (row >= M) continue;
+            float *Cout = Cs + (int64_t)row * ldc;
             const float *Add = addend ? addend + (int64_t)row * ldadd : nullptr;
-            const float rsc = (row_scale && row < M) ? __ldg(row_scale + row) : 1.f;
-            const uint32_t tbase = tmem_base + ((32u * q) << 16) + buf * (uint32_t)(kAcc * BN);
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tbase + (uint32_t)(c * 32), v);
-                for (int a = 1; a < nacc; ++a) {            // the other accumulation chains, fixed order
-                    uint32_t u[32];
-                    tmem_ld32(tbase + (uint32_t)(a * BN + c * 32), u);
+            const float rsc = row_scale ? __ldg(row_scale + row) : 1.f;
 #pragma unroll
-                    for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(u[e]));
-                }
-                const int col0 = n_t * BN + c * 32;
-                if (row < M) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int col = col0 + 4 * j;
-                        if (col + 3 < N) {
-                            float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                   __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                            if (bias) {
-                                const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + col));
-                                o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-                            }
-                            if (Add) {
-                                const float4 aa = *reinterpret_cast<const float4 *>(Add + col);
-                                o.x += aa.x; o.y += aa.y; o.z += aa.z; o.w += aa.w;
-                            }
-                            if (row_scale) { o.x *= rsc; o.y *= rsc; o.z *= rsc; o.w *= rsc; }
-                            *reinterpret_cast<float4 *>(Cout + col) = o;
-                        } else {
-                            for (int e = 0; e < 4; ++e)
-                                if (col + e < N)
-                                    Cout[col + e] = (__uint_as_float(v[4 * j + e]) + (bias ? bias[col + e] : 0.f) + (Add ? Add[col + e] : 0.f)) * rsc;
-                        }
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = n_t * BN + 8 * j + 2 * (lane & 3);
+                float o[2] = {acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h], acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1]};
+                if (col + 1 < N) {
+                    if (bias) {
+                        const float2 bb = __ldg(reinterpret_cast<const float2 *>(bias + col));
+                        o[0] += bb.x; o[1] += bb.y;
                     }
+                    if (Add) {
+                        const float2 aa = *reinterpret_cast<const float2 *>(Add + col);
+                        o[0] += aa.x; o[1] += aa.y;
+                    }
+                    if (row_scale) { o[0] *= rsc; o[1] *= rsc; }
+                    *reinterpret_cast<float2 *>(Cout + col) = make_float2(o[0], o[1]);
+                } else if (col < N) {
+                    Cout[col] = (o[0] + (bias ? bias[col] : 0.f) + (Add ? Add[col] : 0.f)) * rsc;
                 }
             }
-            tc_fence_before();                           // TMEM reads done -> the MMA issuer may overwrite this buffer
-            __syncwarp();
-            if (lane == 0) mbar_arrive(acc_empty_bar(buf));
         }
     }
 #undef BNS_TC_ITEM
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)kTmemCols) : "memory");
-    }
-}
-
-// =====================================================================================================================
-// cta_group::2 variant: a CTA PAIR computes a 256 x 256 tile.  CTA c of the pair keeps A rows [128c, 128c + 128) and the
-// B rows (output columns) [128c, 128c + 128) of the pair tile -- the same 64 KB stage as the single-CTA kernel -- and the
-// leader issues  tcgen05.mma.cta_group::2  (M = 256, N = 256): each tensor core reads its own A tile and BOTH halves
-// of B, so the shared-memory operand reads per output halve (the single-CTA kernel is bound by exactly those reads).
-//   full[s]      local  : TMA -> this CTA's split warps
-//   split[s]     LEADER : 4 split warps of EACH CTA arrive (count 8; remote arrive through mapa)
-//   empty[s]     both   : the leader's tcgen05.commit multicasts to both CTAs -> each TMA producer
-//   acc_full     both   : multicast commit after the item's last k-block -> each CTA's epilogue warps
-//   acc_empty    LEADER : 4 epilogue warps of each CTA arrive (count 8) -> the MMA issuer may start the next item
-// TMEM: kAcc = 2 chains x 256 columns = all 512 columns, i.e. single-buffered: the epilogue is NOT overlapped here.
-// Enable with BNS_TC_PAIR=1 (module/dense.py picks it for N >= 192); validate with tools/check_dense_tc.py first.
-constexpr int BNP = 256;                        // pair tile width (and height: 2 x BM)
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the barrier at the same shared-memory offset in CTA `cta` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-    asm volatile(
-        "{\n"
-        ".reg .b32 rem;\n"
-        "mapa.shared::cluster.u32 rem, %0, %1;\n"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [rem];\n"
-        "}\n" ::"r"(bar), "r"(cta)
-        : "memory");
-}
-__device__ __forceinline__ void umma_tf32_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                               uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit_pair(uint32_t bar) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-        "h"((uint16_t)3)
-        : "memory");
-}
-
-template <bool kMN>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreadsTc, 1)
-gemm3x_pair_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                   float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
-                   const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N,
-                   int num_kb, int tiles_n, int tiles, int splits) {
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t cta = cluster_ctarank();
-    const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
-    const uint32_t bars = base + kStages * STAGE_BYTES;
-    auto full_bar = [&](int s) { return bars + 8u * s; };
-    auto split_bar = [&](int s) { return bars + 8u * (kStages + s); };
-    auto empty_bar = [&](int s) { return bars + 8u * (2 * kStages + s); };
-    const uint32_t acc_full_bar = bars + 8u * (3 * kStages);
-    const uint32_t acc_empty_bar = bars + 8u * (3 * kStages + 1);
-    volatile uint32_t *tmem_slot = reinterpret_cast<volatile uint32_t *>(base_ptr + kStages * STAGE_BYTES + 8 * (3 * kStages + 2));
-
-    const int total_work = tiles * splits;
-    const int pair = blockIdx.x >> 1, n_pairs = gridDim.x >> 1;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
-        for (int s = 0; s < kStages; ++s) {
-            mbar_init(full_bar(s), 1);
-            mbar_init(split_bar(s), 2 * (kSplitThreads / 32));      // used on the leader only
-            mbar_init(empty_bar(s), 1);
-        }
-        mbar_init(acc_full_bar, 1);
-        mbar_init(acc_empty_bar, 2 * (kEpiThreads / 32));           // used on the leader only
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("fence.proxy.async;" ::: "memory");
-    }
-    if (warp == 1) {      // both CTAs, same warp id, same slot offset
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32((const void *)tmem_slot)),
-                     "r"(512u)
-                     : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    cluster_sync_all();              // the peer's barriers exist before anybody arrives on them remotely
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-#define BNS_TC_PAIR_ITEM(w)                                                   \
-    const int split_ = (w) / tiles, tile_ = (w) % tiles;                      \
-    const int m_t = tile_ / tiles_n, n_t = tile_ % tiles_n;                   \
-    const int kb0 = (int)(((int64_t)split_ * num_kb) / splits);               \
-    const int nkb = (int)(((int64_t)(split_ + 1) * num_kb) / splits) - kb0;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            uint32_t g = 0;
-            for (int w = pair; w < total_work; w += n_pairs) {
-                BNS_TC_PAIR_ITEM(w)
-                const int m0 = m_t * 2 * BM + (int)cta * BM, n0 = n_t * BNP + (int)cta * BN;
-                for (int i = 0; i < nkb; ++i, ++g) {
-                    const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
-                    mbar_wait(empty_bar(s), ph ^ 1u);
-                    mbar_expect_tx(full_bar(s), RAW_BYTES);
-                    const uint32_t a_dst = base + s * STAGE_BYTES, b_dst = a_dst + A_BYTES;
-                    const int kc = (kb0 + i) * BK;
-                    if (!kMN) {
-                        tma_load_2d(a_dst, &map_a, full_bar(s), kc, m0);
-                        tma_load_2d(b_dst, &map_b, full_bar(s), kc, n0);
-                    } else {
-#pragma unroll
-                        for (int b = 0; b < BM / 32; ++b) tma_load_2d(a_dst + b * MN_BOX_BYTES, &map_a, full_bar(s), m0 + 32 * b, kc);
-#pragma unroll
-                        for (int b = 0; b < BN / 32; ++b) tma_load_2d(b_dst + b * MN_BOX_BYTES, &map_b, full_bar(s), n0 + 32 * b, kc);
-                    }
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && cta == 0) {
-            // instruction descriptor: D f32, A/B tf32, M = 256 (two CTAs), N = 256
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((kMN ? 1u : 0u) << 15) | ((kMN ? 1u : 0u) << 16) |
-                                   ((uint32_t)(BNP >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);
-            const uint32_t lbo = kMN ? (uint32_t)MN_BOX_BYTES : 0u, sbo = kMN ? 512u : 1024u, lay = kMN ? 1u : 2u;
-            const uint32_t kstep = kMN ? 1024u : (uint32_t)(UMMA_K * 4);
-            uint32_t g = 0, it = 0;
-            for (int w = pair; w < total_work; w += n_pairs, ++it) {
-                BNS_TC_PAIR_ITEM(w)
-                (void)m_t; (void)n_t; (void)kb0;
-                mbar_wait(acc_empty_bar, (it & 1u) ^ 1u);
-                tc_fence_after();
-                for (int i = 0; i < nkb; ++i, ++g) {
-                    const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
-                    mbar_wait(split_bar(s), ph);
-                    tc_fence_after();
-                    const uint32_t a_hi = base + s * STAGE_BYTES, b_hi = a_hi + A_BYTES;
-                    const uint32_t a_lo = a_hi + RAW_BYTES, b_lo = a_lo + A_BYTES;
-                    const uint32_t d = tmem_base + (uint32_t)(i % kAcc) * BNP;
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k) {
-                        const uint64_t dah = smem_desc(a_hi + k * kstep, lbo, sbo, lay), dbh = smem_desc(b_hi + k * kstep, lbo, sbo, lay);
-                        const uint64_t dal = smem_desc(a_lo + k * kstep, lbo, sbo, lay), dbl = smem_desc(b_lo + k * kstep, lbo, sbo, lay);
-                        umma_tf32_pair(d, dal, dbh, idesc, (i >= kAcc || k != 0) ? 1u : 0u);
-                        umma_tf32_pair(d, dah, dbl, idesc, 1u);
-                        umma_tf32_pair(d, dah, dbh, idesc, 1u);
-                    }
-                    umma_commit_pair(empty_bar(s));
-                }
-                umma_commit_pair(acc_full_bar);
-            }
-        }
-    } else if (warp < 2 + kSplitThreads / 32) {
-        const int t = threadIdx.x - 64;
-        uint32_t g = 0;
-        for (int w = pair; w < total_work; w += n_pairs) {
-            BNS_TC_PAIR_ITEM(w)
-            (void)m_t; (void)n_t; (void)kb0;
-            for (int i = 0; i < nkb; ++i, ++g) {
-                const uint32_t s = g % kStages, ph = (g / kStages) & 1u;
-                mbar_wait(full_bar(s), ph);
-                const float4 *raw = reinterpret_cast<const float4 *>(base_ptr + s * STAGE_BYTES);
-                float4 *lo = reinterpret_cast<float4 *>(base_ptr + s * STAGE_BYTES + RAW_BYTES);
-#pragma unroll 4
-                for (int j = 0; j < RAW_BYTES / 16 / kSplitThreads; ++j) {
-                    const int idx = t + j * kSplitThreads;
-                    const float4 x = raw[idx];
-                    float4 l;
-                    l.x = x.x - __uint_as_float(__float_as_uint(x.x) & 0xffffe000u);
-                    l.y = x.y - __uint_as_float(__float_as_uint(x.y) & 0xffffe000u);
-                    l.z = x.z - __uint_as_float(__float_as_uint(x.z) & 0xffffe000u);
-                    l.w = x.w - __uint_as_float(__float_as_uint(x.w) & 0xffffe000u);
-                    lo[idx] = l;
-                }
-                asm volatile("fence.proxy.async;" ::: "memory");     // visible to the (leader-issued) MMA's reads of THIS CTA's smem
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(split_bar(s), 0);
-            }
-        }
-    } else {
-        const uint32_t q = warp & 3u;
-        uint32_t it = 0;
-        for (int w = pair; w < total_work; w += n_pairs, ++it) {
-            BNS_TC_PAIR_ITEM(w)
-            (void)kb0;
-            mbar_wait(acc_full_bar, it & 1u);
-            tc_fence_after();
-            const int nacc = nkb < kAcc ? nkb : kAcc;
-            const int row = m_t * 2 * BM + (int)cta * BM + (int)(32 * q + lane);
-            float *Cout = C + (int64_t)split_ * split_stride + (int64_t)row * ldc;
-            const float *Add = addend ? addend + (int64_t)row * ldadd : nullptr;
-            const float rsc = (row_scale && row < M) ? __ldg(row_scale + row) : 1.f;
-            const uint32_t tbase = tmem_base + ((32u * q) << 16);
-#pragma unroll 1
-            for (int c = 0; c < BNP / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld32(tbase + (uint32_t)(c * 32), v);
-                for (int a = 1; a < nacc; ++a) {
-                    uint32_t u[32];
-                    tmem_ld32(tbase + (uint32_t)(a * BNP + c * 32), u);
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) v[e] = __float_as_uint(__uint_as_float(v[e]) + __uint_as_float(u[e]));
-                }
-                const int col0 = n_t * BNP + c * 32;
-                if (row < M) {
-#pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const int col = col0 + 4 * j;
-                        if (col + 3 < N) {
-                            float4 o = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                                   __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                            if (bias) {
-                                const float4 bb = __ldg(reinterpret_cast<const float4 *>(bias + col));
-                                o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-                            }
-                            if (Add) {
-                                const float4 aa = *reinterpret_cast<const float4 *>(Add + col);
-                                o.x += aa.x; o.y += aa.y; o.z += aa.z; o.w += aa.w;
-                            }
-                            if (row_scale) { o.x *= rsc; o.y *= rsc; o.z *= rsc; o.w *= rsc; }
-                            *reinterpret_cast<float4 *>(Cout + col) = o;
-                        } else {
-                            for (int e = 0; e < 4; ++e)
-                                if (col + e < N)
-                                    Cout[col + e] = (__uint_as_float(v[4 * j + e]) + (bias ? bias[col + e] : 0.f) + (Add ? Add[col + e] : 0.f)) * rsc;
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(acc_empty_bar, 0);
-        }
-    }
-#undef BNS_TC_PAIR_ITEM
-
-    tc_fence_before();
-    cluster_sync_all();              // nobody frees TMEM / leaves while the peer's tensor core may still read its smem
-    if (warp == 1) {
-        __syncwarp();
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-    }
-}
-
-inline bool pair_mode() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("BNS_TC_PAIR");
-        v = (e && e[0] == '1') ? 1 : 0;
-    }
-    return v == 1;
 }
 
 // out[r, c] = sum_s ws[s][r, c]  in split order (deterministic); ws slices are contiguous [rows, cols]
@@ -651,7 +347,7 @@ inline EncodeTiledFn encode_tiled() {
 // 2-D f32 tensor map over a row-major [rows, inner] matrix with leading dimension ld (floats), SWIZZLE_128B,
 // out-of-bounds elements read as zero.
 inline int make_map(CUtensorMap *m, const float *ptr, int64_t inner, int64_t rows, int64_t ld, uint32_t box_inner,
-                    uint32_t box_rows, bool atom32 = false) {
+                    uint32_t box_rows) {
     EncodeTiledFn enc = encode_tiled();
     if (!enc) return fail(BNS_E_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
     cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)rows};
@@ -659,8 +355,7 @@ inline int make_map(CUtensorMap *m, const float *ptr, int64_t inner, int64_t row
     cuuint32_t box[2] = {box_inner, box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(ptr), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(BNS_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
     return BNS_OK;
@@ -668,21 +363,12 @@ inline int make_map(CUtensorMap *m, const float *ptr, int64_t inner, int64_t row
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-inline bool trunc_mode() {
-    static int v = -1;
-    if (v < 0) {
-        const char *e = getenv("BNS_TC_TRUNC");
-        v = (e && e[0] == '0') ? 0 : 1;
-    }
-    return v == 1;
-}
-
-template <bool kMN, bool kTrunc>
+template <bool kMN>
 int configure() {
     static std::atomic<int> done[kMaxDevices];      // the attribute is per function AND per device
     const int dev = current_device();
     if (!done[dev].load(std::memory_order_acquire)) {
-        BNS_CUDA(cudaFuncSetAttribute(gemm3x_kernel<kMN, kTrunc>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        BNS_CUDA(cudaFuncSetAttribute(gemm3x_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         done[dev].store(1, std::memory_order_release);
     }
     return BNS_OK;
@@ -705,37 +391,16 @@ extern "C" int bns_dense_tn_3xtf32(const float *A, int64_t lda, const float *B, 
     if (rc) return rc;
     rc = tc::make_map(&mb, B, K, N, ldb, tc::BK, tc::BN);
     if (rc) return rc;
-    const bool tr = tc::trunc_mode();
-    rc = tr ? tc::configure<false, true>() : tc::configure<false, false>();
+    rc = tc::configure<false>();
     if (rc) return rc;
     const int tiles_m = (int)((M + tc::BM - 1) / tc::BM), tiles_n = (int)((N + tc::BN - 1) / tc::BN);
     const int num_kb = (int)((K + tc::BK - 1) / tc::BK);
-    if (tc::pair_mode() && N >= 192) {      // DRAFT path (cta_group::2), see gemm3x_pair_kernel
-        static std::atomic<int> cfg_done[kMaxDevices];
-        const int dev = current_device();
-        if (!cfg_done[dev].load(std::memory_order_acquire)) {
-            BNS_CUDA(cudaFuncSetAttribute(tc::gemm3x_pair_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
-            cfg_done[dev].store(1, std::memory_order_release);
-        }
-        const int ptm = (int)((M + 2 * tc::BM - 1) / (2 * tc::BM)), ptn = (int)((N + tc::BNP - 1) / tc::BNP);
-        const int ptiles = ptm * ptn, max_pairs = sm_count() / 2;
-        dim3 pgrid((unsigned)(2 * (ptiles < max_pairs ? ptiles : max_pairs)), 1, 1);
-        tc::gemm3x_pair_kernel<false><<<pgrid, tc::kThreadsTc, tc::SMEM_BYTES, as_stream(stream)>>>(
-            ma, mb, C, ldc, 0, bias, addend, ldadd, row_scale, (int)M, (int)N, num_kb, ptn, ptiles, 1);
-        ++g_launches;
-        BNS_CUDA(cudaGetLastError());
-        return BNS_OK;
-    }
     const int64_t tiles64 = tiles_m * (int64_t)tiles_n;
     BNS_REQUIRE(tiles64 < (1ll << 31), "bns_dense_tn_3xtf32: too many tiles");
     const int tiles = (int)tiles64;
     dim3 grid((unsigned)(tiles < sm_count() ? tiles : sm_count()), 1, 1);
-    if (tr)
-        tc::gemm3x_kernel<false, true><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
-                                                                                                   row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
-    else
-        tc::gemm3x_kernel<false, false><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
-                                                                                                    row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
+    tc::gemm3x_kernel<false><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
+                                                                                        row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -786,12 +451,11 @@ extern "C" int bns_dense_nt_3xtf32(const float *A, int64_t lda, const float *B, 
     if (need > ws_bytes || (need && (!ws || !tc::aligned16(ws))))
         return fail(BNS_E_WORKSPACE, "bns_dense_nt_3xtf32: workspace %zu < %zu bytes", ws_bytes, need);
     CUtensorMap ma, mb;
-    int rc = tc::make_map(&ma, A, N1, R, lda, 32, tc::BK, true);
+    int rc = tc::make_map(&ma, A, N1, R, lda, 32, tc::BK);
     if (rc) return rc;
-    rc = tc::make_map(&mb, B, N2, R, ldb, 32, tc::BK, true);
+    rc = tc::make_map(&mb, B, N2, R, ldb, 32, tc::BK);
     if (rc) return rc;
-    const bool tr = tc::trunc_mode();
-    rc = tr ? tc::configure<true, true>() : tc::configure<true, false>();
+    rc = tc::configure<true>();
     if (rc) return rc;
     const int tiles_m = (int)((N1 + tc::BM - 1) / tc::BM), tiles_n = (int)((N2 + tc::BN - 1) / tc::BN);
     const int num_kb = (int)((R + tc::BK - 1) / tc::BK);
@@ -802,12 +466,8 @@ extern "C" int bns_dense_nt_3xtf32(const float *A, int64_t lda, const float *B, 
     cudaStream_t st = as_stream(stream);
     float *w = splits == 1 ? C : static_cast<float *>(ws);
     const int64_t ldw = splits == 1 ? ldc : N2, slice = splits == 1 ? 0 : N1 * N2;
-    if (tr)
-        tc::gemm3x_kernel<true, true><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
-                                                                                    (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
-    else
-        tc::gemm3x_kernel<true, false><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
-                                                                                     (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
+    tc::gemm3x_kernel<true><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
+                                                                         (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
     if (splits == 1) {
         ++g_launches;
     } else {

@@ -4,7 +4,7 @@
 // per-entry algebra with ~25 ATen launches over [nnz, heads] temporaries and one SpMM launch per head.  Here, two forms
 // of the same algebra (same Philox mask, tests compare them):
 //
-// (A) staged -- what graph.GatAttention runs (profiles/gat_r02.md: 2-3x faster on low-degree graphs)
+// (A) staged -- what graph.GatAttention runs (faster on low-degree graphs)
 //   gat_proj_kernel / gat_proj_bwd_kernel   el = <ft, attn_l>, er = <ft, attn_r> per head and their backward
 //   gat_scores_kernel        one warp per destination row, scalars only: score -> online max / sum -> probability P and
 //                            dropped attention a' per entry (a' of the halo entries also at their compacted positions)
@@ -344,7 +344,7 @@ _Pragma("unroll")
 
 // ---- the decomposed form: scalar row walks + the tuned SpMM / SDDMM kernels for everything F-wide --------------------
 // The fused row-walk kernels above keep ONE row's dependent loads in flight per warp; on a low-degree graph (Yelp shape,
-// ~20 entries per row) that is a latency chain per row and 2-9 ms per launch (profiles/gat_r02.md).  The same algebra
+// ~20 entries per row) that is a latency chain per row.  The same algebra
 // as: scores kernel (scalars only) -> weighted SpMM (spmm_kernel, 8 gathers in flight per lane) in forward, and
 // SDDMM -> softmax/leaky backward (scalars only) -> column sums -> weighted transposed SpMM in backward.
 

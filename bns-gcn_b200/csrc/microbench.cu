@@ -3,14 +3,14 @@
 // VERDICT r1, weak #2: "the claim 'at the L2->SM ceiling' rests on the same kernel run on a 51 MB matrix -- a
 // self-referential ceiling".  These kernels share no code with spmm_kernel: no CSR, no index loads, no shared memory.
 //
-//   bnsm_stream_read   every thread streams 16-byte loads over a buffer of `bytes` (L2-resident when it fits the 126 MB
-//                      L2 and was touched before; HBM otherwise), `reps` passes inside ONE launch.
+//   bnsm_stream_read   every thread streams 16-byte loads over a buffer of `bytes` (L2-resident when it fits the L2
+//                      and was touched before; HBM otherwise), `reps` passes inside ONE launch.
 //   bnsm_row_gather    every warp gathers pseudo-random rows of `row_bytes` (512 / 1024: the slab rows of the SpMM) from
 //                      a table of `n_rows` rows, UNROLL independent 16-byte loads in flight per lane, ids from an
 //                      in-register LCG (no index stream).  This is the access pattern of the SpMM stripped of everything
 //                      else: its GB/s is the fabric ceiling for "random 512-byte-row gather".
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 --shared -Xcompiler -fPIC -o libbnsmicro.so microbench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --shared -Xcompiler -fPIC -o libbnsmicro.so microbench.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
@@ -86,7 +86,7 @@ __global__ void fill_kernel(float4 *buf, int64_t n4) {
 }
 
 int sms() {
-    int dev = 0, n = 148;
+    int dev = 0, n = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
     return n;

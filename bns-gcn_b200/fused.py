@@ -479,7 +479,7 @@ class GcnConvFn(torch.autograd.Function):
 
 
 def sage_layer_eligible(layer, feat: torch.Tensor) -> bool:
-    """Shapes the tcgen05 kernels take on every GEMM of the fused layer."""
+    """Shapes the wgmma kernels take on every GEMM of the fused layer."""
     lin = layer.linear if layer.use_pp else layer.linear1
     k = lin.in_features
     return (feat.is_cuda and feat.dtype == torch.float32 and feat.dim() == 2 and feat.stride(1) == 1 and k % 4 == 0

@@ -240,7 +240,7 @@ class GatAttention(torch.autograd.Function):
     ``bns_spmm_weighted_f32`` / ``bns_spmm_compact_f32`` per head; backward ``bns_sddmm_dot_f32`` ->
     ``bns_gat_softmax_bwd_f32`` -> ``bns_gat_colsum_f32`` -> ``bns_spmm_weighted_f32`` on the transposes.  The one-launch
     row walks ``bns_gat_forward_f32`` / ``bns_gat_backward_f32`` compute the same thing (``BNS_GAT_ROWWALK=1``; the
-    tests run both) but are a latency chain per row on low-degree graphs: profiles/gat_r02.md."""
+    tests run both) but are a latency chain per row on low-degree graphs."""
 
     @staticmethod
     def forward(ctx, ft, el, er, g: PartitionGraph, H: int, Fo: int, slope: float, p: float, seed: int):

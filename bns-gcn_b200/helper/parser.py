@@ -45,7 +45,7 @@ def _spellings(flag: str):
 
 
 def build_parser():
-    parser = argparse.ArgumentParser(description='BNS-GCN (B200-native hot path)')
+    parser = argparse.ArgumentParser(description='BNS-GCN (H100-native hot path)')
     for flag, kind, default, extra in _REFERENCE_FLAGS:
         if kind == "switch":
             parser.add_argument(*_spellings(flag), action='store_true')

@@ -1,19 +1,18 @@
 """Dense layers of the path (K8, module/layer.py:30, 38, 83, 92 of the reference are plain ``nn.Linear`` in fp32).
 
-The reference runs them as true-fp32 cuBLAS SGEMMs (torch 1.12: ``allow_tf32=False`` for matmul).  On B200 the fp32
-SIMT pipe gives ~45-60 TFLOP/s -- after the SpMM work the largest share of the epoch -- while one TF32 tensor-core
+The reference runs them as true-fp32 cuBLAS SGEMMs (torch 1.12: ``allow_tf32=False`` for matmul).  The fp32
+SIMT pipe (67 TFLOP/s on the H100 SXM data sheet) is far below the tensor cores, while one TF32 tensor-core
 pass would miss the 1e-4 parity bar (10-bit mantissa).  ``linear()`` therefore uses the error-compensated **3xTF32**
 scheme: split every f32 operand into ``hi = tf32(x)`` and ``lo = x - hi`` (exact in f32) and accumulate
 ``hi*hi + hi*lo + lo*hi`` on the tensor cores with f32 accumulation; the dropped ``lo*lo`` term is 2^-22 relative.
 
-``MODE`` (env BNS_DENSE): "tc" (default) -- the hand-written tcgen05 kernels of csrc/dense_tc.cuh: 3xTF32 with the
-operand split fused into the TMA -> shared memory -> TMEM pipeline (forward, input gradient, split-K weight gradient);
+``MODE`` (env BNS_DENSE): "tc" (default) -- the hand-written wgmma kernels of csrc/dense_tc.cuh: 3xTF32 with the
+operand split fused into the TMA -> shared memory -> wgmma pipeline (forward, input gradient, split-K weight gradient);
 operands whose rows are not 16-byte multiples fall back to fp32 cuBLAS | "fp32" (cuBLAS SIMT, the literal reference
 precision) | "auto" (library-composed 3xtf32 where K >= 512) | "3xtf32" | "bf16x3".
-B200, M=232,965 K=1204 N=256 (tools/check_dense_tc.py perf): fp32 cuBLAS 2.37 ms fwd / 3.15 ms dW; tc 0.95 / 0.97 ms
-with max error 2.7e-6 / 3.5e-6 of max|C| against f64 (cuBLAS fp32: 1.9e-6 / 1.5e-6).  History: the library-composed
-3xtf32 (three cuBLAS TF32 GEMMs + a split pass) was slower than fp32 cuBLAS except at K >= 512, bf16x3 always slower
-(profiles/bench_n1_r01_*_negative_result.json).
+``tools/check_dense_tc.py perf`` times the Reddit-shape layer GEMMs against cuBLAS.  On the previous GPU the
+library-composed 3xtf32 (three cuBLAS TF32 GEMMs + a split pass) was slower than fp32 cuBLAS except at K >= 512, and
+bf16x3 always slower.
 """
 import os
 
@@ -28,7 +27,7 @@ import threading
 _GEMM_LOCK = threading.RLock()
 
 MODE = os.environ.get("BNS_DENSE", "tc")
-# bench.py sets this to a list to collect (start_event, end_event, useful_flops, algorithmic_bytes) per tcgen05 GEMM
+# bench.py sets this to a list to collect (start_event, end_event, useful_flops, algorithmic_bytes) per wgmma GEMM
 PROFILE = None
 MIN_K_3X = 512       # "auto": 3xTF32 only where the GEMM is big enough to repay the split pass (layer 0: K = 2 * n_feat)
 
@@ -157,14 +156,14 @@ class _LinearFp32(torch.autograd.Function):
         return dx, dw, db
 
 
-# ---- "tc": hand-written tcgen05 kernels (csrc/dense_tc.cuh), 3xTF32 with the split fused into the pipeline ---------
+# ---- "tc": hand-written wgmma kernels (csrc/dense_tc.cuh), 3xTF32 with the split fused into the pipeline ---------
 def _tc_operand(t: torch.Tensor) -> bool:
     return (t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.stride(1) == 1 and t.stride(0) % 4 == 0
             and t.stride(0) >= t.shape[1] and t.data_ptr() % 16 == 0 and t.shape[0] > 0 and t.shape[1] > 0)
 
 
 def tc_eligible(x: torch.Tensor, weight: torch.Tensor, bias=None) -> bool:
-    """Shapes the tcgen05 kernels take: 16-byte aligned rows everywhere the forward AND both gradients touch."""
+    """Shapes the wgmma kernels take: 16-byte aligned rows everywhere the forward AND both gradients touch."""
     return (_tc_operand(x) and _tc_operand(weight) and x.shape[1] == weight.shape[1] and weight.shape[0] % 4 == 0
             and weight.shape[1] % 4 == 0
             and (bias is None or (bias.is_cuda and bias.dtype == torch.float32 and bias.is_contiguous()

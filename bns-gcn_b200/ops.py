@@ -167,12 +167,10 @@ def spmm(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *,
 
 
 # ---- source-row blocking ------------------------------------------------------------------------------------------
-# B200's 126 MB L2 is two ~63 MB halves; a gather table shared by all SMs stops being resident well before 126 MB:
-# random 512-byte-row gathers run at 19.8 TB/s from a 49 MB table, 16.7 TB/s from 114 MB, 11 TB/s from 228 MB
-# (profiles/l2_microbench_r02.md).  Column slabs (csrc: pick_slab) bring the Reddit-shape table down to 119 MB; cutting
-# the SOURCE ROWS in two as well makes every pass gather from <= 60 MB: 7.39 -> 6.63 ms per F = 256 launch
-# (profiles/spmm_colblocks_r02.txt).  Only worth it where rows are re-read often (high average degree) and few blocks
-# suffice -- each extra block costs one read-modify-write of the output.
+# Column slabs (csrc: pick_slab) cut the gather table by columns; cutting the SOURCE ROWS into blocks as well makes
+# every pass gather from a smaller table, so more of it stays in L2.  Only worth it where rows are re-read often (high
+# average degree) and few blocks suffice -- each extra block costs one read-modify-write of the output.  On an H100 SXM
+# (700 W) the Reddit-shape F = 256 launch takes 9.4 ms with two blocks of <= 60 MB and 15.5 ms unblocked.
 BLOCK_TABLE_BYTES = 60 << 20
 BLOCK_MIN_AVG_DEGREE = 64
 BLOCK_MAX = 4

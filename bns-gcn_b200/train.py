@@ -524,7 +524,7 @@ class GraphedEpoch:
     """One whole training epoch -- boundary sampling, id exchange, slot-map refresh, forward (feature exchange on
     the comm stream + SpMM + dense), loss, backward (SpMM^T + gradient exchange), weight-gradient all-reduce, Adam --
     captured ONCE into a CUDA graph and replayed.  At 4-8 partitions of the Reddit-shape graph the eager epoch is
-    bound by the ~10 ms the host needs to enqueue ~300 launches (profiles/kineto_n4_r01.txt); a replay costs one.
+    bound by the time the host needs to enqueue ~300 launches; a replay costs one.
 
     What changes between replays is read from device memory, not baked into kernel arguments: the Philox offset of
     the sampler and the flag sequence number of the p2p exchange both come from ``st.epoch_dev``; dropout uses
@@ -547,7 +547,7 @@ class GraphedEpoch:
         torch.cuda.synchronize(dev)
         buf, red = ctx.buffer._get(), ctx.reducer._get()
         if _rank_size()[1] > 2 and getattr(buf, "_backend", None) == 'nccl':
-            # Measured (tools/dist_check.py --graph, 4 x B200): the staged transport replayed from a graph is correct at
+            # Measured (tools/dist_check.py --graph, 4 GPUs): the staged transport replayed from a graph is correct at
             # 2 ranks and WRONG at 4 (its NCCL send/recv batches sit on three streams of the captured graph); the
             # peer-mapped transport -- the default, flags in peer memory -- is bit-identical to the eager run at 2/4/8.
             raise NotImplementedError("GraphedEpoch with more than 2 partitions needs --backend p2p (the staged NCCL "

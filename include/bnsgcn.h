@@ -1,5 +1,5 @@
 /*
- * bnsgcn.h -- C ABI of libbnsgcn.so: the B200 (sm_100a) replacement for the device work the
+ * bnsgcn.h -- C ABI of libbnsgcn.so: the H100 (sm_90a) replacement for the device work the
  * BNS-GCN hot path reaches through DGL / ATen / numpy (SURVEY.md §2.3 K1-K7, §8b).
  *
  * The reference (GATECH-EIC/BNS-GCN, 100 % Python) has no FFI layer of its own: its "operator API"
@@ -121,9 +121,9 @@ int bns_split_tf32_f32(const float *x, int64_t n, float *hi, float *lo, void *st
 /* ------------------------------------------------------------------------------------------------
  * K8: the dense layers themselves.  Replaces, for 2-D f32 operands,
  *     self.linear(feat) / self.linear1(feat) + self.linear2(ah)      module/layer.py:30, 38, 83, 92  (forward)
- * and what autograd runs for them (grad_input = dY W, grad_weight = dY^T X) with hand-written tcgen05 kernels:
- * kind::tf32 MMAs accumulating in TMEM, operands staged by TMA (SWIZZLE_128B), and the 3xTF32 operand split
- * (hi = tf32(x), lo = x - hi; hi*hi + hi*lo + lo*hi) done in shared memory inside the pipeline, so the result is
+ * and what autograd runs for them (grad_input = dY W, grad_weight = dY^T X) with hand-written wgmma kernels:
+ * .tf32 wgmma.mma_async accumulating in registers, operands staged by TMA (SWIZZLE_128B), and the 3xTF32 operand split
+ * (hi = x truncated to tf32, lo = x - hi; hi*hi + hi*lo + lo*hi) done in shared memory inside the pipeline, so the result is
  * f32-accurate (~2^-21 relative per product) while every operand byte crosses HBM/L2 once (csrc/dense_tc.cuh).
  *
  * bns_dense_tn_3xtf32:  C[M, N] = A[M, K] * B[N, K]^T (+ bias[N]) (+ addend[M, N]);  A, B, C row-major with leading

@@ -52,6 +52,8 @@ def run_product(parts, args, device, n_epochs, selected_per_epoch=None, capture=
 
                 def pre(m, inp, i=i):
                     h = inp[1] if len(inp) > 1 else inp[0]
+                    if isinstance(h, tuple):        # GATConv takes (src, dst): dst holds the inner rows
+                        h = h[1]
                     cur_masks[i - 1] = (h[:n_in] > 0).detach().cpu()
                 hooks.append(layer.register_forward_pre_hook(pre))
         for e in range(n_epochs):

@@ -1,4 +1,4 @@
-"""K8 on tcgen05 (csrc/dense_tc.cuh): bns_dense_tn_3xtf32 / bns_dense_nt_3xtf32 against an f64 torch reference.
+"""K8 on wgmma (csrc/dense_tc.cuh): bns_dense_tn_3xtf32 / bns_dense_nt_3xtf32 against an f64 torch reference.
 
 Tolerance: 2e-5 of max|C| (cuBLAS fp32 itself sits at ~2e-6 on these shapes; one TF32 pass would be ~5e-4)."""
 import pytest

@@ -199,7 +199,7 @@ def test_per_rank_generator_partitions_agree_gloo(tmp_path):
 
 
 def test_dense_split_k_plan_is_sane_without_a_gpu(built):
-    """``bns_dense_nt_workspace_bytes`` is pure host arithmetic (SM count falls back to 148 without a device): the
+    """``bns_dense_nt_workspace_bytes`` is pure host arithmetic (SM count falls back to 132, the H100 SXM's, without a device): the
     weight-gradient contraction is cut into slices of at most 48 k-blocks of 32 rows (accumulation-chain bound,
     csrc/dense_tc.cuh), never more slices than k-blocks, and no workspace when one slice suffices."""
     from bns_gcn_b200 import _lib
@@ -212,7 +212,7 @@ def test_dense_split_k_plan_is_sane_without_a_gpu(built):
         kb = (R + 31) // 32
         assert 1 <= splits <= kb
         assert (kb + splits - 1) // splits <= 48 + 5, (R, n1, n2, splits)      # <= 48 up to the -10 % wave rounding
-    assert _lib.lib.bns_colsum_workspace_bytes(256) == 148 * 4 * 64 * 16
+    assert _lib.lib.bns_colsum_workspace_bytes(256) == 132 * 4 * 64 * 16
 
 
 def _planted_partition_graph(n, P, deg_in, deg_out, seed=0):

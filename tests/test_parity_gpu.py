@@ -352,9 +352,16 @@ def test_cuda_gat_reproduces_the_reference_golden(built):
     processes, 2 heads, with dgl.nn.GATConv supplied as a DENSE masked-softmax restatement of DGL 0.9's layer.  The
     CUDA path (entry-list kernels; the 5-class output layer takes the op-by-op path), fed the index sets the reference
     drew, reproduces its stored halo features, head-averaged layer outputs, logits, reduced gradients and updated
-    weights within 1e-4 and its boundary sets exactly.  (Kept last in this file: new in round 2's final hours.)"""
+    weights within 1e-4 and its boundary sets exactly.
+
+    ReLU kinks: in the last epoch one inter-layer pre-activation of this configuration sits 2.6e-7 from zero, so a
+    forward that rounds differently may take the other side and move the gradients by ~1e-3 although it is right.
+    As in tests/harness.py, gradient parity is then defined on a common active set: the CUDA path records its ReLU
+    active sets, the oracle (pinned to this same fixture by tests/test_oracle_cpu.py) reruns on exactly those, every
+    switched entry must lie within KINK_MARGIN of zero, and gradients and updated weights must match that run within
+    1e-4.  Halo features, layer outputs, logits and boundary sets are always compared with the fixture itself."""
     import os
-    from tests.harness import make_args, run_product, _relerr
+    from tests.harness import KINK_MARGIN, _compare, make_args, run_oracle, run_product, _relerr
     from bns_gcn_b200.data import make_graph, partition_graph
     gold = torch.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_gat_p2.pt"))
     cfg, ranks = gold["config"], gold["ranks"]
@@ -378,4 +385,12 @@ def test_cuda_gat_reproduces_the_reference_golden(built):
             errs[f"r{r}/param/{g['param_names'][k]}"] = _relerr(p, gp)
             errs[f"r{r}/grad/{g['param_names'][k]}"] = _relerr(o["grads"][k], gg)
     bad = {k: v for k, v in errs.items() if v >= TOL}
+    if bad and all("/grad/" in k or "/param/" in k for k in bad):
+        prod = run_product(parts, args, "cuda:0", cfg["epochs"], selected_per_epoch=sel, capture_masks=True)
+        masks = [[prod[r]["relu_masks"][e] for r in range(cfg["n_parts"])] for e in range(cfg["epochs"])]
+        orc = run_oracle(parts, args, cfg["epochs"], sel, relu_masks_per_epoch=masks)
+        flips, max_z = sum(o["kink"]["flips"] for o in orc), max(o["kink"]["max_abs_z"] for o in orc)
+        assert 0 < flips and max_z < KINK_MARGIN, (sorted(bad.items()), flips, max_z)
+        worst, detail = _compare(prod, orc, cfg["n_parts"])
+        bad = {k: v for k, v in detail.items() if v >= TOL}
     assert not bad, sorted(bad.items())

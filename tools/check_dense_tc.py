@@ -1,4 +1,4 @@
-"""Bring-up / diagnosis of the tcgen05 dense kernels (csrc/dense_tc.cuh).
+"""Bring-up / diagnosis of the wgmma dense kernels (csrc/dense_tc.cuh).
 
   python tools/check_dense_tc.py tn     structured + random checks of bns_dense_tn_3xtf32
   python tools/check_dense_tc.py nt     structured + random checks of bns_dense_nt_3xtf32

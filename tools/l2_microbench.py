@@ -1,7 +1,7 @@
 """Independent L2 / HBM bandwidth probes (csrc/microbench.cu -> libbnsmicro.so): the ceilings the SpMM's gather rate is
-compared with in profiles/.  No code shared with spmm_kernel.
+compared with.  No code shared with spmm_kernel.
 
-    python tools/l2_microbench.py [--out profiles/l2_microbench_r02.md]
+    python tools/l2_microbench.py [--out FILE.md]
 """
 import argparse
 import ctypes
@@ -21,7 +21,9 @@ def main():
     lib.bnsm_stream_read.argtypes = [ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int]
     lib.bnsm_row_gather.restype = ctypes.c_double
     lib.bnsm_row_gather.argtypes = [ctypes.c_int64, ctypes.c_int, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int]
-    lines = ["# L2 / HBM microbenchmarks (B200, CUDA events, best of 5 launches after 2 warm-up launches)", "",
+    import torch
+    gpu = torch.cuda.get_device_name(0)
+    lines = [f"# L2 / HBM microbenchmarks ({gpu}, CUDA events, best of 5 launches after 2 warm-up launches)", "",
              "## Streaming 16-byte reads (`ld.global.nc.L1::no_allocate.v4`), whole grid, 8 loads in flight per thread", "",
              "| buffer | passes per launch | CTAs/SM | GB/s |", "|---:|---:|---:|---:|"]
     for mb, reps in ((16, 64), (32, 32), (64, 16), (96, 12), (119, 8), (256, 4), (1024, 2), (4096, 1)):
