@@ -498,6 +498,147 @@ __global__ void __launch_bounds__(kThreads) gat_colsum_kernel(const int64_t *__r
     }
 }
 
+// ---- the evaluation forward on a homogeneous graph (DGL 0.9 GATConv, no dropout, no backward) ----------------------
+//   rst[v, h, :] = sum_{u -> v} softmax_u(leaky_relu(el[u, h] + er[v, h])) * ft[u, h, :] + bias[h, :]
+// ONE pass over each row, nothing stored per entry: the row's entries are taken 32 at a time; per head, the block's
+// maximum score is reduced across the warp, and when the running maximum grows the accumulator and the per-lane sums of
+// exp are rescaled by exp(m_old - m_new) (online softmax).  The block's source ids and weights are staged in shared
+// memory and the gathered ft rows accumulated as in gat_fwd_kernel.  Every sum runs in an order fixed per row, so two
+// launches on the same inputs give bit-identical results.
+struct GatInferArgs {
+    const int64_t *indptr; const int32_t *indices; int64_t n_rows;
+    const float *ft; int64_t ldft; int32_t H, Fp;          // ft [n_cols, H, Fp]: Fp = per-head width padded to 4
+    const float *el, *er, *bias;                           // [n_cols, H], [n_rows, H], [H * Fp] or NULL
+    float slope;
+    float *rst; int64_t ldr;                               // [n_rows, H, Fp]
+};
+
+template <int NV>
+__global__ void __launch_bounds__(kThreads) gat_infer_kernel(GatInferArgs a) {
+    __shared__ int32_t s_u[kWarps][32];
+    __shared__ float s_w[kWarps][32][kGatMaxHeads];
+    __shared__ float s_h[kWarps][kGatMaxHeads];           // per-head rescale factors, then the row's sums of exp
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    const int H = a.H, F = a.H * a.Fp;
+    int hd[NV];                                   // head that owns each float4 column group of this lane
+#pragma unroll
+    for (int t = 0; t < NV; ++t) {
+        const int c = (lane + 32 * t) * 4;
+        hd[t] = c < F ? c / a.Fp : 0;
+    }
+    constexpr int U = NV <= 2 ? 4 : (NV == 4 ? 2 : 1);            // entries whose row gathers are in flight together
+    for (int64_t v = (int64_t)blockIdx.x * kWarps + w; v < a.n_rows; v += warps_total) {
+        float erv[kGatMaxHeads], m[kGatMaxHeads], l[kGatMaxHeads];   // m: running max (warp-uniform); l: this lane's sum
+#pragma unroll
+        for (int h = 0; h < kGatMaxHeads; ++h) {
+            erv[h] = h < H ? a.er[v * H + h] : 0.f;
+            m[h] = -INFINITY;
+            l[h] = 0.f;
+        }
+        float4 acc[NV];
+#pragma unroll
+        for (int t = 0; t < NV; ++t) acc[t] = make_float4(0.f, 0.f, 0.f, 0.f);
+        const int64_t b = a.indptr[v], e = a.indptr[v + 1];
+        for (int64_t k0 = b; k0 < e; k0 += 32) {
+            const int64_t k = k0 + lane;
+            const bool valid = k < e;
+            const int32_t u = valid ? __ldg(a.indices + k) : 0;
+            const int cnt = (int)((e - k0) < 32 ? (e - k0) : 32);
+            float f[kGatMaxHeads];                // exp(m_old - m_new) per head
+#pragma unroll
+            for (int h = 0; h < kGatMaxHeads; ++h) {
+                f[h] = 1.f;
+                if (h < H) {
+                    const float sc = valid ? leaky(__ldg(a.el + (int64_t)u * H + h) + erv[h], a.slope) : -INFINITY;
+                    float mn = sc;
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) mn = fmaxf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+                    mn = fmaxf(mn, m[h]);
+                    if (mn != -INFINITY) {
+                        f[h] = expf(m[h] - mn);   // 0 on the first block, 1 while the maximum does not grow
+                        const float p = valid ? expf(sc - mn) : 0.f;
+                        l[h] = fmaf(l[h], f[h], p);
+                        m[h] = mn;
+                        s_w[w][lane][h] = p;
+                    } else {
+                        s_w[w][lane][h] = 0.f;
+                    }
+                }
+            }
+            s_u[w][lane] = u;
+            if (lane == 0) {                      // per-head factors through shared memory: hd[t] is a runtime index
+#pragma unroll
+                for (int h = 0; h < kGatMaxHeads; ++h) s_h[w][h] = f[h];
+            }
+            __syncwarp();
+#pragma unroll
+            for (int t = 0; t < NV; ++t) {
+                const float sf = s_h[w][hd[t]];
+                acc[t].x *= sf; acc[t].y *= sf; acc[t].z *= sf; acc[t].w *= sf;
+            }
+            int jj = 0;
+            for (; jj + U <= cnt; jj += U) {
+                float4 x[U][NV];
+#pragma unroll
+                for (int q = 0; q < U; ++q) {
+                    const float *fr = a.ft + (int64_t)s_u[w][jj + q] * a.ldft;
+#pragma unroll
+                    for (int t = 0; t < NV; ++t) {
+                        const int c = (lane + 32 * t) * 4;
+                        x[q][t] = c < F ? __ldg(reinterpret_cast<const float4 *>(fr + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < U; ++q)
+#pragma unroll
+                    for (int t = 0; t < NV; ++t) {
+                        const float wt = s_w[w][jj + q][hd[t]];
+                        acc[t].x = fmaf(x[q][t].x, wt, acc[t].x); acc[t].y = fmaf(x[q][t].y, wt, acc[t].y);
+                        acc[t].z = fmaf(x[q][t].z, wt, acc[t].z); acc[t].w = fmaf(x[q][t].w, wt, acc[t].w);
+                    }
+            }
+            for (; jj < cnt; ++jj) {
+                const float *fr = a.ft + (int64_t)s_u[w][jj] * a.ldft;
+#pragma unroll
+                for (int t = 0; t < NV; ++t) {
+                    const int c = (lane + 32 * t) * 4;
+                    if (c < F) {
+                        const float wt = s_w[w][jj][hd[t]];
+                        const float4 x = __ldg(reinterpret_cast<const float4 *>(fr + c));
+                        acc[t].x = fmaf(x.x, wt, acc[t].x); acc[t].y = fmaf(x.y, wt, acc[t].y);
+                        acc[t].z = fmaf(x.z, wt, acc[t].z); acc[t].w = fmaf(x.w, wt, acc[t].w);
+                    }
+                }
+            }
+            __syncwarp();
+        }
+#pragma unroll
+        for (int h = 0; h < kGatMaxHeads; ++h) l[h] = warp_sum(l[h]);
+        if (lane == 0) {
+#pragma unroll
+            for (int h = 0; h < kGatMaxHeads; ++h) s_h[w][h] = l[h];
+        }
+        __syncwarp();
+        float *out = a.rst + v * a.ldr;
+#pragma unroll
+        for (int t = 0; t < NV; ++t) {
+            const int c = (lane + 32 * t) * 4;
+            if (c < F) {
+                const float den = s_h[w][hd[t]];
+                float4 r = den > 0.f ? make_float4(acc[t].x / den, acc[t].y / den, acc[t].z / den, acc[t].w / den)
+                                     : make_float4(0.f, 0.f, 0.f, 0.f);          // a row without entries: bias only
+                if (a.bias) {
+                    const float4 bb = __ldg(reinterpret_cast<const float4 *>(a.bias + c));
+                    r.x += bb.x; r.y += bb.y; r.z += bb.z; r.w += bb.w;
+                }
+                *reinterpret_cast<float4 *>(out + c) = r;
+            }
+        }
+        __syncwarp();                             // s_h is rewritten by the next row
+    }
+}
+
 
 #undef BNS_GAT_FOR_EACH_ENTRY
 
@@ -638,6 +779,36 @@ extern "C" int bns_gat_colsum_f32(const bns_graph_t *gT, const float *dE, int32_
     BNS_REQUIRE(d_el && (dE || gT->nnz == 0), "bns_gat_colsum_f32: NULL pointer");
     gat_colsum_kernel<<<gat_grid(gT->n_rows), kThreads, 0, as_stream(stream)>>>(gT->indptr, gT->perm, gT->n_rows, dE, H, row_map,
                                                                                out_base, d_el);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// the evaluation forward of GATConv on a homogeneous graph: score -> online softmax -> weighted sum (+ bias), one pass
+extern "C" int bns_gat_infer_f32(const bns_graph_t *g, const float *ft, int64_t ldft, int32_t H, int32_t Fp, const float *el,
+                                 const float *er, float slope, const float *bias, float *rst, int64_t ldr, void *stream) {
+    BNS_REQUIRE(g, "bns_gat_infer_f32: NULL graph");
+    BNS_REQUIRE(H >= 1 && H <= kGatMaxHeads && Fp > 0 && Fp % 4 == 0 && (int64_t)H * Fp <= 1024,
+                "bns_gat_infer_f32: need 1 <= heads <= 8, padded width %% 4 == 0, heads * padded width <= 1024 (got %d, %d)",
+                H, Fp);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(ft && el && er && rst, "bns_gat_infer_f32: NULL pointer");
+    const int64_t HF = (int64_t)H * Fp;
+    BNS_REQUIRE(ldft % 4 == 0 && ldr % 4 == 0 && ldft >= HF && ldr >= HF &&
+                    ((reinterpret_cast<uintptr_t>(ft) | reinterpret_cast<uintptr_t>(rst) |
+                      reinterpret_cast<uintptr_t>(bias)) & 15u) == 0,
+                "bns_gat_infer_f32: 16-byte aligned rows required");
+    GatInferArgs a{};
+    a.indptr = g->indptr; a.indices = g->indices; a.n_rows = g->n_rows;
+    a.ft = ft; a.ldft = ldft; a.H = H; a.Fp = Fp; a.el = el; a.er = er; a.bias = bias; a.slope = slope;
+    a.rst = rst; a.ldr = ldr;
+    const int nv = (int)((HF + 127) / 128);
+    const unsigned grid = gat_grid(g->n_rows);
+    cudaStream_t st = as_stream(stream);
+    if (nv <= 1) gat_infer_kernel<1><<<grid, kThreads, 0, st>>>(a);
+    else if (nv == 2) gat_infer_kernel<2><<<grid, kThreads, 0, st>>>(a);
+    else if (nv <= 4) gat_infer_kernel<4><<<grid, kThreads, 0, st>>>(a);
+    else gat_infer_kernel<8><<<grid, kThreads, 0, st>>>(a);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

@@ -9,7 +9,8 @@ checkpoints are interchangeable.
 
 Differences, deliberate: the reference copies the model to the CPU and evaluates in a thread pool with DGL on the host;
 here the copy stays on the GPU and the full-graph forward uses the same SpMM / dense kernels as training
-(``FullGraphHandle``: module/layer.py:39-45, 93-102 eval branches), synchronously.
+(``FullGraphHandle``: module/layer.py:39-45, 93-102 eval branches; GAT: ``GATConv``'s homogeneous call on the one-pass
+attention kernel, module/gat.py), synchronously.
 """
 from __future__ import annotations
 

@@ -75,6 +75,12 @@ class FullGraphHandle:
     def out_degrees(self):
         return self._out
 
+    def has_zero_in_degree(self) -> bool:
+        """Whether some node has no in-edge (checked once: it synchronises with the device)."""
+        if getattr(self, "_zero_in", None) is None:
+            self._zero_in = bool((self._in == 0).any())
+        return self._zero_in
+
 
 def halo_aggregate(g: PartitionGraph, x_halo: torch.Tensor, y: torch.Tensor, rs, cs_halo) -> None:
     """``y += rs * A_out[:, sampled] (cs_halo * x_halo)``.  With the epoch's compaction (the default) the kernel walks
@@ -336,3 +342,54 @@ class GatAttention(torch.autograd.Function):
                 ops.spmm_weighted(g.a_out_t, d_rst[:, cols], d_ft[n_in:, cols], w_out, h, through_perm=True,
                                   row_map=g.slot)
         return d_ft, d_el, d_er, None, None, None, None, None, None
+
+
+GAT_INFER_MAX_HEADS, GAT_INFER_MAX_WIDTH = 8, 1024
+
+
+def gat_padded_width(Fo: int) -> int:
+    """The per-head width rounded up to a multiple of 4 (16-byte lanes)."""
+    return (Fo + 3) // 4 * 4
+
+
+def gat_infer_unsupported(H: int, Fo: int) -> Optional[str]:
+    """``None`` when ``bns_gat_infer_f32`` takes ``H`` heads of width ``Fo``, else the limit that is exceeded."""
+    if not 1 <= H <= GAT_INFER_MAX_HEADS:
+        return f"heads = {H} is outside 1..{GAT_INFER_MAX_HEADS}"
+    if Fo < 1 or H * gat_padded_width(Fo) > GAT_INFER_MAX_WIDTH:
+        return (f"heads * padded per-head width = {H} * {gat_padded_width(Fo)} exceeds {GAT_INFER_MAX_WIDTH}"
+                if Fo >= 1 else f"per-head width {Fo} < 1")
+    return None
+
+
+def gat_infer(a: ops.DeviceGraph, ft: torch.Tensor, el: torch.Tensor, er: torch.Tensor, H: int, Fp: int, slope: float,
+              bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The evaluation forward of ``dgl.nn.GATConv``'s attention on a homogeneous graph ``a`` (``bns_gat_infer_f32``):
+
+        rst[v, h, :] = sum_{u -> v} softmax_u(leaky_relu(el[u, h] + er[v, h], slope)) * ft[u, h, :] + bias[h, :]
+
+    ``ft [a.n_cols, H * Fp]`` (head-major, ``Fp`` a multiple of 4, pad columns zero), ``el [a.n_cols, H]``,
+    ``er [a.n_rows, H]``, ``bias [H * Fp]`` or None -> ``[a.n_rows, H * Fp]``.  No dropout, no gradient."""
+    from ._lib import BnsError, check, lib
+    why = gat_infer_unsupported(H, Fp)
+    if why is not None or Fp % 4:
+        raise BnsError(f"gat_infer: {why or f'padded width {Fp} is not a multiple of 4'}")
+    for t, name in ((ft, "ft"), (el, "el"), (er, "er")) + (((bias, "bias"),) if bias is not None else ()):
+        ops._req(t, torch.float32, name)
+        if t.device != a.device:
+            raise BnsError(f"gat_infer: {name} is on {t.device}, the graph on {a.device}")
+    if ft.dim() != 2 or tuple(ft.shape) != (a.n_cols, H * Fp) or ft.stride(1) != 1:
+        raise BnsError(f"gat_infer: ft must be [{a.n_cols}, {H * Fp}] with unit column stride, got {tuple(ft.shape)}")
+    if tuple(el.shape) != (a.n_cols, H) or tuple(er.shape) != (a.n_rows, H):
+        raise BnsError(f"gat_infer: el / er must be [{a.n_cols}, {H}] / [{a.n_rows}, {H}], got {tuple(el.shape)} / "
+                       f"{tuple(er.shape)}")
+    if bias is not None and tuple(bias.shape) != (H * Fp,):
+        raise BnsError(f"gat_infer: bias must be [{H * Fp}], got {tuple(bias.shape)}")
+    el, er = el.contiguous(), er.contiguous()
+    bias = bias.contiguous() if bias is not None else None
+    rst = torch.empty(a.n_rows, H * Fp, dtype=torch.float32, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.bns_gat_infer_f32(a._h, ft.data_ptr(), ft.stride(0), H, Fp, el.data_ptr(), er.data_ptr(), float(slope),
+                                    ops._ptr(bias), rst.data_ptr(), rst.stride(0),
+                                    torch.cuda.current_stream(a.device).cuda_stream), "bns_gat_infer_f32")
+    return rst

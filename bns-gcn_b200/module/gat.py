@@ -10,13 +10,18 @@ Everything after ``fc`` runs as kernels of libbnsgcn.so (``graph.GatProjection``
 dropout on the Philox kernel).  The op-by-op fallback (``BNS_GAT_FUSED=0`` or a per-head width that is not a multiple
 of 4) writes the per-entry score / softmax algebra as torch ops on ``[nnz, heads]`` vectors over the STATIC entry lists
 of the partition graph (an unsampled halo entry gets e = -inf, i.e. weight 0) around the weighted SpMM, its transpose
-and the SDDMM-dot of the attention gradient (``graph.WeightedAggregate``)."""
+and the SDDMM-dot of the attention gradient (``graph.WeightedAggregate``).
+
+In evaluation the layer also takes DGL's homogeneous call ``layer(g, h)`` on the full graph (``FullGraphHandle``, what
+``GAT.forward`` makes when not training): one ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, and the attention as
+one pass over each row (``graph.gat_infer``: online softmax, nothing stored per entry)."""
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from .. import fused, ops
-from ..graph import GatAttention, GatProjection, PartitionGraph, WeightedAggregate, gat_entries
+from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionGraph, WeightedAggregate, gat_entries,
+                     gat_infer, gat_infer_unsupported, gat_padded_width)
 from . import dense
 
 
@@ -52,8 +57,14 @@ class GATConv(nn.Module):
             nn.init.constant_(self.bias, 0)
 
     def forward(self, graph, feat):
+        if isinstance(graph, FullGraphHandle) and isinstance(feat, torch.Tensor):
+            if self.training:
+                raise NotImplementedError("GATConv: layer(g, h) on the full graph is the evaluation forward only; "
+                                          "call .eval() first")
+            return self._forward_full_graph(graph, feat)
         if not isinstance(graph, PartitionGraph) or not isinstance(feat, tuple):
-            raise NotImplementedError("GATConv: only the training call layer(g, (h_src, h_dst)) of the reference")
+            raise NotImplementedError("GATConv: the training call layer(g, (h_src, h_dst)) on a partition graph, or "
+                                      "layer(g, h) on the full graph in evaluation")
         H, Fo = self._num_heads, self._out_feats
         n_in = graph.n_in
         ready = getattr(feat[0], '_bns_ready', None)
@@ -120,3 +131,29 @@ class GATConv(nn.Module):
         if self.bias is not None:
             rst = rst + self.bias.view(1, H, Fo)
         return rst
+
+    @torch.no_grad()
+    def _forward_full_graph(self, graph: FullGraphHandle, feat: torch.Tensor) -> torch.Tensor:
+        """DGL's homogeneous branch with ``h_src = h_dst = feat`` (``feat_drop`` is the identity in evaluation): one
+        ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, then the one-pass attention kernel (``graph.gat_infer``).
+        A per-head width that is not a multiple of 4 runs padded -- zero rows of ``fc.weight``, zero columns of
+        ``attn_l`` / ``attn_r`` / ``bias`` per head -- and the pad is sliced off.  No gradient flows through it."""
+        H, Fo = self._num_heads, self._out_feats
+        why = gat_infer_unsupported(H, Fo)
+        if why is not None:
+            raise NotImplementedError(f"GATConv evaluation forward: {why}")
+        if graph.has_zero_in_degree():
+            # dgl.nn.GATConv(allow_zero_in_degree=False) refuses such a graph (DGLError)
+            raise RuntimeError("GATConv: there are 0-in-degree nodes in the graph, their output would be invalid; "
+                               "add self-loops")
+        Fp = gat_padded_width(Fo)
+        w, al, ar, b = self.fc.weight, self.attn_l, self.attn_r, self.bias
+        if Fp != Fo:
+            pad = Fp - Fo
+            w = F.pad(w.view(H, Fo, -1), (0, 0, 0, pad)).reshape(H * Fp, -1)
+            al, ar = F.pad(al, (0, pad)), F.pad(ar, (0, pad))
+            b = F.pad(b.view(H, Fo), (0, pad)).reshape(-1) if b is not None else None
+        ft = dense.linear(feat, w)                                  # [n, H * Fp]
+        el, er = GatProjection.apply(ft, ft, al, ar, H, Fp)
+        rst = gat_infer(graph.a, ft, el, er, H, Fp, self.negative_slope, b)
+        return rst.view(-1, H, Fp)[..., :Fo]

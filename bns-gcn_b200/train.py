@@ -582,9 +582,16 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     dev = st.feat.device
     evaluator = None
     if getattr(args, 'eval', False) and rank == 0:
+        why = None
         if args.model == 'gat':
+            # the full-graph GAT forward runs on bns_gat_infer_f32: decide now whether every attention layer fits it
+            from .graph import gat_infer_unsupported
+            from .module.gat import GATConv
+            why = next((w for w in (gat_infer_unsupported(m._num_heads, m._out_feats) for m in st.model.layers
+                                    if isinstance(m, GATConv)) if w is not None), None)
+        if why is not None:
             import warnings
-            warnings.warn('--eval: the full-graph GAT forward (dgl.nn.GATConv on a homogeneous graph) is not rebuilt; '
+            warnings.warn(f'--eval: the full-graph GAT evaluation forward does not take this model ({why}); '
                           'training runs without the evaluation branch')
         else:
             from .data import make_graph

@@ -358,6 +358,16 @@ int bns_gat_proj_bwd_f32(const float *X, int64_t ldx, int64_t rows, int32_t head
                          void *stream);
 int bns_gat_colsum_f32(const bns_graph_t *gT, const float *dE, int32_t heads, const int32_t *row_map, int64_t out_base,
                        float *d_el, void *stream);
+/* The evaluation forward of GATConv on a homogeneous graph g (CSR by destination; DGL 0.9 gatconv.py with
+ * h_src = h_dst, no dropout):
+ *     rst[v, h, :] = sum_{u -> v} softmax_u(leaky_relu(el[u, h] + er[v, h])) * ft[u, h, :] + bias[h, :]
+ * in ONE pass over each row (online softmax: running maximum and sum rescaled per block of 32 entries), one warp per
+ * destination row, nothing stored per entry.  ft [n_cols, heads, Fp] and rst [n_rows, heads, Fp] (rows ldft / ldr
+ * floats apart, 16-byte aligned), Fp = the per-head width rounded up to a multiple of 4 with zero pad columns;
+ * heads <= 8, heads * Fp <= 1024.  el [n_cols, heads], er [n_rows, heads], bias [heads * Fp] (16-byte aligned) or NULL.
+ * A row without entries gets the bias alone.  Deterministic: the summation order is fixed per row. */
+int bns_gat_infer_f32(const bns_graph_t *g, const float *ft, int64_t ldft, int32_t heads, int32_t Fp, const float *el,
+                      const float *er, float negative_slope, const float *bias, float *rst, int64_t ldr, void *stream);
 int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                           const float *weights, int64_t ldw, int perm_from_transpose, const int32_t *row_map, int64_t x_rows,
                           int accumulate, void *ws, size_t ws_bytes, void *stream);
