@@ -712,6 +712,7 @@ extern "C" int bns_gat_backward_f32(const bns_graph_t *a_in, const bns_graph_t *
     BNS_REQUIRE(ldft % 4 == 0 && ldd % 4 == 0 && ldft >= H * Fo && ldd >= H * Fo &&
                     ((reinterpret_cast<uintptr_t>(ft) | reinterpret_cast<uintptr_t>(d_rst)) & 15u) == 0,
                 "bns_gat_backward_f32: 16-byte aligned rows required");
+    BNS_REQUIRE(p_drop >= 0.f && p_drop < 1.f, "bns_gat_backward_f32: p must be in [0, 1)");
     a.ft = ft; a.ldft = ldft; a.H = H; a.Fo = Fo; a.el = el; a.er = er; a.slope = slope; a.p_drop = p_drop;
     a.keep_scale = 1.f / (1.f - p_drop); a.seed = seed; a.offset = offset; a.offset_dev = offset_dev;
     a.d_rst = d_rst; a.ldd = ldd; a.P_in = const_cast<float *>(P_in); a.P_out = const_cast<float *>(P_out);
@@ -760,6 +761,7 @@ extern "C" int bns_gat_softmax_bwd_f32(const bns_graph_t *a_in, const bns_graph_
     BNS_REQUIRE(H >= 1 && H <= kGatMaxHeads, "bns_gat_softmax_bwd_f32: 1 <= heads <= 8");
     if (a.g.n_rows == 0) return BNS_OK;
     BNS_REQUIRE(el && er && P_in && dE_in && d_er && (a.g.cidx == nullptr || (P_out && dE_out)), "bns_gat_softmax_bwd_f32: NULL pointer");
+    BNS_REQUIRE(p_drop >= 0.f && p_drop < 1.f, "bns_gat_softmax_bwd_f32: p must be in [0, 1)");
     a.H = H; a.Fo = 4; a.el = el; a.er = er; a.slope = slope; a.p_drop = p_drop; a.keep_scale = 1.f / (1.f - p_drop);
     a.seed = seed; a.offset = offset; a.offset_dev = offset_dev;
     a.P_in = const_cast<float *>(P_in); a.P_out = const_cast<float *>(P_out); a.dE_in = dE_in; a.dE_out = dE_out; a.d_er = d_er;

@@ -234,6 +234,13 @@ class GatProjection(torch.autograd.Function):
         return outs[0][0], outs[1][0], outs[0][1], outs[1][1], None, None
 
 
+def gat_attention_supported(H: int, Fo: int) -> bool:
+    """Whether ``GatAttention`` takes ``H`` heads of width ``Fo``: exactly what ``bns_gat_forward_f32`` and
+    ``bns_gat_backward_f32`` accept -- 1..8 heads, a positive per-head width that is a multiple of 4 (16-byte lanes),
+    at most 1024 columns in all."""
+    return 1 <= H <= 8 and Fo > 0 and Fo % 4 == 0 and H * Fo <= 1024
+
+
 class GatAttention(torch.autograd.Function):
     """The attention of ``dgl.nn.GATConv`` for all heads:
 

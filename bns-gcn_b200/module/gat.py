@@ -20,8 +20,8 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import fused, ops
-from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionGraph, WeightedAggregate, gat_entries,
-                     gat_infer, gat_infer_unsupported, gat_padded_width)
+from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionGraph, WeightedAggregate,
+                     gat_attention_supported, gat_entries, gat_infer, gat_infer_unsupported, gat_padded_width)
 from . import dense
 
 
@@ -70,7 +70,7 @@ class GATConv(nn.Module):
         ready = getattr(feat[0], '_bns_ready', None)
         if ready is not None:          # every row of h_src is read below: wait for the overlapped exchange
             torch.cuda.current_stream(feat[0].device).wait_event(ready)
-        kernels = FUSED_ATTENTION and Fo % 4 == 0 and H <= 8 and H * Fo <= 1024 and \
+        kernels = FUSED_ATTENTION and gat_attention_supported(H, Fo) and \
             (graph.a_out is None or (graph.compact is not None and graph.compact.cpos is not None))
         salt = ops.RNG["seed"] + 15485863 * (1 + getattr(self, "_layer_index", 0))
         pf = self.feat_drop.p if self.training else 0.0

@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 import torch
 
+from tests.gat_reference import gat_attention_reference, gat_row_walk_nv
+
 pytestmark = pytest.mark.gpu
 
 RTOL = 1e-5
@@ -336,7 +338,7 @@ def test_dense_3xtf32_is_fp32_accurate(built):
     assert _relerr(y.detach().cpu(), y32.cpu()) < 1e-5
 
 
-@pytest.mark.parametrize("F,p", [(256, 0.0), (256, 0.5), (64, 0.3), (600, 0.5), (16, 0.0)])
+@pytest.mark.parametrize("F,p", [(256, 0.0), (256, 0.5), (64, 0.3), (600, 0.5), (16, 0.0), (512, 0.5), (388, 0.0)])
 def test_fused_layernorm_relu_dropout(built, F, p):
     """ops.LnReluDropout == dropout(relu(layer_norm(x))) forward and backward (mask recovered from the output),
     mask keep-rate ~ 1-p, masks differ across offsets and repeat for the same (seed, offset)."""
@@ -699,8 +701,16 @@ def _gat_case(H, Fo, seed, with_halo=True):
     return g, n_in, n_u, torch.cat(u), torch.cat(v), gen
 
 
+GAT_ATTENTION_CASES = [(1, 64, True), (2, 8, True), (4, 16, False), (1, 256, True), (1, 100, True), (4, 128, True),
+                       (3, 100, True), (8, 128, True), (5, 16, True), (8, 4, False), (1, 1024, True)]
+# every instantiation of the row-walk kernels, and heads above 4 (the upper half of their per-head registers and the
+# second Philox counter word of the dropout mask), stay covered when the list is edited
+assert {gat_row_walk_nv(H, Fo) for H, Fo, _ in GAT_ATTENTION_CASES} == {1, 2, 4, 8}
+assert any(H > 4 for H, _, _ in GAT_ATTENTION_CASES)
+
+
 @pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
-@pytest.mark.parametrize("H,Fo,with_halo", [(1, 64, True), (2, 8, True), (4, 16, False), (1, 256, True), (1, 100, True)])
+@pytest.mark.parametrize("H,Fo,with_halo", GAT_ATTENTION_CASES)
 def test_fused_gat_attention_matches_the_per_entry_reference(built, monkeypatch, H, Fo, with_halo, rowwalk):
     """graph.GatAttention == the u_add_v / leaky_relu / edge_softmax / u_mul_e+sum algebra of dgl.nn.GATConv written with
     torch ops on explicit entry lists (what module/gat.py's op-by-op path and oracle.GATConvRef do), forward and the
@@ -713,22 +723,14 @@ def test_fused_gat_attention_matches_the_per_entry_reference(built, monkeypatch,
     el = torch.randn(n_u, H, generator=gen)
     er = torch.randn(n_in, H, generator=gen)
     d = torch.randn(n_in, H * Fo, generator=gen)
-    # reference (f64 on the CPU)
-    ftr, elr, err = (t.double().clone().requires_grad_(True) for t in (ft, el, er))
-    e = torch.nn.functional.leaky_relu(elr[u] + err[v], 0.2)
-    m = torch.full((n_in, H), float("-inf"), dtype=torch.float64).scatter_reduce(0, v.unsqueeze(1).expand(-1, H), e.detach(), "amax")
-    ex = torch.exp(e - m[v])
-    den = torch.zeros(n_in, H, dtype=torch.float64).index_add(0, v, ex)
-    a = ex / den[v]
-    ref = torch.zeros(n_in, H, Fo, dtype=torch.float64).index_add(0, v, a.unsqueeze(-1) * ftr.view(-1, H, Fo)[u]).reshape(n_in, H * Fo)
-    (ref * d.double()).sum().backward()
+    ref, d_ft, d_el, d_er = gat_attention_reference(ft, el, er, u, v, n_in, H, Fo, d)[:4]
     ftg, elg, erg = (t.to(dev).requires_grad_(True) for t in (ft, el, er))
     out = GatAttention.apply(ftg, elg, erg, g, H, Fo, 0.2, 0.0, 1)
     (out * d.to(dev)).sum().backward()
-    assert _relerr(out.detach().cpu(), ref.detach().float()) < 2e-5
-    assert _relerr(ftg.grad.cpu(), ftr.grad.float()) < 2e-5
-    assert _relerr(elg.grad.cpu(), elr.grad.float()) < 5e-5
-    assert _relerr(erg.grad.cpu(), err.grad.float()) < 5e-5
+    assert _relerr(out.detach().cpu(), ref.float()) < 2e-5
+    assert _relerr(ftg.grad.cpu(), d_ft.float()) < 2e-5
+    assert _relerr(elg.grad.cpu(), d_el.float()) < 5e-5
+    assert _relerr(erg.grad.cpu(), d_er.float()) < 5e-5
     # rows without any entry produce zeros
     deg = torch.bincount(v, minlength=n_in)
     assert torch.all(out.detach().cpu()[deg == 0] == 0)
