@@ -101,6 +101,9 @@ SIGNATURES = {
     "bns_gat_colsum_f32": (c_int, [c_void_p, c_void_p, c_int32, c_void_p, c_int64, c_void_p, c_void_p]),
     "bns_gat_infer_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_float, c_void_p,
                                   c_void_p, c_int64, c_void_p]),
+    "bns_gat_infer_block_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_float,
+                                        c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p, c_int64,
+                                        c_void_p]),
     "bns_spmm_weighted_f32": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int,
                                       c_void_p, c_int64, c_int, c_void_p, c_size_t, c_void_p]),
     "bns_spmm_compact_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_void_p,

@@ -20,6 +20,7 @@
 #include <cstring>
 #include <atomic>
 #include <new>
+#include <type_traits>
 
 namespace {
 

@@ -505,6 +505,15 @@ __global__ void __launch_bounds__(kThreads) gat_colsum_kernel(const int64_t *__r
 // exp are rescaled by exp(m_old - m_new) (online softmax).  The block's source ids and weights are staged in shared
 // memory and the gathered ft rows accumulated as in gat_fwd_kernel.  Every sum runs in an order fixed per row, so two
 // launches on the same inputs give bit-identical results.
+//
+// BLOCK = true (bns_gat_infer_block_f32): the row's entries arrive as several matrices over different column sets (a
+// partition's inner matrix, then one block per peer's halo rows), one launch each, and the softmax state is carried
+// between launches in memory: m [n_rows, H] running maximum, l [n_rows, H] warp-reduced sum of exp, acc [n_rows, H * Fp]
+// un-normalised accumulator.  A launch that is not `first` reloads it (l into lane 0, the other lanes start at 0) and
+// rescales it as the single pass does when the maximum grows; one that is not `last` stores it back, `last` writes
+// acc / l + bias.  A row without entries in a launch keeps its state untouched.  The state rides in a derived argument
+// struct of the BLOCK instantiations only, so the single-pass ones compile exactly as before.  (BLOCK, NV = 1 asks for
+// one resident block per SM as its register budget: without it ptxas picks 64 registers and spills.)
 struct GatInferArgs {
     const int64_t *indptr; const int32_t *indices; int64_t n_rows;
     const float *ft; int64_t ldft; int32_t H, Fp;          // ft [n_cols, H, Fp]: Fp = per-head width padded to 4
@@ -513,8 +522,14 @@ struct GatInferArgs {
     float *rst; int64_t ldr;                               // [n_rows, H, Fp]
 };
 
-template <int NV>
-__global__ void __launch_bounds__(kThreads) gat_infer_kernel(GatInferArgs a) {
+struct GatInferBlockArgs : GatInferArgs {
+    float *sm, *sl, *sacc; int64_t ldacc;                  // the carried state
+    int32_t first, last;
+};
+
+template <int NV, bool BLOCK = false>
+__global__ void __launch_bounds__(kThreads, BLOCK ? 1 : 0)
+gat_infer_kernel(typename std::conditional<BLOCK, GatInferBlockArgs, GatInferArgs>::type a) {
     __shared__ int32_t s_u[kWarps][32];
     __shared__ float s_w[kWarps][32][kGatMaxHeads];
     __shared__ float s_h[kWarps][kGatMaxHeads];           // per-head rescale factors, then the row's sums of exp
@@ -540,6 +555,23 @@ __global__ void __launch_bounds__(kThreads) gat_infer_kernel(GatInferArgs a) {
 #pragma unroll
         for (int t = 0; t < NV; ++t) acc[t] = make_float4(0.f, 0.f, 0.f, 0.f);
         const int64_t b = a.indptr[v], e = a.indptr[v + 1];
+        if constexpr (BLOCK) {
+            if (b == e && !a.first && !a.last) continue;        // (warp-uniform) no entries here: state untouched
+            if (!a.first) {
+#pragma unroll
+                for (int h = 0; h < kGatMaxHeads; ++h)
+                    if (h < H) {
+                        m[h] = a.sm[v * H + h];
+                        l[h] = lane == 0 ? a.sl[v * H + h] : 0.f;
+                    }
+                const float *sa = a.sacc + v * a.ldacc;
+#pragma unroll
+                for (int t = 0; t < NV; ++t) {
+                    const int c = (lane + 32 * t) * 4;
+                    if (c < F) acc[t] = *reinterpret_cast<const float4 *>(sa + c);
+                }
+            }
+        }
         for (int64_t k0 = b; k0 < e; k0 += 32) {
             const int64_t k = k0 + lane;
             const bool valid = k < e;
@@ -615,6 +647,23 @@ __global__ void __launch_bounds__(kThreads) gat_infer_kernel(GatInferArgs a) {
         }
 #pragma unroll
         for (int h = 0; h < kGatMaxHeads; ++h) l[h] = warp_sum(l[h]);
+        if constexpr (BLOCK) {
+            if (!a.last) {
+                if (lane == 0) {
+#pragma unroll
+                    for (int h = 0; h < kGatMaxHeads; ++h)
+                        if (h < H) { a.sm[v * H + h] = m[h]; a.sl[v * H + h] = l[h]; }
+                }
+                float *sa = a.sacc + v * a.ldacc;
+#pragma unroll
+                for (int t = 0; t < NV; ++t) {
+                    const int c = (lane + 32 * t) * 4;
+                    if (c < F) *reinterpret_cast<float4 *>(sa + c) = acc[t];
+                }
+                __syncwarp();                     // s_h is rewritten by the next row
+                continue;
+            }
+        }
         if (lane == 0) {
 #pragma unroll
             for (int h = 0; h < kGatMaxHeads; ++h) s_h[w][h] = l[h];
@@ -811,6 +860,43 @@ extern "C" int bns_gat_infer_f32(const bns_graph_t *g, const float *ft, int64_t 
     else if (nv == 2) gat_infer_kernel<2><<<grid, kThreads, 0, st>>>(a);
     else if (nv <= 4) gat_infer_kernel<4><<<grid, kThreads, 0, st>>>(a);
     else gat_infer_kernel<8><<<grid, kThreads, 0, st>>>(a);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// the same forward over a row set whose entries come as several column blocks, one launch per block, the online-softmax
+// state (m, l, acc) carried between launches (gat_infer_kernel<NV, true>)
+extern "C" int bns_gat_infer_block_f32(const bns_graph_t *g, const float *ft, int64_t ldft, int32_t H, int32_t Fp,
+                                       const float *el, const float *er, float slope, float *m, float *l, float *acc,
+                                       int64_t ldacc, int first, int last, const float *bias, float *rst, int64_t ldr,
+                                       void *stream) {
+    BNS_REQUIRE(g, "bns_gat_infer_block_f32: NULL graph");
+    BNS_REQUIRE(H >= 1 && H <= kGatMaxHeads && Fp > 0 && Fp % 4 == 0 && (int64_t)H * Fp <= 1024,
+                "bns_gat_infer_block_f32: need 1 <= heads <= 8, padded width %% 4 == 0, heads * padded width <= 1024 "
+                "(got %d, %d)", H, Fp);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(er && m && l && acc && (g->nnz == 0 || (ft && el)) && (!last || rst),
+                "bns_gat_infer_block_f32: NULL pointer");
+    const int64_t HF = (int64_t)H * Fp;
+    BNS_REQUIRE(ldft % 4 == 0 && ldr % 4 == 0 && ldacc % 4 == 0 && (g->nnz == 0 || ldft >= HF) && (!last || ldr >= HF) &&
+                    ldacc >= HF &&
+                    ((reinterpret_cast<uintptr_t>(ft) | reinterpret_cast<uintptr_t>(rst) |
+                      reinterpret_cast<uintptr_t>(acc) | reinterpret_cast<uintptr_t>(bias)) & 15u) == 0,
+                "bns_gat_infer_block_f32: 16-byte aligned rows required");
+    BNS_REQUIRE(!last || rst != acc || ldr == ldacc, "bns_gat_infer_block_f32: rst aliases acc with a different stride");
+    GatInferBlockArgs a{};
+    a.indptr = g->indptr; a.indices = g->indices; a.n_rows = g->n_rows;
+    a.ft = ft; a.ldft = ldft; a.H = H; a.Fp = Fp; a.el = el; a.er = er; a.bias = bias; a.slope = slope;
+    a.rst = rst; a.ldr = ldr;
+    a.sm = m; a.sl = l; a.sacc = acc; a.ldacc = ldacc; a.first = first ? 1 : 0; a.last = last ? 1 : 0;
+    const int nv = (int)((HF + 127) / 128);
+    const unsigned grid = gat_grid(g->n_rows);
+    cudaStream_t st = as_stream(stream);
+    if (nv <= 1) gat_infer_kernel<1, true><<<grid, kThreads, 0, st>>>(a);
+    else if (nv == 2) gat_infer_kernel<2, true><<<grid, kThreads, 0, st>>>(a);
+    else if (nv <= 4) gat_infer_kernel<4, true><<<grid, kThreads, 0, st>>>(a);
+    else gat_infer_kernel<8, true><<<grid, kThreads, 0, st>>>(a);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

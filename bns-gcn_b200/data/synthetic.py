@@ -67,8 +67,9 @@ SHAPES = {
     "yelp": dict(n=716_847, e=13_954_819, n_feat=300, n_class=100, train=0.75, multilabel=True, law="powerlaw"),
     # configs[4]: ogbn-papers100M: 111,059,956 nodes, 1,615,685,872 edges, 128 feats, 172 classes.  Never built as one
     # graph (57 GB of features): every rank generates ITS piece on its GPU, see make_local_partition
+    # (val / test: ogbn-papers100M's split, 125,265 / 214,338 nodes; read by make_local_partition only)
     "papers100m": dict(n=111_059_956, e=1_615_685_872, n_feat=128, n_class=172, train=0.011, multilabel=False,
-                       law="powerlaw"),
+                       law="powerlaw", val=0.0011, test=0.0019),
     # small shapes used by tests / smoke
     "tiny": dict(n=600, e=6_000, n_feat=16, n_class=5, train=0.5, multilabel=False, law="powerlaw"),
     "tiny-ml": dict(n=500, e=5_000, n_feat=12, n_class=6, train=0.6, multilabel=True, law="powerlaw"),
@@ -270,8 +271,17 @@ def make_local_partition(name: str, rank: int, world: int, seed: int = 0, device
     else:
         label = torch.randint(0, n_class, (n_in,), generator=fgen, dtype=torch.int64, device=device)
     train_mask = torch.rand(n_in, generator=fgen, device=device) < spec["train"]
+    # val / test from a generator of their own, so that every tensor above stays what it was without them; disjoint
+    # from train_mask and from each other, at the shape's fractions of all nodes (default: make_graph's 1/3 : 2/3 split
+    # of the rest)
+    rest = 1.0 - spec["train"]
+    p_val, p_test = spec.get("val", rest / 3) / rest, spec.get("test", 2 * rest / 3) / rest
+    u = torch.rand(n_in, generator=torch.Generator(device=device).manual_seed(seed * 1_000_003 + 11 + rank),
+                   device=device)
+    val_mask = ~train_mask & (u < p_val)
+    test_mask = ~train_mask & (u >= p_val) & (u < p_val + p_test)
     nd = {NID: gid, "part_id": part_id, "inner_node": inner_node, "feat": feat, "label": label, "in_deg": in_deg,
-          "out_deg": in_deg.clone(), "train_mask": train_mask}
+          "out_deg": in_deg.clone(), "train_mask": train_mask, "val_mask": val_mask, "test_mask": test_mask}
     meta = {"n_feat": n_feat, "n_class": n_class, "n_train": max(int(round(spec["train"] * n)), 1)}
     return Partition(rank, world, LocalGraph(n_in, int(halo.numel()), indptr, local.contiguous()), nd,
                      GraphPartitionBook(ranges.clone()), meta)

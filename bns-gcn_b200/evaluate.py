@@ -11,6 +11,9 @@ Differences, deliberate: the reference copies the model to the CPU and evaluates
 here the copy stays on the GPU and the full-graph forward uses the same SpMM / dense kernels as training
 (``FullGraphHandle``: module/layer.py:39-45, 93-102 eval branches; GAT: ``GATConv``'s homogeneous call on the one-pass
 attention kernel, module/gat.py), synchronously.
+
+``ParallelEvaluator`` (``--parallel-eval``, transductive runs only) splits that forward over the ranks instead: each
+evaluates its own nodes on its partition with the whole halo exchanged layer by layer, and nobody builds the full graph.
 """
 from __future__ import annotations
 
@@ -154,4 +157,94 @@ class Evaluator:
         print('model saved')
         print("Max Validation Accuracy {:.2%}".format(self.best_acc))
         _, acc = evaluate_induc('Test Result', self.best_model, self.test_g, 'test')
+        return acc
+
+
+def acc_counts(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
+    """What ``calc_acc`` needs, as sums that add up across ranks: ``[correct, total]`` for single-label tasks,
+    ``[TP, FP, FN]`` of ``logits > 0`` for multi-label ones (float64 on the device: exact up to 2^53)."""
+    if labels.dim() == 1:
+        correct = (logits.argmax(dim=1) == labels).sum()
+        return torch.stack([correct, correct.new_tensor(labels.shape[0])]).double()
+    pred, lab = logits > 0, labels > 0.5
+    return torch.stack([(pred & lab).sum(), (pred & ~lab).sum(), (~pred & lab).sum()]).double()
+
+
+def acc_of_counts(c: torch.Tensor) -> float:
+    """``calc_acc`` from the summed counts of ``acc_counts``."""
+    c = c.tolist()
+    if len(c) == 2:
+        return c[0] / c[1] if c[1] else 0.0
+    den = 2 * c[0] + c[1] + c[2]
+    return 2.0 * c[0] / den if den else 0.0
+
+
+def build_partition_eval_graph(part, node_dict, boundary, comm):
+    """``graph.PartitionEvalGraph`` of a training partition (``train.setup``'s ``part`` and ``boundary``; ``node_dict``
+    of ``load_partition``).  Collective: the halo's out-degrees come from their owners (``train.collect_out_degree``)."""
+    from .graph import PartitionEvalGraph
+    from .train import _halo_counts, collect_out_degree
+    dev = part.a_in.device
+    nd = {k: node_dict[k].to(dev) for k in ('part_id', 'in_deg', 'out_deg')}
+    out_deg = collect_out_degree(nd, boundary)
+    return PartitionEvalGraph(part.a_in, part.a_out, _halo_counts(nd), boundary, nd['in_deg'], out_deg, comm)
+
+
+class ParallelEvaluator:
+    """``Evaluator`` with the evaluation forward split over the ranks (``--parallel-eval``, transductive runs): each
+    rank computes the logits of its own inner nodes on its partition with every halo node present
+    (``graph.PartitionEvalGraph``: the whole boundary exchanged layer by layer), counts its masked nodes, and the counts
+    are summed over the ranks -- every rank gets the same accuracy.  No rank builds the whole graph.
+
+    Collective: ALL ranks call ``after_epoch`` / ``finish`` at the same epochs.  Rank 0 alone writes the checkpoints and
+    the result lines (same names and formats as ``Evaluator``); every rank keeps its own snapshot of the best model (the
+    weights are replicated), so the final test pass needs no broadcast."""
+
+    def __init__(self, args, graph, feat: torch.Tensor, labels: torch.Tensor, val_mask: torch.Tensor,
+                 test_mask: torch.Tensor, comm):
+        self.args, self.graph, self.comm = args, graph, comm
+        self.feat, self.labels, self.val_mask, self.test_mask = feat, labels, val_mask, test_mask
+        self.is_root = comm.rank == 0
+        if self.is_root:
+            os.makedirs('checkpoint/', exist_ok=True)
+            os.makedirs('results/', exist_ok=True)
+        self.best_model, self.best_acc = None, 0.0
+        self.result_file_name = result_file_name(args)
+
+    @torch.no_grad()
+    def logits(self, model: torch.nn.Module) -> torch.Tensor:
+        """This rank's inner nodes' logits (collective)."""
+        model.eval()
+        return model(self.graph, self.feat)
+
+    def _acc(self, logits: torch.Tensor, mask: torch.Tensor) -> float:
+        c = acc_counts(logits[mask], self.labels[mask])
+        self.comm.all_reduce_sum(c)
+        return acc_of_counts(c)
+
+    def after_epoch(self, model: torch.nn.Module, epoch: int) -> float:
+        if self.is_root:
+            save_checkpoint(model, checkpoint_path(self.args, epoch))
+        snap = copy.deepcopy(model)
+        was_training = model.training
+        logits = self.logits(snap)
+        val_acc, test_acc = self._acc(logits, self.val_mask), self._acc(logits, self.test_mask)
+        if self.is_root:
+            _emit("{:s} | Validation Accuracy {:.2%} | Test Accuracy {:.2%}".format('Epoch %05d' % epoch, val_acc,
+                                                                                     test_acc), self.result_file_name)
+        if val_acc > self.best_acc or self.best_model is None:
+            self.best_acc, self.best_model = val_acc, snap
+        model.train(was_training)
+        return val_acc
+
+    def finish(self, model: torch.nn.Module) -> float:
+        if self.best_model is None:
+            self.best_model = copy.deepcopy(model)
+        if self.is_root:
+            save_checkpoint(self.best_model, checkpoint_path(self.args))
+            print('model saved')
+            print("Max Validation Accuracy {:.2%}".format(self.best_acc))
+        acc = self._acc(self.logits(self.best_model), self.test_mask)
+        if self.is_root:
+            _emit("{:s} | Accuracy {:.2%}".format('Test Result', acc), None)
         return acc

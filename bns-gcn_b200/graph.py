@@ -82,6 +82,112 @@ class FullGraphHandle:
         return self._zero_in
 
 
+class PartitionEvalGraph:
+    """This rank's partition with EVERY halo node present: the graph of the partition-parallel evaluation
+    (``evaluate.ParallelEvaluator``).  Every inner node holds all its in-edges and full-graph degrees, so with the whole
+    boundary exchanged (sampling ratio 1) the forward over the inner rows equals the whole-graph forward (SURVEY §4).
+
+    ``a_in`` (inner -> inner) and ``blocks[j]``: the columns of ``a_out`` owned by peer ``j`` (the halo is sorted by
+    global id, so each owner's columns are one contiguous range, ``halo_begin[j]`` onwards), renumbered from 0.
+    ``peer_rows(h)`` exchanges one peer at a time -- send ``h[boundary[right]]``, receive the left peer's rows -- so a
+    layer's extra memory is one peer's rows, not the whole halo.  Every rank must walk ``peer_rows`` in step: it is
+    collective.
+
+    The blocks are cut from ``a_out`` at the first evaluation, not when the handle is made, so training before it runs
+    at its own peak; they stay for the later evaluations: ``a_out``'s column ids once more (4 bytes per halo entry) and
+    one row-offset array per peer (8 bytes per inner node and peer)."""
+
+    EXCHANGE_TAG = 3000
+
+    def __init__(self, a_in: ops.DeviceGraph, a_out: Optional[ops.DeviceGraph], halo_counts, boundary, in_deg: torch.Tensor,
+                 out_deg: torch.Tensor, comm):
+        self.a_in, self.n_in = a_in, a_in.n_rows
+        self.comm, self.rank, self.size = comm, comm.rank, comm.size
+        self.boundary = boundary
+        self.halo_count = [0 if c is None else int(c) for c in halo_counts]
+        self.halo_begin, tot = [], 0
+        for c in self.halo_count:
+            self.halo_begin.append(tot)
+            tot += c
+        self.n_halo = tot
+        self._in, self._out = in_deg, out_deg               # full-graph degrees: [inner], [inner | halo]
+        dev = in_deg.device
+        # the peers in the order of the exchange steps (a ring, as precompute_streaming): a fixed summation order
+        self.order = [(self.rank - i + self.size) % self.size for i in range(1, self.size)]
+        self._a_out = a_out
+        self._blocks: Optional[Dict[int, ops.DeviceGraph]] = None
+        # decided over ALL ranks: a layer that refuses such a graph must refuse it on every rank, or the others hang
+        zero = torch.tensor([float(bool((in_deg == 0).any()))], dtype=torch.float32, device=dev)
+        comm.all_reduce_sum(zero)
+        self._zero_in = bool(zero.item() > 0)
+
+    @property
+    def blocks(self) -> Dict[int, ops.DeviceGraph]:
+        """``blocks[j]``: the entries of ``a_out`` whose column peer ``j`` owns, columns renumbered from 0."""
+        if self._blocks is None:
+            a_out, n_in, dev = self._a_out, self.n_in, self._in.device
+            blocks = {}
+            if a_out is not None and a_out.nnz:
+                ip, ix = a_out.csr()
+                rows = torch.repeat_interleave(torch.arange(n_in, dtype=torch.int32, device=dev), ip[1:] - ip[:-1])
+                del ip
+            for j in self.order:
+                b0, cnt = self.halo_begin[j], self.halo_count[j]
+                ipb = torch.zeros(n_in + 1, dtype=torch.int64, device=dev)
+                if a_out is not None and a_out.nnz:
+                    m = (ix >= b0) & (ix < b0 + cnt)
+                    ipb[1:] = torch.cumsum(torch.bincount(rows[m], minlength=n_in), 0)
+                    idx = ix[m] - b0
+                    del m
+                else:
+                    idx = torch.empty(0, dtype=torch.int32, device=dev)
+                blocks[j] = ops.DeviceGraph.from_csr(ipb, idx, cnt)
+                del ipb, idx
+            self._blocks = blocks
+        return self._blocks
+
+    def num_nodes(self, ntype: str = '_V') -> int:
+        return self.n_in
+
+    def in_degrees(self):
+        return self._in
+
+    def out_degrees(self):
+        return self._out
+
+    def has_zero_in_degree(self) -> bool:
+        """Whether some node of the whole graph has no in-edge (the same answer on every rank)."""
+        return self._zero_in
+
+    def peer_rows(self, h: torch.Tensor):
+        """Yields ``(j, blocks[j], rows of h of j's nodes that are my halo)`` for each peer ``j`` in ``order``, one
+        exchange per step (``h``: this rank's inner rows)."""
+        dev, blocks = h.device, self.blocks
+        for i, left in enumerate(self.order, start=1):
+            right = (self.rank + i) % self.size
+            send, recv = [None] * self.size, [None] * self.size
+            send[right] = h[self.boundary[right]]
+            recv[left] = torch.empty(self.halo_count[left], h.shape[1], dtype=h.dtype, device=dev)
+            self.comm.alltoall(send, recv, tag=self.EXCHANGE_TAG + i)
+            yield left, blocks[left], recv[left]
+            del send, recv
+
+    def aggregate(self, x: torch.Tensor, rs: torch.Tensor, cs: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``rs * (A_in (cs_in * x) + sum_j A_j (cs_j * x_j))`` over the inner rows: the whole-graph ``AggregateSum``
+        restricted to them (``cs`` over ``[inner | halo]``, ``x`` the inner rows; the halo rows arrive peer by peer)."""
+        n_in = self.n_in
+        x = x.contiguous()
+        # the column scale rides in the gather (no scaled copy of x or of a peer's rows)
+        y = ops.spmm_auto(self.a_in, x, row_scale=rs, col_scale=None if cs is None else cs[:n_in])
+        for j, blk, xr in self.peer_rows(x):
+            if blk.nnz == 0:
+                continue
+            b0 = n_in + self.halo_begin[j]
+            ops.spmm(blk, xr, y, row_scale=rs, col_scale=None if cs is None else cs[b0:b0 + self.halo_count[j]],
+                     accumulate=True)
+        return y
+
+
 def halo_aggregate(g: PartitionGraph, x_halo: torch.Tensor, y: torch.Tensor, rs, cs_halo) -> None:
     """``y += rs * A_out[:, sampled] (cs_halo * x_halo)``.  With the epoch's compaction (the default) the kernel walks
     the sampled entries only; without it (a graph whose slot map was set by hand) every halo entry is looked up."""
@@ -400,3 +506,39 @@ def gat_infer(a: ops.DeviceGraph, ft: torch.Tensor, el: torch.Tensor, er: torch.
                                     ops._ptr(bias), rst.data_ptr(), rst.stride(0),
                                     torch.cuda.current_stream(a.device).cuda_stream), "bns_gat_infer_f32")
     return rst
+
+
+def gat_infer_block(a: ops.DeviceGraph, ft: Optional[torch.Tensor], el: Optional[torch.Tensor], er: torch.Tensor, H: int,
+                    Fp: int, slope: float, m: torch.Tensor, l: torch.Tensor, acc: torch.Tensor, first: bool, last: bool,
+                    bias: Optional[torch.Tensor] = None, rst: Optional[torch.Tensor] = None) -> None:
+    """One column block of ``gat_infer`` (``bns_gat_infer_block_f32``): the rows' online-softmax state ``m``, ``l``
+    ``[a.n_rows, H]`` and ``acc [a.n_rows, H * Fp]`` is carried from the previous block (``first``: from empty);
+    ``last`` writes ``acc / l + bias`` to ``rst`` (which may be ``acc`` itself, same rows and stride).  ``ft [a.n_cols, H * Fp]`` / ``el
+    [a.n_cols, H]`` are this block's source rows (may be None when the block has no entries), ``er`` the rows' own."""
+    from ._lib import BnsError, check, lib
+    why = gat_infer_unsupported(H, Fp)
+    if why is not None or Fp % 4:
+        raise BnsError(f"gat_infer_block: {why or f'padded width {Fp} is not a multiple of 4'}")
+    if a.nnz and (ft is None or el is None):
+        raise BnsError("gat_infer_block: a block with entries needs ft and el")
+    if last and rst is None:
+        raise BnsError("gat_infer_block: the last block needs rst")
+    HF = H * Fp
+    for t, name, shape in ((ft, "ft", (a.n_cols, HF)), (el, "el", (a.n_cols, H)), (er, "er", (a.n_rows, H)),
+                           (m, "m", (a.n_rows, H)), (l, "l", (a.n_rows, H)), (acc, "acc", (a.n_rows, HF)),
+                           (bias, "bias", (HF,)), (rst, "rst", (a.n_rows, HF))):
+        if t is None:
+            continue
+        ops._req(t, torch.float32, name)
+        if t.device != a.device:
+            raise BnsError(f"gat_infer_block: {name} is on {t.device}, the graph on {a.device}")
+        if tuple(t.shape) != shape or t.stride(-1) != 1 or (t.dim() == 2 and name in ("el", "er", "m", "l")
+                                                               and not t.is_contiguous()):
+            raise BnsError(f"gat_infer_block: {name} must be {list(shape)} with unit column stride, got "
+                           f"{tuple(t.shape)}")
+    with torch.cuda.device(a.device):
+        check(lib.bns_gat_infer_block_f32(a._h, ops._ptr(ft), ft.stride(0) if ft is not None else HF, H, Fp, ops._ptr(el),
+                                          er.data_ptr(), float(slope), m.data_ptr(), l.data_ptr(), acc.data_ptr(),
+                                          acc.stride(0), 1 if first else 0, 1 if last else 0, ops._ptr(bias),
+                                          ops._ptr(rst), rst.stride(0) if rst is not None else HF,
+                                          torch.cuda.current_stream(a.device).cuda_stream), "bns_gat_infer_block_f32")

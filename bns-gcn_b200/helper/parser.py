@@ -61,6 +61,10 @@ def build_parser():
     # only here
     parser.add_argument(*_spellings("sampler-seed"), type=int, default=0,
                         help="NEW: Philox seed of the boundary sampler (the reference draws from unseeded numpy)")
+    parser.add_argument(*_spellings("parallel-eval"), action='store_true',
+                        help="NEW: with --eval, every rank evaluates its own nodes on its partition (the whole halo "
+                             "exchanged layer by layer) instead of rank 0 evaluating the full graph alone; the full "
+                             "graph is never built.  Transductive runs only")
     return parser
 
 

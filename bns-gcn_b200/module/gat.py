@@ -14,14 +14,17 @@ and the SDDMM-dot of the attention gradient (``graph.WeightedAggregate``).
 
 In evaluation the layer also takes DGL's homogeneous call ``layer(g, h)`` on the full graph (``FullGraphHandle``, what
 ``GAT.forward`` makes when not training): one ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, and the attention as
-one pass over each row (``graph.gat_infer``: online softmax, nothing stored per entry)."""
+one pass over each row (``graph.gat_infer``: online softmax, nothing stored per entry).  On a partition with every
+halo node present (``PartitionEvalGraph``, the partition-parallel evaluation) the same forward runs over the inner rows,
+the softmax state carried from the inner block to each peer's block (``graph.gat_infer_block``)."""
 import torch
 import torch.nn.functional as F
 from torch import nn
 
 from .. import fused, ops
-from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionGraph, WeightedAggregate,
-                     gat_attention_supported, gat_entries, gat_infer, gat_infer_unsupported, gat_padded_width)
+from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionEvalGraph, PartitionGraph, WeightedAggregate,
+                     gat_attention_supported, gat_entries, gat_infer, gat_infer_block, gat_infer_unsupported,
+                     gat_padded_width)
 from . import dense
 
 
@@ -62,6 +65,11 @@ class GATConv(nn.Module):
                 raise NotImplementedError("GATConv: layer(g, h) on the full graph is the evaluation forward only; "
                                           "call .eval() first")
             return self._forward_full_graph(graph, feat)
+        if isinstance(graph, PartitionEvalGraph):
+            if self.training:
+                raise NotImplementedError("GATConv: the partition graph with every halo node is for evaluation only; "
+                                          "call .eval() first")
+            return self._forward_partition(graph, feat)
         if not isinstance(graph, PartitionGraph) or not isinstance(feat, tuple):
             raise NotImplementedError("GATConv: the training call layer(g, (h_src, h_dst)) on a partition graph, or "
                                       "layer(g, h) on the full graph in evaluation")
@@ -138,6 +146,14 @@ class GATConv(nn.Module):
         ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, then the one-pass attention kernel (``graph.gat_infer``).
         A per-head width that is not a multiple of 4 runs padded -- zero rows of ``fc.weight``, zero columns of
         ``attn_l`` / ``attn_r`` / ``bias`` per head -- and the pad is sliced off.  No gradient flows through it."""
+        H, Fo, Fp, w, al, ar, b = self._eval_params(graph)
+        ft = dense.linear(feat, w)                                  # [n, H * Fp]
+        el, er = GatProjection.apply(ft, ft, al, ar, H, Fp)
+        rst = gat_infer(graph.a, ft, el, er, H, Fp, self.negative_slope, b)
+        return rst.view(-1, H, Fp)[..., :Fo]
+
+    def _eval_params(self, graph):
+        """The evaluation forward's checks and its parameters with each head's width padded to a multiple of 4."""
         H, Fo = self._num_heads, self._out_feats
         why = gat_infer_unsupported(H, Fo)
         if why is not None:
@@ -153,7 +169,36 @@ class GATConv(nn.Module):
             w = F.pad(w.view(H, Fo, -1), (0, 0, 0, pad)).reshape(H * Fp, -1)
             al, ar = F.pad(al, (0, pad)), F.pad(ar, (0, pad))
             b = F.pad(b.view(H, Fo), (0, pad)).reshape(-1) if b is not None else None
-        ft = dense.linear(feat, w)                                  # [n, H * Fp]
-        el, er = GatProjection.apply(ft, ft, al, ar, H, Fp)
-        rst = gat_infer(graph.a, ft, el, er, H, Fp, self.negative_slope, b)
-        return rst.view(-1, H, Fp)[..., :Fo]
+        return H, Fo, Fp, w, al, ar, b
+
+    @torch.no_grad()
+    def _forward_partition(self, graph: PartitionEvalGraph, feat) -> torch.Tensor:
+        """``_forward_full_graph`` over this rank's inner rows: the attention of the inner block first, then one block
+        per peer, the online-softmax state carried between them (``gat_infer_block``).  ``feat``: the inner rows (each
+        peer's halo rows are exchanged and transformed one peer at a time), or ``(h_src, h_dst)`` when ``h_src`` already
+        holds ``[inner | every halo row]`` (layer 0 of the precomputed model: ``train.precompute``)."""
+        H, Fo, Fp, w, al, ar, b = self._eval_params(graph)
+        n_in = graph.n_in
+        held = isinstance(feat, tuple)
+        src = feat[0] if held else feat
+        ft = dense.linear(src, w)                                   # [n_in (+ n_halo), H * Fp]
+        el, er = GatProjection.apply(ft, ft[:n_in], al, ar, H, Fp)
+        m = torch.empty(n_in, H, dtype=torch.float32, device=ft.device)
+        l = torch.empty_like(m)
+        acc = torch.empty(n_in, H * Fp, dtype=torch.float32, device=ft.device)
+        live = [j for j in graph.order if graph.blocks[j].nnz]
+        slope = self.negative_slope
+        gat_infer_block(graph.a_in, ft[:n_in], el[:n_in], er, H, Fp, slope, m, l, acc, True, not live, b, acc)
+        if held:
+            for j in live:
+                rows = slice(n_in + graph.halo_begin[j], n_in + graph.halo_begin[j] + graph.halo_count[j])
+                gat_infer_block(graph.blocks[j], ft[rows], el[rows], er, H, Fp, slope, m, l, acc, False, j == live[-1],
+                                b, acc)
+        else:
+            for j, blk, xr in graph.peer_rows(src):
+                if blk.nnz == 0:
+                    continue
+                ft_j = dense.linear(xr, w)
+                el_j, _ = GatProjection.apply(ft_j, ft_j[:0], al, ar, H, Fp)
+                gat_infer_block(blk, ft_j, el_j, er, H, Fp, slope, m, l, acc, False, j == live[-1], b, acc)
+        return acc.view(-1, H, Fp)[..., :Fo]

@@ -6,7 +6,7 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from ..graph import FullGraphHandle, PartitionAggregate, PartitionGraph
+from ..graph import FullGraphHandle, PartitionAggregate, PartitionEvalGraph, PartitionGraph
 from . import dense
 from ..ops import AggregateSum
 
@@ -43,6 +43,8 @@ def _aggregate(graph, feat, rs, cs_u=None):
         return PartitionAggregate.apply(feat, graph, rs, cs_in, cs_halo, getattr(feat, '_bns_ready', None))
     if isinstance(graph, FullGraphHandle):
         return AggregateSum.apply(feat, graph.a, rs, cs_u)
+    if isinstance(graph, PartitionEvalGraph):
+        return graph.aggregate(feat, rs, cs_u)
     raise TypeError(f"unsupported graph handle {type(graph).__name__}")
 
 
@@ -95,6 +97,10 @@ class GCNLayer(nn.Module):
                 return h + self.linear.bias if self.linear.bias is not None else h
             h = _aggregate(graph, feat, graph.recip(in_norm), graph.recip(out_norm))  # :32-38
             return self._lin(self.linear, h)
+        if self.use_pp and isinstance(graph, PartitionEvalGraph):
+            # D_in^-1/2 A D_out^-1/2 x over the whole graph, restricted to the inner rows, IS the precomputed input
+            # this rank holds (train.precompute): nothing to aggregate, nothing to exchange
+            return self._lin(self.linear, feat)
         in_n = torch.sqrt(graph.in_degrees().float())                                # :40-45
         out_n = torch.sqrt(graph.out_degrees().float())
         return self._lin(self.linear, _aggregate(graph, feat, 1.0 / in_n, 1.0 / out_n))
@@ -147,6 +153,10 @@ class GraphSAGELayer(nn.Module):
             ah = _aggregate(graph, feat, graph.recip(in_norm))                       # :85-91  (sum / degs)
             return dense.linear(feat[0:num_dst], self.linear1.weight, self.linear1.bias,
                                 addend=self._lin(self.linear2, ah))                  # :92, "+" fused into the epilogue
+        if self.use_pp and isinstance(graph, PartitionEvalGraph):
+            # [x | mean over the whole graph's in-neighbours] of the inner rows IS the precomputed input this rank
+            # holds (train.precompute / precompute_streaming): nothing to aggregate, nothing to exchange
+            return self._lin(self.linear, feat)
         degs = graph.in_degrees()                                                    # :94-102
         ah = _aggregate(graph, feat, 1.0 / degs.float())
         if self.use_pp:

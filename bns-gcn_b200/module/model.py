@@ -6,6 +6,7 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import ops
+from ..graph import PartitionEvalGraph
 from ..helper import context as ctx
 from .layer import GCNLayer, GraphSAGELayer
 
@@ -143,7 +144,10 @@ class GAT(GNNBase):
             if i >= self.n_conv:
                 h = layer(self.dropout(h))
             elif not self.training:
-                h = layer(g, h).mean(1)
+                if i == 0 and self.use_pp and isinstance(g, PartitionEvalGraph):
+                    h = layer(g, (h, h[0:g.n_in])).mean(1)          # layer 0 holds every halo row (train.precompute)
+                else:
+                    h = layer(g, h).mean(1)
             else:
                 if i == 0 and self.use_pp:
                     src, dst = h, h[0:g.num_nodes('_V')]                # :120-121: layer 0 holds the stored halo rows

@@ -204,14 +204,14 @@ def make_col_blocks(g: DeviceGraph, n_blocks: int, chunk_nnz: int = 0):
 
 
 def spmm_auto(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *, row_scale=None,
-              n_out_rows: Optional[int] = None, accumulate: bool = False) -> torch.Tensor:
+              n_out_rows: Optional[int] = None, accumulate: bool = False, col_scale=None) -> torch.Tensor:
     """``spmm`` of a plain matrix (no maps, no weights), source-row blocked when ``plan_col_blocks`` says so: one pass
     per block, each accumulating into ``out``.  Counts as ONE launch in bench.py's roofline bookkeeping."""
     global PROFILE
     F = x.shape[1]
     nb = plan_col_blocks(g, F)
     if nb <= 1:
-        return spmm(g, x, out, row_scale=row_scale, n_out_rows=n_out_rows, accumulate=accumulate)
+        return spmm(g, x, out, row_scale=row_scale, n_out_rows=n_out_rows, accumulate=accumulate, col_scale=col_scale)
     blocks = g.__dict__.get("_col_blocks")
     if blocks is None or len(blocks) != nb:
         blocks = g._col_blocks = make_col_blocks(g, nb)
@@ -223,7 +223,8 @@ def spmm_auto(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = Non
             ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             ev0.record(torch.cuda.current_stream(x.device))
         for i, (gb, c0, c1) in enumerate(blocks):
-            spmm(gb, x[c0:c1], out, row_scale=row_scale, accumulate=accumulate or i > 0)
+            spmm(gb, x[c0:c1], out, row_scale=row_scale, accumulate=accumulate or i > 0,
+                 col_scale=None if col_scale is None else col_scale[c0:c1])
         if prof is not None:
             ev1.record(torch.cuda.current_stream(x.device))
             alg = 8 * (g.n_rows + 1) + 4 * g.nnz + 4 * F * x.shape[0] + 4 * F * out.shape[0]

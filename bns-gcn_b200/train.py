@@ -573,22 +573,43 @@ class GraphedEpoch:
         return self.loss
 
 
+def _gat_eval_unsupported(model) -> Optional[str]:
+    """The GAT evaluation forward runs on bns_gat_infer_f32 / bns_gat_infer_block_f32: ``None`` when every attention
+    layer fits them, else the first limit a layer exceeds."""
+    from .graph import gat_infer_unsupported
+    from .module.gat import GATConv
+    return next((w for w in (gat_infer_unsupported(m._num_heads, m._out_feats) for m in model.layers
+                             if isinstance(m, GATConv)) if w is not None), None)
+
+
 def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     """train.py:300-456.  With ``args.eval`` rank 0 also runs the evaluation / checkpoint branch (:308-321, 427-456)
     through ``evaluate.Evaluator`` -- on the GPU with the same kernels, synchronously, instead of a CPU thread pool;
-    ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: regenerated from ``args.dataset``)."""
+    ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: regenerated from ``args.dataset``).
+    With ``args.parallel_eval`` as well, EVERY rank evaluates its own nodes on its partition instead
+    (``evaluate.ParallelEvaluator``) and the full graph is never built; inductive runs are refused."""
     rank, size = _rank_size()
+    parallel = getattr(args, 'eval', False) and getattr(args, 'parallel_eval', False)
+    if parallel and args.inductive:
+        raise ValueError("--parallel-eval: inductive runs evaluate on the train | val subgraph and the full graph, "
+                         "which the training partitions do not hold; drop --parallel-eval to evaluate them on rank 0")
     st = setup(graph, node_dict, gpb, args, device)
     dev = st.feat.device
     evaluator = None
-    if getattr(args, 'eval', False) and rank == 0:
-        why = None
-        if args.model == 'gat':
-            # the full-graph GAT forward runs on bns_gat_infer_f32: decide now whether every attention layer fits it
-            from .graph import gat_infer_unsupported
-            from .module.gat import GATConv
-            why = next((w for w in (gat_infer_unsupported(m._num_heads, m._out_feats) for m in st.model.layers
-                                    if isinstance(m, GATConv)) if w is not None), None)
+    if parallel:
+        why = _gat_eval_unsupported(st.model) if args.model == 'gat' else None
+        if why is not None:
+            if rank == 0:
+                import warnings
+                warnings.warn(f'--eval: the GAT evaluation forward does not take this model ({why}); '
+                              'training runs without the evaluation branch')
+        else:
+            from .evaluate import ParallelEvaluator, build_partition_eval_graph
+            eg = build_partition_eval_graph(st.part, node_dict, st.boundary, ctx.comm())
+            evaluator = ParallelEvaluator(args, eg, st.feat, st.labels, node_dict['val_mask'].to(dev),
+                                          node_dict['test_mask'].to(dev), ctx.comm())
+    elif getattr(args, 'eval', False) and rank == 0:
+        why = _gat_eval_unsupported(st.model) if args.model == 'gat' else None
         if why is not None:
             import warnings
             warnings.warn(f'--eval: the full-graph GAT evaluation forward does not take this model ({why}); '

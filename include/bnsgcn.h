@@ -368,6 +368,19 @@ int bns_gat_colsum_f32(const bns_graph_t *gT, const float *dE, int32_t heads, co
  * A row without entries gets the bias alone.  Deterministic: the summation order is fixed per row. */
 int bns_gat_infer_f32(const bns_graph_t *g, const float *ft, int64_t ldft, int32_t heads, int32_t Fp, const float *el,
                       const float *er, float negative_slope, const float *bias, float *rst, int64_t ldr, void *stream);
+/* bns_gat_infer_f32 over destination rows whose in-entries come as several matrices with the same rows and different
+ * columns (a partition's inner matrix, then one column block per peer's halo rows): one call per block, g / ft / el
+ * that block's, er the rows' own.  The online-softmax state is carried between calls, per row and head:
+ * m [n_rows, heads] running maximum, l [n_rows, heads] sum of exp, acc [n_rows, heads * Fp] (rows ldacc floats apart,
+ * 16-byte aligned) the un-normalised weighted sum.  `first` starts from the empty state (m, l, acc need not be
+ * initialised); otherwise the call reloads it and rescales it when the maximum grows.  `last` writes
+ * rst = acc / l + bias (rst may be acc itself, with ldr == ldacc; ft / el may be NULL for a block without entries);
+ * otherwise the state is
+ * stored.  A row without entries in a block keeps its state; a row without entries in any block gets the bias alone.
+ * Same limits as bns_gat_infer_f32.  Deterministic for a fixed block order. */
+int bns_gat_infer_block_f32(const bns_graph_t *g, const float *ft, int64_t ldft, int32_t heads, int32_t Fp,
+                            const float *el, const float *er, float negative_slope, float *m, float *l, float *acc,
+                            int64_t ldacc, int first, int last, const float *bias, float *rst, int64_t ldr, void *stream);
 int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                           const float *weights, int64_t ldw, int perm_from_transpose, const int32_t *row_map, int64_t x_rows,
                           int accumulate, void *ws, size_t ws_bytes, void *stream);
