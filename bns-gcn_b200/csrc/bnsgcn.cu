@@ -1359,6 +1359,9 @@ extern "C" int bns_ln_relu_dropout_fwd_f32(const float *x, int64_t ldx, int64_t 
     BNS_REQUIRE(x && y && gamma && beta && mean && rstd, "bns_ln_relu_dropout_fwd_f32: NULL pointer");
     BNS_REQUIRE(ldx % 4 == 0 && ldy % 4 == 0 && ldx >= F && ldy >= F, "bns_ln_relu_dropout_fwd_f32: bad leading dimension");
     BNS_REQUIRE(p >= 0.f && p < 1.f, "bns_ln_relu_dropout_fwd_f32: p must be in [0, 1)");
+    BNS_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(gamma) |
+                  reinterpret_cast<uintptr_t>(beta)) & 15u) == 0,
+                "bns_ln_relu_dropout_fwd_f32: x, y, gamma and beta must be 16-byte aligned");
     LnArgs a{};
     a.x = x; a.ldx = ldx; a.y = y; a.ldy = ldy; a.gamma = gamma; a.beta = beta; a.mean = mean; a.rstd = rstd;
     a.n = n; a.F = (int32_t)F; a.eps = eps; a.p = p; a.keep_scale = 1.f / (1.f - p);
@@ -1376,7 +1379,12 @@ extern "C" int bns_ln_relu_dropout_bwd_f32(const float *dy, int64_t lddy, const 
                                            void *stream) {
     BNS_REQUIRE(n >= 0 && F > 0 && F % 4 == 0 && F <= kLnMaxNV * 128, "bns_ln_relu_dropout_bwd_f32: need F %% 4 == 0, F <= 1024");
     BNS_REQUIRE(dy && x && dx && gamma && beta && mean && rstd && dgamma && dbeta, "bns_ln_relu_dropout_bwd_f32: NULL pointer");
-    BNS_REQUIRE(ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0, "bns_ln_relu_dropout_bwd_f32: bad leading dimension");
+    BNS_REQUIRE(ldx % 4 == 0 && lddy % 4 == 0 && lddx % 4 == 0 && ldx >= F && lddy >= F && lddx >= F,
+                "bns_ln_relu_dropout_bwd_f32: bad leading dimension");
+    BNS_REQUIRE(p >= 0.f && p < 1.f, "bns_ln_relu_dropout_bwd_f32: p must be in [0, 1)");
+    BNS_REQUIRE(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dx) |
+                  reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15u) == 0,
+                "bns_ln_relu_dropout_bwd_f32: dy, x, dx, gamma and beta must be 16-byte aligned");
     const unsigned grid = ln_grid(n > 0 ? n : 1);
     if (!ws || ws_bytes < (size_t)grid * 2 * F * sizeof(float))
         return fail(BNS_E_WORKSPACE, "bns_ln_relu_dropout_bwd_f32: workspace too small");

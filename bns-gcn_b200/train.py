@@ -527,8 +527,10 @@ class GraphedEpoch:
     bound by the time the host needs to enqueue ~300 launches; a replay costs one.
 
     What changes between replays is read from device memory, not baked into kernel arguments: the Philox offset of
-    the sampler and the flag sequence number of the p2p exchange both come from ``st.epoch_dev``; dropout uses
-    torch's graph-safe Philox state.  Sizes (sample counts, slab rows) are fixed for the run (train.py:344-345).
+    the sampler and the flag sequence number of the p2p exchange both come from ``st.epoch_dev``, and so does the
+    offset of the fused step's dropout masks (``ops.RNG["offset_dev"]``: LayerNorm -> ReLU -> dropout and layer 0's
+    input dropout draw their Philox counters from ``2**64 - 1 + epoch_dev``, i.e. the epoch index; ``nn.Dropout`` of
+    the op-by-op path uses torch's graph-safe Philox state).  Sizes (sample counts, slab rows) are fixed for the run (train.py:344-345).
     """
 
     def __init__(self, st: TrainState, warmup: int = 3):

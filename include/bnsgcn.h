@@ -217,7 +217,8 @@ int bns_halo_slot_update(const int64_t *pos /*device [part size of the peer]*/, 
  *     y = dropout_p( relu( (x - mean) * rstd * gamma + beta ) )        mean / biased var over the F columns
  * The dropout mask is Philox4x32-10(counter = (row, vector, offset), key = seed) -- regenerated, not stored, in
  * backward; offset_dev (optional, device) is added to offset at run time (CUDA-graph replays).  F % 4 == 0,
- * F <= 1024.  Backward also returns dgamma / dbeta (column sums, fixed summation order: deterministic);
+ * F <= 1024, 0 <= p < 1, leading dimensions >= F and multiples of 4, x / y / dy / dx / gamma / beta 16-byte
+ * aligned (they are read and written as float4).  Backward also returns dgamma / dbeta (column sums, fixed summation order: deterministic);
  * ws: bns_ln_bwd_workspace_bytes(F) bytes.
  * ----------------------------------------------------------------------------------------------*/
 size_t bns_ln_bwd_workspace_bytes(int64_t F);

@@ -26,7 +26,8 @@ def _launch(world: int, extra, port: int, log_dir, timeout: int = 600):
     env = dict(os.environ)
     env.pop("CUDA_VISIBLE_DEVICES", None)
     p = subprocess.run(cmd, cwd=ROOT, env=env, capture_output=True, text=True, timeout=timeout)
-    tag = f"w{world}_{'graph' if '--graph' in extra else 'eager'}{'_abi' if 'abi' in extra else ''}"
+    tag = (f"w{world}_{'graph' if '--graph' in extra else 'eager'}{'_abi' if 'abi' in extra else ''}"
+           f"{'_dropout' if '--dropout' in extra else ''}")
     with open(os.path.join(log_dir, f"dist_check_{tag}.log"), "w") as f:      # kept for the post-mortem of a failure
         f.write(p.stdout[-20000:] + "\n---- stderr ----\n" + p.stderr[-20000:])
     line = None
@@ -49,6 +50,20 @@ def test_one_process_per_gpu_matches_in_process_run(built, tmp_path, world, grap
         assert line[backend]["max_rel_err_vs_inprocess"] < 1e-5, line
         assert line[backend]["loss_rel_err"] < 1e-5, line
     print("[multiprocess]", json.dumps(line))
+
+
+def test_replayed_epochs_with_dropout_match_in_process_run(built, tmp_path):
+    """World 2 replayed from a CUDA graph at dropout 0.5: every replay's masks take the epoch from the device counter
+    (offset 2**64 - 1 + epoch_dev) and must equal those of the eager in-process run."""
+    if torch.cuda.device_count() < 2:
+        pytest.skip(f"needs 2 GPUs, this box has {torch.cuda.device_count()}")
+    extra = ["--shape", "small", "--rate", "0.3", "--hidden", "64", "--epochs", "4", "--graph", "--dropout", "0.5"]
+    p, line = _launch(2, extra, 29680, tmp_path)
+    assert p.returncode == 0 and line is not None, (p.stdout[-3000:], p.stderr[-3000:])
+    assert line["ok"] and line["world"] == 2, line
+    for backend in ("nccl", "p2p"):
+        assert line[backend]["max_rel_err_vs_inprocess"] < 1e-5, line
+        assert line[backend]["loss_rel_err"] < 1e-5, line
 
 
 @pytest.mark.parametrize("world", [2, 8])

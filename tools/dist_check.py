@@ -1,7 +1,7 @@
 """Multi-process / multi-GPU check of the exchange transports (run under torchrun, one rank per GPU):
 
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 \
-      tools/dist_check.py [--shape small] [--rate 0.3]
+      tools/dist_check.py [--shape small] [--rate 0.3] [--graph] [--dropout 0.5]
 
 Every rank trains a few epochs of the same seeded configuration with backend=nccl and backend=p2p (real NCCL
 send/recv, real cudaIpc peer mappings over NVLink) and rank 0 compares the result -- loss, all-reduced weight
@@ -25,9 +25,9 @@ from bns_gcn_b200.helper.comm import run_threads  # noqa: E402
 from bns_gcn_b200.helper.timer.timer import comm_timer  # noqa: E402
 
 
-def mk_args(shape, rate, backend, hidden, P):
+def mk_args(shape, rate, backend, hidden, P, dropout=0.0):
     return argparse.Namespace(dataset=shape, model="graphsage", n_layers=3, n_hidden=hidden, sampling_rate=rate,
-                              use_pp=True, dropout=0.0, norm="layer", lr=1e-2, weight_decay=0.0, seed=0, n_linear=0,
+                              use_pp=True, dropout=dropout, norm="layer", lr=1e-2, weight_decay=0.0, seed=0, n_linear=0,
                               backend=backend, sampler_seed=0, n_epochs=0, log_every=10 ** 9, heads=1, n_partitions=P,
                               inductive=False, partition_method="random", eval=False, chunk_nnz=0)
 
@@ -58,6 +58,8 @@ def main():
     ap.add_argument("--hidden", type=int, default=64)
     ap.add_argument("--epochs", type=int, default=3)
     ap.add_argument("--graph", action="store_true", help="run the distributed side from a captured CUDA graph")
+    ap.add_argument("--dropout", type=float, default=0.0,
+                    help="dropout rate of the model (the replayed masks must equal the eager ones)")
     ap.add_argument("--comm", default="torch", choices=["torch", "abi"],
                     help="abi: all-reduce / all-to-all through libbnsgcn.so's own communicator (bns_ctx_create ...)")
     a = ap.parse_args()
@@ -74,7 +76,7 @@ def main():
     backends = ("p2p",) if (a.graph and world > 2) else ("nccl", "p2p")
     for backend in backends:
         ctx.reset()
-        out = train_rank(parts[rank], mk_args(a.shape, a.rate, backend, a.hidden, world), dev, a.epochs, a.graph)
+        out = train_rank(parts[rank], mk_args(a.shape, a.rate, backend, a.hidden, world, a.dropout), dev, a.epochs, a.graph)
         tot = torch.tensor(out["loss"], dtype=torch.float64, device=dev)
         dist.all_reduce(tot)
         out["loss_sum"] = tot.tolist()
@@ -83,7 +85,7 @@ def main():
     ok, report = True, {}
     if rank == 0:
         ctx.reset()
-        ref = run_threads(world, lambda c, r: train_rank(parts[r], mk_args(a.shape, a.rate, "nccl", a.hidden, world), dev,
+        ref = run_threads(world, lambda c, r: train_rank(parts[r], mk_args(a.shape, a.rate, "nccl", a.hidden, world, a.dropout), dev,
                                                          a.epochs), device=str(dev))
         ref_loss = [sum(ref[r]["loss"][e] for r in range(world)) for e in range(a.epochs)]
         for backend in backends:
