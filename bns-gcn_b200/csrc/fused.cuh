@@ -121,7 +121,8 @@ extern "C" int bns_xent_f32(const float *logits, int64_t ld, int64_t n_rows, int
                             const float *labels_f, int64_t ldl, const uint8_t *mask, float grad_scale, float *loss_out,
                             float *dlogits, int64_t ldd, int32_t n_cols_out, void *ws, size_t ws_bytes, void *stream) {
     BNS_REQUIRE(n_rows >= 0 && n_class > 0 && n_cols_out >= n_class, "bns_xent_f32: bad shape");
-    BNS_REQUIRE(logits && loss_out && dlogits && (labels || labels_f), "bns_xent_f32: NULL pointer");
+    // no rows: the matrices may be empty allocations (NULL); the loss is still written (0)
+    BNS_REQUIRE(loss_out && (n_rows == 0 || (logits && dlogits && (labels || labels_f))), "bns_xent_f32: NULL pointer");
     BNS_REQUIRE(ld >= n_class && ldd >= n_cols_out && (!labels_f || ldl >= n_class), "bns_xent_f32: bad leading dimension");
     BNS_REQUIRE(!(labels && labels_f), "bns_xent_f32: give class indices OR per-class targets");
     unsigned grid = xent_grid(n_rows);
