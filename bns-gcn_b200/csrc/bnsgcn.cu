@@ -1608,6 +1608,7 @@ extern "C" int bns_halo_slot_update(const int64_t *pos, const int64_t *one_hops,
 // =================================================================================================
 struct bns_p2p {
     int32_t rank = 0, world = 0, n_flags = 0;
+    int32_t n_tickets = 0;                // completion counters behind the flags: world + max(n_flags, 16)
     size_t slab_bytes = 0;
     char *slab = nullptr;                 // this rank's receive slab
     unsigned long long *flags = nullptr;  // this rank's flag block
@@ -1702,9 +1703,11 @@ extern "C" int bns_p2p_create(bns_p2p_t **out, int32_t rank, int32_t world, size
     p->peer_flags = new unsigned long long *[world]();
     p->peer_slab_bytes = new size_t[world]();
     p->imported = new bool[world]();
-    // flags block: n_flags u64 + u32 completion tickets (one per peer for bns_p2p_put_rows_f32, 16 more for the
-    // all-peer puts), zero-initialised
-    const size_t flag_bytes = align256((size_t)n_flags * 8) + align256((size_t)(world + 16) * 4);
+    // flags block: n_flags u64 + u32 completion tickets (one per peer for bns_p2p_put_rows_f32, then one per flag --
+    // at least 16 -- for the all-peer puts, so that every exchange a flag block can signal has a ticket of its own),
+    // zero-initialised
+    p->n_tickets = world + (n_flags > 16 ? n_flags : 16);
+    const size_t flag_bytes = align256((size_t)n_flags * 8) + align256((size_t)p->n_tickets * 4);
     if (cudaMalloc(&p->slab, p->slab_bytes) != cudaSuccess || cudaMalloc(&p->flags, flag_bytes) != cudaSuccess) {
         int rc = fail(BNS_E_CUDA, "bns_p2p_create: cudaMalloc failed: %s", cudaGetErrorString(cudaGetLastError()));
         bns_p2p_destroy(p);

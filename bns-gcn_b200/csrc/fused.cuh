@@ -533,11 +533,12 @@ extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_
     BNS_REQUIRE(p && segs, "bns_p2p_put_all_f32: NULL argument");
     BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "bns_p2p_put_all_f32: too many segments");
     BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "bns_p2p_put_all_f32: bad flag index");
-    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->world + 16, "bns_p2p_put_all_f32: bad ticket index");
+    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "bns_p2p_put_all_f32: bad ticket index");
     BNS_REQUIRE(F > 0 && ldh >= F && ld_remote >= F, "bns_p2p_put_all_f32: bad shape");
     if (segs->n_seg == 0) return BNS_OK;
     PutAllDev a;
     a.n_seg = segs->n_seg;
+    // the 16-byte path also needs every destination 16-byte aligned; the scalar path takes rows of any width
     bool vec = F % 4 == 0 && ldh % 4 == 0 && ld_remote % 4 == 0 && (reinterpret_cast<uintptr_t>(H) & 15u) == 0;
     for (int s = 0; s <= segs->n_seg; ++s) a.row_begin[s] = segs->row_begin[s];
     for (int s = 0; s < segs->n_seg; ++s) {
@@ -547,9 +548,10 @@ extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_
         BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "bns_p2p_put_all_f32: peer %d not connected", peer);
         BNS_REQUIRE(k >= 0, "bns_p2p_put_all_f32: negative row count");
         BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "bns_p2p_put_all_f32: division by zero");
-        BNS_REQUIRE(segs->remote_off[s] % 16 == 0 &&
+        BNS_REQUIRE(segs->remote_off[s] % 4 == 0 &&
                         segs->remote_off[s] + (size_t)k * ld_remote * 4 <= p->peer_slab_bytes[peer],
                     "bns_p2p_put_all_f32: remote range of segment %d outside peer %d's slab", s, peer);
+        vec = vec && segs->remote_off[s] % 16 == 0;
         a.remote[s] = reinterpret_cast<float *>(p->peer_slab[peer] + segs->remote_off[s]);
         a.flag[s] = p->peer_flags[peer] + flag_index;
         a.src_begin[s] = segs->src_begin[s];
@@ -574,7 +576,7 @@ extern "C" int bns_p2p_put_ids_i64(bns_p2p_t *p, int32_t n_seg, const int64_t *b
     BNS_REQUIRE(p && begin && peers && remote_off, "bns_p2p_put_ids_i64: NULL argument");
     BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "bns_p2p_put_ids_i64: too many segments");
     BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "bns_p2p_put_ids_i64: bad flag index");
-    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->world + 16, "bns_p2p_put_ids_i64: bad ticket index");
+    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "bns_p2p_put_ids_i64: bad ticket index");
     if (n_seg == 0) return BNS_OK;
     PutIdsDev a;
     a.n_seg = n_seg;

@@ -134,6 +134,8 @@ class Buffer(object):
         slab_bytes = self._ids_off + max(tot, 1) * 8
         self._n_comm_layers = n_comm_layers
         n_flags = (n_comm_layers * 2 + 1) * self._size          # (layer, direction, source) + (ids, source)
+        # completion tickets of the all-peer puts: size + 2 (layer - 1) forward, + 1 backward, size + 2 n_comm_layers
+        # the ids -- all below size + n_flags, which the library provides for any depth
         h = ctypes.c_void_p()
         with torch.cuda.device(self._device):
             check(lib.bns_p2p_create(ctypes.byref(h), self._rank, self._size, slab_bytes, n_flags), "bns_p2p_create")
@@ -205,7 +207,8 @@ class Buffer(object):
         cs.wait_event(start)
         with torch.cuda.stream(cs):
             check(lib.bns_p2p_put_ids_i64(self._p2p, n, begin, peers, roff, sel_cat.data_ptr() if tot else None,
-                                          flag_base + self._rank, self._size + 15, seq, seq_dev, cs.cuda_stream),
+                                          flag_base + self._rank, self._size + 2 * self._n_comm_layers, seq, seq_dev,
+                                          cs.cuda_stream),
                   "bns_p2p_put_ids_i64")
             for j in self._peers:
                 self._post_put_event(j, 1999, cs)

@@ -390,9 +390,11 @@ int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64_t ldx, int
  * C1/C2 + K3/K5 for ALL peers at once (helper/feature_buffer.py:101-129).
  * bns_p2p_put_all_f32: segment s sends rows [row_begin[s], row_begin[s+1]) of the concatenated send list to peer[s]:
  *     remote_s[i, :F] = H[idx_cat[row_begin[s] + i], :F] / div[s]      (idx_cat == NULL: H[src_begin[s] + i, :F])
- * into the peer's slab at byte offset remote_off[s]; after the last row of the LAUNCH every peer's flags[flag_index]
- * is set to flag_value (+ *flag_value_dev) with a system-scope release.  ticket_index < world + 16 picks the completion
- * counter; launches that share one must be stream-ordered.
+ * into the peer's slab at byte offset remote_off[s] (a multiple of 4; rows of any F, the 16-byte path is taken when
+ * every remote_off is a multiple of 16 and F, ldh, ld_remote are multiples of 4); after the last row of the LAUNCH
+ * every peer's flags[flag_index] is set to flag_value (+ *flag_value_dev) with a system-scope release.
+ * ticket_index < world + max(n_flags, 16) (n_flags of bns_p2p_create) picks the completion counter; launches that
+ * share one must be stream-ordered.
  * bns_p2p_put_ids_i64: the same for the sampled id lists (data_transfer(..., tag=NODE), helper/utils.py:187-213).
  * bns_p2p_wait_all: one kernel that waits for n flags of this rank (bounded spin, 20 s -> trap).
  * bns_scatter_rows_all_f32: G[r, :] += recv_s[inv_s[r], :] / div[s] for every segment s IN ORDER and every row r with
