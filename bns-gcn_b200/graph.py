@@ -12,8 +12,6 @@ from __future__ import annotations
 
 from typing import Dict, Optional
 
-import os
-
 import torch
 
 from . import ops
@@ -236,60 +234,6 @@ class PartitionAggregate(torch.autograd.Function):
         return du, None, None, None, None, None
 
 
-def _entry_rows(a: ops.DeviceGraph):
-    """(row id, column id) of every CSR entry of ``a`` as int64 vectors (static, built once)."""
-    indptr, indices = a.csr()
-    rows = torch.repeat_interleave(torch.arange(a.n_rows, device=indptr.device), indptr[1:] - indptr[:-1])
-    return rows, indices.long()
-
-
-def gat_entries(g: PartitionGraph):
-    """Static per-entry index vectors the attention scores are computed on (rows / cols of a_in and a_out)."""
-    if getattr(g, "_gat_entries", None) is None:
-        rin, cin = _entry_rows(g.a_in)
-        if g.a_out is not None:
-            rout, cout = _entry_rows(g.a_out)
-        else:
-            rout = cout = torch.empty(0, dtype=torch.int64, device=g.device)
-        g._gat_entries = (rin, cin, rout, cout)
-    return g._gat_entries
-
-
-class WeightedAggregate(torch.autograd.Function):
-    """``rst[v] = sum_k w_k * ft_u[xrow(c_k)]`` over the inner entries (weights ``w_in``) and the sampled halo entries
-    (``w_out``; unsampled entries are skipped through the slot map) -- DGL's ``update_all(u_mul_e, sum)`` of GATConv.
-    Backward: ``d ft = A_w^T d rst`` (weights carried to the transposes by their entry permutation) and
-    ``d w_k = <d rst[v], ft_u[xrow(c_k)]>`` (``bns_sddmm_dot_f32``)."""
-
-    @staticmethod
-    def forward(ctx, ft_u, w_in, w_out, g: PartitionGraph):
-        ft_u, w_in, w_out = ft_u.contiguous(), w_in.contiguous(), w_out.contiguous()
-        ctx.g = g
-        ctx.save_for_backward(ft_u, w_in, w_out)
-        y = ops.spmm(g.a_in, ft_u, edge_weight=w_in)
-        if g.a_out is not None and ft_u.shape[0] > g.n_in:
-            ops.spmm(g.a_out, ft_u[g.n_in:], y, edge_weight=w_out, col_map=g.slot, n_direct=0, accumulate=True)
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        g = ctx.g
-        ft_u, w_in, w_out = ctx.saved_tensors
-        dy = dy.contiguous()
-        n_u, n_in = ft_u.shape[0], g.n_in
-        d_ft = torch.empty_like(ft_u)
-        ops.spmm(g.a_in_t, dy, d_ft[:n_in], edge_weight=w_in[g.a_in_t.perm().long()])
-        d_w_in = ops.sddmm_dot(g.a_in, dy, ft_u)
-        d_w_out = torch.zeros_like(w_out)
-        if n_u > n_in:
-            tail = d_ft[n_in:]
-            tail.zero_()
-            if g.a_out_t is not None:
-                ops.spmm(g.a_out_t, dy, tail, edge_weight=w_out[g.a_out_t.perm().long()], row_map=g.slot)
-                ops.sddmm_dot(g.a_out, dy, ft_u[n_in:], col_map=g.slot, n_direct=0, out=d_w_out)
-        return d_ft, d_w_in, d_w_out, None
-
-
 _PROJ_WS = {}
 
 
@@ -340,13 +284,6 @@ class GatProjection(torch.autograd.Function):
         return outs[0][0], outs[1][0], outs[0][1], outs[1][1], None, None
 
 
-def gat_attention_supported(H: int, Fo: int) -> bool:
-    """Whether ``GatAttention`` takes ``H`` heads of width ``Fo``: exactly what ``bns_gat_forward_f32`` and
-    ``bns_gat_backward_f32`` accept -- 1..8 heads, a positive per-head width that is a multiple of 4 (16-byte lanes),
-    at most 1024 columns in all."""
-    return 1 <= H <= 8 and Fo > 0 and Fo % 4 == 0 and H * Fo <= 1024
-
-
 class GatAttention(torch.autograd.Function):
     """The attention of ``dgl.nn.GATConv`` for all heads:
 
@@ -357,9 +294,7 @@ class GatAttention(torch.autograd.Function):
 
     Stages (include/bnsgcn.h): ``bns_gat_scores_f32`` (scalars: probabilities + dropped attention per entry) ->
     ``bns_spmm_weighted_f32`` / ``bns_spmm_compact_f32`` per head; backward ``bns_sddmm_dot_f32`` ->
-    ``bns_gat_softmax_bwd_f32`` -> ``bns_gat_colsum_f32`` -> ``bns_spmm_weighted_f32`` on the transposes.  The one-launch
-    row walks ``bns_gat_forward_f32`` / ``bns_gat_backward_f32`` compute the same thing (``BNS_GAT_ROWWALK=1``; the
-    tests run both) but are a latency chain per row on low-degree graphs."""
+    ``bns_gat_softmax_bwd_f32`` -> ``bns_gat_colsum_f32`` -> ``bns_spmm_weighted_f32`` on the transposes."""
 
     @staticmethod
     def forward(ctx, ft, el, er, g: PartitionGraph, H: int, Fo: int, slope: float, p: float, seed: int):
@@ -367,37 +302,32 @@ class GatAttention(torch.autograd.Function):
         ft, el, er = ft.contiguous(), el.contiguous(), er.contiguous()
         n_in, dev = g.n_in, ft.device
         c = g.compact if (g.a_out is not None and ft.shape[0] > n_in) else None
+        if c is None and g.a_out is not None and g.a_out.nnz and ft.shape[0] > n_in:
+            raise RuntimeError("GatAttention: halo rows were passed but the partition graph has no compaction "
+                               "(refresh_compaction)")
         if c is not None and c.cpos is None:
             raise RuntimeError("GatAttention: the partition graph was compacted without positions (want_positions)")
         rst = torch.empty(n_in, H * Fo, dtype=torch.float32, device=dev)
         p_in = torch.empty(max(g.a_in.nnz, 1), H, dtype=torch.float32, device=dev)
         p_out = torch.empty(max(g.a_out.nnz, 1), H, dtype=torch.float32, device=dev) if c is not None else None
+        w_in = torch.empty_like(p_in) if p > 0 else None
+        w_out = torch.empty_like(p_out) if p > 0 and p_out is not None else None
+        wc = torch.empty_like(p_out) if p_out is not None else None              # halo attention, compacted positions
         off, off_dev = ops.RNG["offset"], ops.RNG["offset_dev"]
         head = (g.a_in._h, None if c is None else g.a_out._h, None if c is None else c.cidx.data_ptr(),
                 None if c is None else c.chunk_cnt.data_ptr(), None if c is None else c.cpos.data_ptr(), n_in)
         tail = (H, el.data_ptr(), er.data_ptr(), float(slope), float(p), seed & (2 ** 64 - 1), off & (2 ** 64 - 1),
                 ops._ptr(off_dev))
-        rowwalk = os.environ.get("BNS_GAT_ROWWALK", "0") == "1"
         st = torch.cuda.current_stream(dev).cuda_stream
-        w_in = w_out = None
-        if rowwalk:
-            with torch.cuda.device(dev):
-                check(lib.bns_gat_forward_f32(*head, ft.data_ptr(), ft.stride(0), H, Fo, *tail[1:], rst.data_ptr(),
-                                              rst.stride(0), p_in.data_ptr(), ops._ptr(p_out), st), "bns_gat_forward_f32")
-        else:
-            if p > 0:
-                w_in = torch.empty_like(p_in)
-                w_out = torch.empty_like(p_out) if p_out is not None else None
-            wc = torch.empty_like(p_out) if p_out is not None else None          # halo attention, compacted positions
-            with torch.cuda.device(dev):
-                check(lib.bns_gat_scores_f32(*head, *tail, p_in.data_ptr(), ops._ptr(p_out), ops._ptr(w_in), ops._ptr(w_out),
-                                             ops._ptr(wc), st), "bns_gat_scores_f32")
-            for h in range(H):
-                cols = slice(h * Fo, (h + 1) * Fo)
-                ops.spmm_weighted(g.a_in, ft[:n_in, cols], rst[:, cols], p_in if w_in is None else w_in, h)
-                if c is not None:
-                    ops.spmm_compact(c, ft[n_in:, cols], rst[:, cols], accumulate=True, weights=wc, head=h)
-        ctx.g, ctx.c, ctx.head, ctx.tail, ctx.cfg, ctx.rowwalk = g, c, head, tail, (H, Fo, float(p)), rowwalk
+        with torch.cuda.device(dev):
+            check(lib.bns_gat_scores_f32(*head, *tail, p_in.data_ptr(), ops._ptr(p_out), ops._ptr(w_in), ops._ptr(w_out),
+                                         ops._ptr(wc), st), "bns_gat_scores_f32")
+        for h in range(H):
+            cols = slice(h * Fo, (h + 1) * Fo)
+            ops.spmm_weighted(g.a_in, ft[:n_in, cols], rst[:, cols], p_in if w_in is None else w_in, h)
+            if c is not None:
+                ops.spmm_compact(c, ft[n_in:, cols], rst[:, cols], accumulate=True, weights=wc, head=h)
+        ctx.g, ctx.c, ctx.head, ctx.tail, ctx.cfg = g, c, head, tail, (H, Fo)
         saved = [ft, el, er, p_in] + ([p_out] if p_out is not None else [])
         if w_in is not None:
             saved += [w_in] + ([w_out] if w_out is not None else [])
@@ -409,7 +339,7 @@ class GatAttention(torch.autograd.Function):
     def backward(ctx, d_rst):
         from ._lib import check, lib
         g, c = ctx.g, ctx.c
-        H, Fo, p = ctx.cfg
+        H, Fo = ctx.cfg
         ft, el, er, p_in, *rest = ctx.saved_tensors
         p_out = rest.pop(0) if c is not None else None
         d_rst = d_rst.contiguous()
@@ -418,28 +348,18 @@ class GatAttention(torch.autograd.Function):
         de_out = torch.empty_like(p_out) if p_out is not None else None
         d_er = torch.empty(n_in, H, dtype=torch.float32, device=dev)
         st = torch.cuda.current_stream(dev).cuda_stream
-        if ctx.rowwalk:
-            a_in = torch.empty_like(p_in) if p > 0 else None
-            a_out = torch.empty_like(p_out) if (p > 0 and p_out is not None) else None
-            with torch.cuda.device(dev):
-                check(lib.bns_gat_backward_f32(*ctx.head, ft.data_ptr(), ft.stride(0), H, Fo, *ctx.tail[1:], d_rst.data_ptr(),
-                                               d_rst.stride(0), p_in.data_ptr(), ops._ptr(p_out), de_in.data_ptr(),
-                                               ops._ptr(de_out), ops._ptr(a_in), ops._ptr(a_out), d_er.data_ptr(), st),
-                      "bns_gat_backward_f32")
-            w_in, w_out = (a_in, a_out) if p > 0 else (p_in, p_out)
-        else:
-            w_in, w_out = p_in, p_out
-            if ctx.n_w:
-                w_in = rest.pop(0)
-                w_out = rest.pop(0) if ctx.n_w == 2 else None
-            for h in range(H):                                 # d a'_uv = <d rst_v, ft_u> (0 for an unsampled halo node)
-                cols = slice(h * Fo, (h + 1) * Fo)
-                ops.sddmm_dot(g.a_in, d_rst[:, cols], ft[:n_in, cols], out=de_in[:, h])
-                if c is not None:
-                    ops.sddmm_dot(g.a_out, d_rst[:, cols], ft[n_in:, cols], col_map=g.slot, n_direct=0, out=de_out[:, h])
-            with torch.cuda.device(dev):
-                check(lib.bns_gat_softmax_bwd_f32(*ctx.head, *ctx.tail, p_in.data_ptr(), ops._ptr(p_out), de_in.data_ptr(),
-                                                  ops._ptr(de_out), d_er.data_ptr(), st), "bns_gat_softmax_bwd_f32")
+        w_in, w_out = p_in, p_out
+        if ctx.n_w:
+            w_in = rest.pop(0)
+            w_out = rest.pop(0) if ctx.n_w == 2 else None
+        for h in range(H):                                     # d a'_uv = <d rst_v, ft_u> (0 for an unsampled halo node)
+            cols = slice(h * Fo, (h + 1) * Fo)
+            ops.sddmm_dot(g.a_in, d_rst[:, cols], ft[:n_in, cols], out=de_in[:, h])
+            if c is not None:
+                ops.sddmm_dot(g.a_out, d_rst[:, cols], ft[n_in:, cols], col_map=g.slot, n_direct=0, out=de_out[:, h])
+        with torch.cuda.device(dev):
+            check(lib.bns_gat_softmax_bwd_f32(*ctx.head, *ctx.tail, p_in.data_ptr(), ops._ptr(p_out), de_in.data_ptr(),
+                                              ops._ptr(de_out), d_er.data_ptr(), st), "bns_gat_softmax_bwd_f32")
         with torch.cuda.device(dev):
             d_el = torch.empty(n_u, H, dtype=torch.float32, device=dev)
             check(lib.bns_gat_colsum_f32(g.a_in_t._h, de_in.data_ptr(), H, None, 0, d_el.data_ptr(), st),
@@ -457,7 +377,7 @@ class GatAttention(torch.autograd.Function):
         return d_ft, d_el, d_er, None, None, None, None, None, None
 
 
-GAT_INFER_MAX_HEADS, GAT_INFER_MAX_WIDTH = 8, 1024
+GAT_MAX_HEADS, GAT_MAX_WIDTH = 8, 1024
 
 
 def gat_padded_width(Fo: int) -> int:
@@ -465,12 +385,13 @@ def gat_padded_width(Fo: int) -> int:
     return (Fo + 3) // 4 * 4
 
 
-def gat_infer_unsupported(H: int, Fo: int) -> Optional[str]:
-    """``None`` when ``bns_gat_infer_f32`` takes ``H`` heads of width ``Fo``, else the limit that is exceeded."""
-    if not 1 <= H <= GAT_INFER_MAX_HEADS:
-        return f"heads = {H} is outside 1..{GAT_INFER_MAX_HEADS}"
-    if Fo < 1 or H * gat_padded_width(Fo) > GAT_INFER_MAX_WIDTH:
-        return (f"heads * padded per-head width = {H} * {gat_padded_width(Fo)} exceeds {GAT_INFER_MAX_WIDTH}"
+def gat_unsupported(H: int, Fo: int) -> Optional[str]:
+    """``None`` when the GAT kernels (``bns_gat_proj_f32``, ``bns_gat_scores_f32``, ``bns_gat_infer_f32``) take ``H``
+    heads of width ``Fo`` padded to a multiple of 4, else the limit that is exceeded."""
+    if not 1 <= H <= GAT_MAX_HEADS:
+        return f"heads = {H} is outside 1..{GAT_MAX_HEADS}"
+    if Fo < 1 or H * gat_padded_width(Fo) > GAT_MAX_WIDTH:
+        return (f"heads * padded per-head width = {H} * {gat_padded_width(Fo)} exceeds {GAT_MAX_WIDTH}"
                 if Fo >= 1 else f"per-head width {Fo} < 1")
     return None
 
@@ -484,7 +405,7 @@ def gat_infer(a: ops.DeviceGraph, ft: torch.Tensor, el: torch.Tensor, er: torch.
     ``ft [a.n_cols, H * Fp]`` (head-major, ``Fp`` a multiple of 4, pad columns zero), ``el [a.n_cols, H]``,
     ``er [a.n_rows, H]``, ``bias [H * Fp]`` or None -> ``[a.n_rows, H * Fp]``.  No dropout, no gradient."""
     from ._lib import BnsError, check, lib
-    why = gat_infer_unsupported(H, Fp)
+    why = gat_unsupported(H, Fp)
     if why is not None or Fp % 4:
         raise BnsError(f"gat_infer: {why or f'padded width {Fp} is not a multiple of 4'}")
     for t, name in ((ft, "ft"), (el, "el"), (er, "er")) + (((bias, "bias"),) if bias is not None else ()):
@@ -516,7 +437,7 @@ def gat_infer_block(a: ops.DeviceGraph, ft: Optional[torch.Tensor], el: Optional
     ``last`` writes ``acc / l + bias`` to ``rst`` (which may be ``acc`` itself, same rows and stride).  ``ft [a.n_cols, H * Fp]`` / ``el
     [a.n_cols, H]`` are this block's source rows (may be None when the block has no entries), ``er`` the rows' own."""
     from ._lib import BnsError, check, lib
-    why = gat_infer_unsupported(H, Fp)
+    why = gat_unsupported(H, Fp)
     if why is not None or Fp % 4:
         raise BnsError(f"gat_infer_block: {why or f'padded width {Fp} is not a multiple of 4'}")
     if a.nnz and (ft is None or el is None):

@@ -7,10 +7,11 @@ call the reference makes -- ``layer(g, (h_src, h_dst))`` on the bipartite ``_U -
     e_uv = leaky_relu(el_u + er_v)   a = attn_drop(edge_softmax(e))     rst_v = sum_u a_uv ft_u + bias
 
 Everything after ``fc`` runs as kernels of libbnsgcn.so (``graph.GatProjection``, ``graph.GatAttention``; feature
-dropout on the Philox kernel).  The op-by-op fallback (``BNS_GAT_FUSED=0`` or a per-head width that is not a multiple
-of 4) writes the per-entry score / softmax algebra as torch ops on ``[nnz, heads]`` vectors over the STATIC entry lists
-of the partition graph (an unsampled halo entry gets e = -inf, i.e. weight 0) around the weighted SpMM, its transpose
-and the SDDMM-dot of the attention gradient (``graph.WeightedAggregate``).
+dropout on the Philox kernel).  The kernels read each head's columns as 16-byte lanes, so every forward pads a per-head
+width that is not a multiple of 4 (zero rows of ``fc.weight``, zero columns of ``attn_l`` / ``attn_r`` / ``bias`` per
+head) and slices the pad off; in training the gradients flow back through the padding to the unpadded parameters.
+The kernels take at most 8 heads and 1024 padded columns in all (``graph.gat_unsupported``); the constructor refuses
+a layer beyond that.
 
 In evaluation the layer also takes DGL's homogeneous call ``layer(g, h)`` on the full graph (``FullGraphHandle``, what
 ``GAT.forward`` makes when not training): one ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, and the attention as
@@ -22,16 +23,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import fused, ops
-from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionEvalGraph, PartitionGraph, WeightedAggregate,
-                     gat_attention_supported, gat_entries, gat_infer, gat_infer_block, gat_infer_unsupported,
-                     gat_padded_width)
+from ..graph import (FullGraphHandle, GatAttention, GatProjection, PartitionEvalGraph, PartitionGraph, gat_infer,
+                     gat_infer_block, gat_padded_width, gat_unsupported)
 from . import dense
-
-
-# the attention (u_add_v, leaky_relu, edge_softmax, attn_drop, u_mul_e + sum of DGL's GATConv) as kernels
-# (graph.GatAttention); False / per-head widths that are not multiples of 4: the op-by-op torch path below
-import os as _os
-FUSED_ATTENTION = _os.environ.get("BNS_GAT_FUSED", "1") != "0"
 
 
 class GATConv(nn.Module):
@@ -41,6 +35,9 @@ class GATConv(nn.Module):
         super(GATConv, self).__init__()
         if residual or activation is not None:
             raise NotImplementedError("the reference constructs GATConv(in, out, heads, dropout, dropout) only")
+        why = gat_unsupported(num_heads, out_feats)
+        if why is not None:
+            raise NotImplementedError(f"GATConv: the attention kernels do not take this layer: {why}")
         self._num_heads, self._in_feats, self._out_feats = num_heads, in_feats, out_feats
         self.fc = nn.Linear(in_feats, out_feats * num_heads, bias=False)
         self.attn_l = nn.Parameter(torch.empty(1, num_heads, out_feats))
@@ -73,95 +70,43 @@ class GATConv(nn.Module):
         if not isinstance(graph, PartitionGraph) or not isinstance(feat, tuple):
             raise NotImplementedError("GATConv: the training call layer(g, (h_src, h_dst)) on a partition graph, or "
                                       "layer(g, h) on the full graph in evaluation")
-        H, Fo = self._num_heads, self._out_feats
-        n_in = graph.n_in
+        H, Fo, Fp, w, al, ar, b = self._padded_params()
         ready = getattr(feat[0], '_bns_ready', None)
         if ready is not None:          # every row of h_src is read below: wait for the overlapped exchange
             torch.cuda.current_stream(feat[0].device).wait_event(ready)
-        kernels = FUSED_ATTENTION and gat_attention_supported(H, Fo) and \
-            (graph.a_out is None or (graph.compact is not None and graph.compact.cpos is not None))
         salt = ops.RNG["seed"] + 15485863 * (1 + getattr(self, "_layer_index", 0))
         pf = self.feat_drop.p if self.training else 0.0
-        if kernels and pf > 0 and fused.dropout_supported(feat[0]) and fused.dropout_supported(feat[1]):
+        if pf > 0 and fused.dropout_supported(feat[0]) and fused.dropout_supported(feat[1]):
             # two independent masks, as DGL draws them (feat_drop is applied to the source and the destination rows)
             h_src, h_dst = fused.DropoutFn.apply(feat[0], pf, salt + 1), fused.DropoutFn.apply(feat[1], pf, salt + 2)
         else:
             h_src, h_dst = self.feat_drop(feat[0]), self.feat_drop(feat[1])
-        ft_src = dense.linear(h_src, self.fc.weight).view(-1, H, Fo)
-        ft_dst = dense.linear(h_dst, self.fc.weight).view(-1, H, Fo)
-        if kernels:
-            # el / er, score -> edge softmax -> dropout -> weighted aggregation (and their backward) as kernels
-            ft2 = ft_src.reshape(-1, H * Fo)
-            el, er = GatProjection.apply(ft2, ft_dst.reshape(-1, H * Fo), self.attn_l, self.attn_r, H, Fo)
-            p = self.attn_drop.p if self.training else 0.0
-            rst = GatAttention.apply(ft2, el, er, graph, H, Fo, self.negative_slope, p, salt)
-            if self.bias is not None:
-                rst += self.bias                                    # in place: the attention saved nothing of it
-            return rst.view(-1, H, Fo)
-        el = (ft_src * self.attn_l).sum(dim=-1)                     # [n_U, H]
-        er = (ft_dst * self.attn_r).sum(dim=-1)                     # [n_in, H]
-        rin, cin, rout, cout = gat_entries(graph)
-        e_in = F.leaky_relu(el[cin] + er[rin], self.negative_slope)                                  # [nnz_in, H]
-        n_u = ft_src.shape[0]
-        if rout.numel() and n_u > n_in:
-            xrow = graph.slot.long()[cout]                                                           # -1 = unsampled
-            valid = (xrow >= 0).unsqueeze(1)
-            e_out = F.leaky_relu(el[n_in + xrow.clamp(min=0)] + er[rout], self.negative_slope)
-            e_out = torch.where(valid, e_out, torch.full_like(e_out, float('-inf')))
-        else:
-            rout = cout = rout[:0]
-            e_out = e_in.new_empty(0, H)
-        # edge softmax over each destination's in-entries (inner + sampled halo)
-        m = torch.full((n_in, H), float('-inf'), device=e_in.device)
-        m = m.scatter_reduce(0, rin.unsqueeze(1).expand(-1, H), e_in.detach(), 'amax')
-        if e_out.numel():
-            m = m.scatter_reduce(0, rout.unsqueeze(1).expand(-1, H), e_out.detach(), 'amax')
-        ex_in = torch.exp(e_in - m[rin])
-        ex_out = torch.exp(e_out - m[rout]) if e_out.numel() else e_out
-        den = torch.zeros(n_in, H, device=e_in.device).index_add(0, rin, ex_in)
-        if e_out.numel():
-            den = den.index_add(0, rout, ex_out)
-        a_in = self.attn_drop(ex_in / den[rin])
-        a_out = self.attn_drop(ex_out / den[rout]) if e_out.numel() else ex_out
-        # weighted aggregation, one head at a time (16-byte lanes need the per-head width padded to 4)
-        pad = (-Fo) % 4
-        outs = []
-        for h in range(H):
-            ft_h = ft_src[:, h, :]
-            if pad:
-                ft_h = F.pad(ft_h, (0, pad))
-            w_out_h = a_out[:, h] if a_out.numel() else a_in.new_empty(graph.a_out.nnz if graph.a_out is not None else 0)
-            if a_out.numel() == 0 and graph.a_out is not None:
-                w_out_h = a_in.new_zeros(graph.a_out.nnz)
-            r = WeightedAggregate.apply(ft_h.contiguous(), a_in[:, h], w_out_h, graph)
-            outs.append(r[:, :Fo])
-        rst = torch.stack(outs, dim=1)                              # [n_in, H, Fo]
-        if self.bias is not None:
-            rst = rst + self.bias.view(1, H, Fo)
-        return rst
+        ft_src = dense.linear(h_src, w)                             # [n_U, H * Fp]
+        ft_dst = dense.linear(h_dst, w)
+        # el / er, score -> edge softmax -> dropout -> weighted aggregation (and their backward) as kernels
+        el, er = GatProjection.apply(ft_src, ft_dst, al, ar, H, Fp)
+        p = self.attn_drop.p if self.training else 0.0
+        rst = GatAttention.apply(ft_src, el, er, graph, H, Fp, self.negative_slope, p, salt)
+        if b is not None:
+            rst += b                                                # in place: the attention saved nothing of it
+        return rst.view(-1, H, Fp)[..., :Fo]
 
     @torch.no_grad()
     def _forward_full_graph(self, graph: FullGraphHandle, feat: torch.Tensor) -> torch.Tensor:
         """DGL's homogeneous branch with ``h_src = h_dst = feat`` (``feat_drop`` is the identity in evaluation): one
         ``fc`` GEMM, ``el`` / ``er`` from the same ``ft``, then the one-pass attention kernel (``graph.gat_infer``).
-        A per-head width that is not a multiple of 4 runs padded -- zero rows of ``fc.weight``, zero columns of
-        ``attn_l`` / ``attn_r`` / ``bias`` per head -- and the pad is sliced off.  No gradient flows through it."""
-        H, Fo, Fp, w, al, ar, b = self._eval_params(graph)
+        No gradient flows through it."""
+        _refuse_zero_in_degree(graph)
+        H, Fo, Fp, w, al, ar, b = self._padded_params()
         ft = dense.linear(feat, w)                                  # [n, H * Fp]
         el, er = GatProjection.apply(ft, ft, al, ar, H, Fp)
         rst = gat_infer(graph.a, ft, el, er, H, Fp, self.negative_slope, b)
         return rst.view(-1, H, Fp)[..., :Fo]
 
-    def _eval_params(self, graph):
-        """The evaluation forward's checks and its parameters with each head's width padded to a multiple of 4."""
+    def _padded_params(self):
+        """``H, Fo, Fp`` and the parameters with each head's width padded to ``Fp``, a multiple of 4 (the
+        parameters themselves when ``Fo`` is one already)."""
         H, Fo = self._num_heads, self._out_feats
-        why = gat_infer_unsupported(H, Fo)
-        if why is not None:
-            raise NotImplementedError(f"GATConv evaluation forward: {why}")
-        if graph.has_zero_in_degree():
-            # dgl.nn.GATConv(allow_zero_in_degree=False) refuses such a graph (DGLError)
-            raise RuntimeError("GATConv: there are 0-in-degree nodes in the graph, their output would be invalid; "
-                               "add self-loops")
         Fp = gat_padded_width(Fo)
         w, al, ar, b = self.fc.weight, self.attn_l, self.attn_r, self.bias
         if Fp != Fo:
@@ -177,7 +122,8 @@ class GATConv(nn.Module):
         per peer, the online-softmax state carried between them (``gat_infer_block``).  ``feat``: the inner rows (each
         peer's halo rows are exchanged and transformed one peer at a time), or ``(h_src, h_dst)`` when ``h_src`` already
         holds ``[inner | every halo row]`` (layer 0 of the precomputed model: ``train.precompute``)."""
-        H, Fo, Fp, w, al, ar, b = self._eval_params(graph)
+        _refuse_zero_in_degree(graph)
+        H, Fo, Fp, w, al, ar, b = self._padded_params()
         n_in = graph.n_in
         held = isinstance(feat, tuple)
         src = feat[0] if held else feat
@@ -202,3 +148,10 @@ class GATConv(nn.Module):
                 el_j, _ = GatProjection.apply(ft_j, ft_j[:0], al, ar, H, Fp)
                 gat_infer_block(blk, ft_j, el_j, er, H, Fp, slope, m, l, acc, False, j == live[-1], b, acc)
         return acc.view(-1, H, Fp)[..., :Fo]
+
+
+def _refuse_zero_in_degree(graph) -> None:
+    if graph.has_zero_in_degree():
+        # dgl.nn.GATConv(allow_zero_in_degree=False) refuses such a graph (DGLError)
+        raise RuntimeError("GATConv: there are 0-in-degree nodes in the graph, their output would be invalid; "
+                           "add self-loops")

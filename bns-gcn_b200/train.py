@@ -575,15 +575,6 @@ class GraphedEpoch:
         return self.loss
 
 
-def _gat_eval_unsupported(model) -> Optional[str]:
-    """The GAT evaluation forward runs on bns_gat_infer_f32 / bns_gat_infer_block_f32: ``None`` when every attention
-    layer fits them, else the first limit a layer exceeds."""
-    from .graph import gat_infer_unsupported
-    from .module.gat import GATConv
-    return next((w for w in (gat_infer_unsupported(m._num_heads, m._out_feats) for m in model.layers
-                             if isinstance(m, GATConv)) if w is not None), None)
-
-
 def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     """train.py:300-456.  With ``args.eval`` rank 0 also runs the evaluation / checkpoint branch (:308-321, 427-456)
     through ``evaluate.Evaluator`` -- on the GPU with the same kernels, synchronously, instead of a CPU thread pool;
@@ -599,29 +590,16 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     dev = st.feat.device
     evaluator = None
     if parallel:
-        why = _gat_eval_unsupported(st.model) if args.model == 'gat' else None
-        if why is not None:
-            if rank == 0:
-                import warnings
-                warnings.warn(f'--eval: the GAT evaluation forward does not take this model ({why}); '
-                              'training runs without the evaluation branch')
-        else:
-            from .evaluate import ParallelEvaluator, build_partition_eval_graph
-            eg = build_partition_eval_graph(st.part, node_dict, st.boundary, ctx.comm())
-            evaluator = ParallelEvaluator(args, eg, st.feat, st.labels, node_dict['val_mask'].to(dev),
-                                          node_dict['test_mask'].to(dev), ctx.comm())
+        from .evaluate import ParallelEvaluator, build_partition_eval_graph
+        eg = build_partition_eval_graph(st.part, node_dict, st.boundary, ctx.comm())
+        evaluator = ParallelEvaluator(args, eg, st.feat, st.labels, node_dict['val_mask'].to(dev),
+                                      node_dict['test_mask'].to(dev), ctx.comm())
     elif getattr(args, 'eval', False) and rank == 0:
-        why = _gat_eval_unsupported(st.model) if args.model == 'gat' else None
-        if why is not None:
-            import warnings
-            warnings.warn(f'--eval: the full-graph GAT evaluation forward does not take this model ({why}); '
-                          'training runs without the evaluation branch')
-        else:
-            from .data import make_graph
-            from .evaluate import Evaluator
-            fg = full_graph if full_graph is not None else make_graph(args.dataset, seed=getattr(args, 'graph_seed', 0),
-                                                                      device=dev)
-            evaluator = Evaluator(args, fg, dev)
+        from .data import make_graph
+        from .evaluate import Evaluator
+        fg = full_graph if full_graph is not None else make_graph(args.dataset, seed=getattr(args, 'graph_seed', 0),
+                                                                  device=dev)
+        evaluator = Evaluator(args, fg, dev)
     train_dur, comm_dur, reduce_dur = [], [], []
     torch.cuda.reset_peak_memory_stats(dev)
     print(f'Process {rank} start training')

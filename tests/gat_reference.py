@@ -5,13 +5,6 @@ import torch
 import torch.nn.functional as F
 
 
-def gat_row_walk_nv(H, Fo):
-    """The NV of gat_fwd_kernel<NV> / gat_bwd_kernel<NV> that bns_gat_forward_f32 / bns_gat_backward_f32 launch for
-    H heads of width Fo (float4 column groups per lane, 128 columns per group of the warp)."""
-    nv = (H * Fo + 127) // 128
-    return 1 if nv <= 1 else 2 if nv == 2 else 4 if nv <= 4 else 8
-
-
 def gat_attention_reference(ft, el, er, u, v, n_rows, H, Fo, d, slope=0.2, keep=None, p=0.0):
     """Entry ``k`` sends ``ft[u[k]]`` to row ``v[k]``.  Per head
 

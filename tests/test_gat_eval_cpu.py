@@ -32,17 +32,30 @@ def test_oracle_gat_evaluation_forward_reproduces_the_reference():
     assert _rel(logits, want) < 1e-5
 
 
-def test_gat_infer_limits():
-    """Heads 1..8 and heads * (per-head width rounded up to 4) <= 1024, as the training kernels; anything else is
-    named, so train.run can say which limit keeps a model from evaluating."""
-    from bns_gcn_b200.graph import gat_infer_unsupported, gat_padded_width
+def test_gat_unsupported_names_the_exceeded_limit():
+    """Heads 1..8 and heads * (per-head width rounded up to 4) <= 1024, the limits of every GAT kernel; anything else is
+    named, so GATConv can say which limit keeps it from being built."""
+    from bns_gcn_b200.graph import gat_padded_width, gat_unsupported
     assert [gat_padded_width(f) for f in (1, 4, 5, 41, 256)] == [4, 4, 8, 44, 256]
     for H, Fo in ((1, 5), (2, 5), (4, 256), (8, 128), (1, 1024), (8, 125)):
-        assert gat_infer_unsupported(H, Fo) is None, (H, Fo)
-    assert "heads" in gat_infer_unsupported(9, 16)
-    assert "1024" in gat_infer_unsupported(8, 129)
-    assert "1024" in gat_infer_unsupported(1, 1025)
-    assert gat_infer_unsupported(2, 0) is not None
+        assert gat_unsupported(H, Fo) is None, (H, Fo)
+    assert "heads" in gat_unsupported(9, 16)
+    assert "1024" in gat_unsupported(8, 129)
+    assert "1024" in gat_unsupported(1, 1025)
+    assert gat_unsupported(2, 0) is not None
+
+
+def test_gatconv_refuses_layers_beyond_the_kernel_limits():
+    """A layer the attention kernels cannot run is refused when the model is built, naming the limit; a per-head width
+    that is not a multiple of 4 builds (it runs padded)."""
+    import pytest
+    from bns_gcn_b200.module.gat import GATConv
+    with pytest.raises(NotImplementedError, match="heads = 9 is outside 1..8"):
+        GATConv(16, 16, 9)
+    with pytest.raises(NotImplementedError, match="1028 exceeds 1024"):
+        GATConv(16, 1025, 1)
+    layer = GATConv(16, 41, 1)
+    assert layer.fc.weight.shape == (41, 16) and layer.attn_l.shape == (1, 1, 41)
 
 
 def test_gat_conv_full_graph_training_call_raises():

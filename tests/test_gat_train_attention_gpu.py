@@ -1,20 +1,19 @@
 """GAT's training attention (``graph.GatAttention``) against a float64 restatement, on one crafted partition graph.
 
-Both implementations run every case: the staged kernels (``bns_gat_scores_f32`` -> weighted SpMM per head; SDDMM ->
-``bns_gat_softmax_bwd_f32`` -> ``bns_gat_colsum_f32`` -> transposed SpMM) and the row walks ``gat_fwd_kernel<NV>`` /
-``gat_bwd_kernel<NV>`` (``BNS_GAT_ROWWALK=1``) at NV = 1, 2, 4 and 8 with 1 to 8 heads.  The graph has rows of degree
-0, 1, 31, 32, 33 and 4100 (the long one ordered so that its running maximum grows at every block of 32), halo-only rows,
+The staged kernels (``bns_gat_scores_f32`` -> weighted SpMM per head; SDDMM -> ``bns_gat_softmax_bwd_f32`` ->
+``bns_gat_colsum_f32`` -> transposed SpMM) run every case, with 1 to 8 heads and up to 1024 columns.  The graph has rows
+of degree 0, 1, 31, 32, 33 and 4100 (the long one ordered so that its running maximum grows at every block of 32), halo-only rows,
 rows whose halo entries are all unsampled, and a halo row whose chunks hold 0, 1, 31, 32 and 33 sampled entries.  The
 scores reach 120, where exp overflows float32 without the max subtraction, and some are exactly 0.  Also: dropout
-against a replay of its Philox mask, degenerate partitions, determinism, argument rejection, and ``GATConv`` on the
-kernels against its op-by-op path."""
+against a replay of its Philox mask, degenerate partitions, determinism, argument rejection, and ``GATConv``'s training call (padded per-head widths
+included) against float64."""
 import types
 
 import numpy as np
 import pytest
 import torch
 
-from tests.gat_reference import gat_attention_reference, gat_row_walk_nv
+from tests.gat_reference import gat_attention_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -123,10 +122,9 @@ def _crafted(H, seed):
     return case
 
 
-def _run(g, ft, el, er, d, H, Fo, p, seed, rowwalk, monkeypatch):
+def _run(g, ft, el, er, d, H, Fo, p, seed):
     """GatAttention forward and backward on the device: (rst, d ft, d el, d er) on the CPU."""
     from bns_gcn_b200.graph import GatAttention
-    monkeypatch.setenv("BNS_GAT_ROWWALK", rowwalk)
     dev = torch.device("cuda:0")
     ftg, elg, erg = (t.to(dev).requires_grad_(True) for t in (ft, el, er))
     out = GatAttention.apply(ftg, elg, erg, g, H, Fo, SLOPE, p, seed)
@@ -157,13 +155,12 @@ def _check(got, want, v, special=LIVE_SPECIAL):
 
 
 CASES = [(1, 64), (3, 68), (5, 80), (8, 128), (1, 512), (5, 16), (3, 300)]
-assert {gat_row_walk_nv(H, Fo) for H, Fo in CASES} == {1, 2, 4, 8} and {1, 3, 5, 8} <= {H for H, _ in CASES}
+assert {1, 3, 5, 8} <= {H for H, _ in CASES}
 
 
-@pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
 @pytest.mark.parametrize("H,Fo", CASES)
-def test_attention_matches_float64_on_crafted_rows(built, monkeypatch, H, Fo, rowwalk):
-    """Forward, d ft, d el and d er of both implementations against the float64 restatement, on the whole graph and
+def test_attention_matches_float64_on_crafted_rows(built, H, Fo):
+    """Forward, d ft, d el and d er against the float64 restatement, on the whole graph and
     on each special row; scores beyond exp's float32 range, of exactly 0, and on both sides of 0."""
     case = _crafted(H, 10 * H + Fo)
     ft = torch.randn(case.n_u, H * Fo, generator=case.gen)
@@ -171,7 +168,7 @@ def test_attention_matches_float64_on_crafted_rows(built, monkeypatch, H, Fo, ro
     want = gat_attention_reference(ft, case.el, case.er, case.u, case.v, N_IN, H, Fo, d, SLOPE)
     e = want[4]
     assert e.max().item() > 89.0 and (e == 0).any() and (e < 0).any() and (e > 0).any()
-    got = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.0, 1, rowwalk, monkeypatch)
+    got = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.0, 1)
     _check(got, want, case.v)
 
 
@@ -192,10 +189,10 @@ def _philox_keep(gid, H, seed, offset, p):
 
 @pytest.mark.parametrize("H", [5, 8])
 @pytest.mark.parametrize("p", [0.1, 0.5])
-def test_attention_dropout_mask_and_gradients(built, monkeypatch, H, p):
+def test_attention_dropout_mask_and_gradients(built, H, p):
     """bns_gat_scores_f32, called as GatAttention.forward calls it, gives P and W = P * mask / (1 - p); the mask is the
-    Philox replay, keeps 1 - p of every head, and heads h and h + 4 draw independent masks.  Both implementations under
-    that mask equal the float64 restatement, forward and backward."""
+    Philox replay, keeps 1 - p of every head, and heads h and h + 4 draw independent masks.  GatAttention under that
+    mask equals the float64 restatement, forward and backward."""
     from bns_gcn_b200 import ops
     from bns_gcn_b200._lib import check, lib
     dev = torch.device("cuda:0")
@@ -233,8 +230,7 @@ def test_attention_dropout_mask_and_gradients(built, monkeypatch, H, p):
         ft = torch.randn(case.n_u, H * Fo, generator=case.gen)
         d = torch.randn(N_IN, H * Fo, generator=case.gen)
         want = gat_attention_reference(ft, case.el, case.er, case.u, case.v, N_IN, H, Fo, d, SLOPE, keep=mask, p=p)
-        for rowwalk in ("0", "1"):
-            _check(_run(g, ft, case.el, case.er, d, H, Fo, p, seed, rowwalk, monkeypatch), want, case.v)
+        _check(_run(g, ft, case.el, case.er, d, H, Fo, p, seed), want, case.v)
     finally:
         ops.RNG.update(seed=0, offset=0, offset_dev=None)
 
@@ -266,8 +262,7 @@ def _plain_partition(n_in, n_halo, n_slab, inner_deg, halo_deg, seed):
     return g, (ix_in, rows_in), (n_in + x[x >= 0], rows_out[x >= 0]), gen
 
 
-@pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
-def test_attention_on_degenerate_partitions(built, monkeypatch, rowwalk):
+def test_attention_on_degenerate_partitions(built):
     """A partition without inner entries (every row fed by the halo alone), and a halo matrix while no halo node is
     received (ft has only the n_in inner rows, so the halo entries are left out), against the float64 restatement."""
     H, Fo, n_in, n_slab = 3, 24, 300, 150
@@ -276,16 +271,15 @@ def test_attention_on_degenerate_partitions(built, monkeypatch, rowwalk):
     el, er = _grid(n_in + n_slab, H, gen), _grid(n_in, H, gen)
     ft, d = torch.randn(n_in + n_slab, H * Fo, generator=gen), torch.randn(n_in, H * Fo, generator=gen)
     want = gat_attention_reference(ft, el, er, u, v, n_in, H, Fo, d, SLOPE)
-    _check(_run(g, ft, el, er, d, H, Fo, 0.0, 1, rowwalk, monkeypatch), want, v, ())
+    _check(_run(g, ft, el, er, d, H, Fo, 0.0, 1), want, v, ())
     g, (u, v), _, gen = _plain_partition(n_in, 400, n_slab, 7, 9, seed=6)
     el, er = _grid(n_in, H, gen), _grid(n_in, H, gen)
     ft, d = torch.randn(n_in, H * Fo, generator=gen), torch.randn(n_in, H * Fo, generator=gen)
     want = gat_attention_reference(ft, el, er, u, v, n_in, H, Fo, d, SLOPE)
-    _check(_run(g, ft, el, er, d, H, Fo, 0.0, 1, rowwalk, monkeypatch), want, v, ())
+    _check(_run(g, ft, el, er, d, H, Fo, 0.0, 1), want, v, ())
 
 
-@pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
-def test_attention_repeats_bit_identically(built, monkeypatch, rowwalk):
+def test_attention_repeats_bit_identically(built):
     """Forward and backward launched twice on the same inputs (dropout on, 8 heads) give bit-identical results."""
     from bns_gcn_b200 import ops
     H, Fo = 8, 32
@@ -294,38 +288,31 @@ def test_attention_repeats_bit_identically(built, monkeypatch, rowwalk):
     d = torch.randn(N_IN, H * Fo, generator=case.gen)
     ops.RNG.update(offset=9, offset_dev=None)
     try:
-        first = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.3, 99, rowwalk, monkeypatch)
-        second = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.3, 99, rowwalk, monkeypatch)
+        first = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.3, 99)
+        second = _run(case.g, ft, case.el, case.er, d, H, Fo, 0.3, 99)
     finally:
         ops.RNG.update(seed=0, offset=0, offset_dev=None)
     for a, b in zip(first, second):
         assert torch.equal(a, b)
 
 
-def test_attention_entry_points_reject_bad_arguments(built):
-    """Heads outside 1..8, a width that is not a multiple of 4, more than 1024 columns, a misaligned ft and p = 1 are
-    answered with BNS_E_INVALID and a message naming the function; GATConv's choice of the kernels
-    (graph.gat_attention_supported) accepts exactly what bns_gat_forward_f32 and bns_gat_backward_f32 accept."""
+def test_attention_kernels_and_gatconv_reject_bad_arguments(built):
+    """Heads outside 1..8, a width that is not a multiple of 4, more than 1024 columns and p = 1 are answered with
+    BNS_E_INVALID and a message naming the function.  GATConv builds exactly when graph.gat_unsupported accepts its
+    heads and width, and that is exactly when bns_gat_scores_f32 takes the heads and bns_gat_proj_f32 the padded width."""
     from bns_gcn_b200 import ops
     from bns_gcn_b200._lib import lib
-    from bns_gcn_b200.graph import gat_attention_supported
+    from bns_gcn_b200.graph import gat_padded_width, gat_unsupported
+    from bns_gcn_b200.module.gat import GATConv
     dev = torch.device("cuda:0")
     a = ops.DeviceGraph.from_csr(torch.tensor([0, 1, 2], dtype=torch.int64, device=dev),
                                  torch.tensor([1, 0], dtype=torch.int32, device=dev), 2)
     aT = a.transpose()
     LD = 1040                                                   # wide enough that only the width limit rejects 1028
-    ft, rst = torch.zeros(2, LD, device=dev), torch.zeros(2, LD, device=dev)
+    ft, attn = torch.zeros(2, LD, device=dev), torch.zeros(LD, device=dev)
     el, er, P, dE, d_er = (torch.zeros(2, 8, device=dev) for _ in range(5))
+    proj_out = torch.zeros(2, 16, device=dev)
     st = torch.cuda.current_stream().cuda_stream
-
-    def fwd(H=2, Fo=8, ft_off=0, p=0.0):
-        return lib.bns_gat_forward_f32(a._h, None, None, None, None, 2, ft.data_ptr() + ft_off, LD, H, Fo, el.data_ptr(),
-                                       er.data_ptr(), SLOPE, p, 1, 0, None, rst.data_ptr(), LD, P.data_ptr(), None, st)
-
-    def bwd(H=2, Fo=8, ft_off=0, p=0.0):
-        return lib.bns_gat_backward_f32(a._h, None, None, None, None, 2, ft.data_ptr() + ft_off, LD, H, Fo,
-                                        el.data_ptr(), er.data_ptr(), SLOPE, p, 1, 0, None, rst.data_ptr(), LD,
-                                        P.data_ptr(), None, dE.data_ptr(), None, None, None, d_er.data_ptr(), st)
 
     def scores(H=2, p=0.0):
         return lib.bns_gat_scores_f32(a._h, None, None, None, None, 2, H, el.data_ptr(), er.data_ptr(), SLOPE, p, 1, 0,
@@ -338,46 +325,73 @@ def test_attention_entry_points_reject_bad_arguments(built):
     def colsum(H=2):
         return lib.bns_gat_colsum_f32(aT._h, dE.data_ptr(), H, None, 0, d_er.data_ptr(), st)
 
-    bad = {fwd: [dict(H=0), dict(H=9), dict(Fo=6), dict(H=1, Fo=1028), dict(ft_off=4), dict(p=1.0)],
-           bwd: [dict(H=0), dict(H=9), dict(Fo=6), dict(H=1, Fo=1028), dict(ft_off=4), dict(p=1.0)],
-           scores: [dict(H=0), dict(H=9), dict(p=1.0)],
+    def proj(H=2, Fo=8):
+        return lib.bns_gat_proj_f32(ft.data_ptr(), LD, 2, H, Fo, attn.data_ptr(), proj_out.data_ptr(), st)
+
+    bad = {scores: [dict(H=0), dict(H=9), dict(p=1.0)],
            softmax_bwd: [dict(H=0), dict(H=9), dict(p=1.0)],
-           colsum: [dict(H=0), dict(H=9)]}
+           colsum: [dict(H=0), dict(H=9)],
+           proj: [dict(H=0), dict(Fo=6), dict(H=1, Fo=1028), dict(H=2, Fo=516), dict(H=8, Fo=132)]}
     for fn, cases in bad.items():
         assert fn() == 0, fn.__name__                             # the same call with good arguments runs
-        name = {fwd: b"bns_gat_forward_f32", bwd: b"bns_gat_backward_f32", scores: b"bns_gat_scores_f32",
-                softmax_bwd: b"bns_gat_softmax_bwd_f32", colsum: b"bns_gat_colsum_f32"}[fn]
+        name = {scores: b"bns_gat_scores_f32", softmax_bwd: b"bns_gat_softmax_bwd_f32", colsum: b"bns_gat_colsum_f32",
+                proj: b"bns_gat_proj_f32"}[fn]
         for kw in cases:
             assert fn(**kw) == -1 and name in lib.bns_last_error(), (fn.__name__, kw)
     for H in range(0, 10):
-        for Fo in (-4, 0, 1, 2, 4, 6, 8, 12, 100, 126, 128, 129, 256, 340, 512, 1024, 1028):
-            ok = gat_attention_supported(H, Fo)
-            assert (fwd(H, Fo) == 0) == ok and (bwd(H, Fo) == 0) == ok, (H, Fo)
+        for Fo in (-4, 0, 1, 2, 4, 5, 6, 8, 12, 41, 100, 126, 127, 128, 129, 256, 340, 341, 512, 1021, 1024, 1028):
+            ok = gat_unsupported(H, Fo) is None
+            assert ok == (scores(H) == 0 and proj(H, gat_padded_width(Fo)) == 0), (H, Fo)
+            try:
+                GATConv(4, Fo, H)
+                built_layer = True
+            except NotImplementedError as e:
+                built_layer = False
+                assert gat_unsupported(H, Fo) in str(e), (H, Fo)
+            assert built_layer == ok, (H, Fo)
     torch.cuda.synchronize()
 
 
-def test_gatconv_kernel_path_matches_op_by_op_path(built, monkeypatch):
-    """GATConv's training call on a partition graph: the attention kernels (graph.GatAttention) and the op-by-op torch
-    path (what a per-head width that is not a multiple of 4, such as Reddit's 41 classes, trains on) give the same
-    output and the same gradients of every parameter and of both inputs."""
+def test_gatconv_training_matches_float64(built):
+    """GATConv's training call layer(g, (h_src, h_dst)) on a partition graph -- fc, el / er, the attention and the bias,
+    with a per-head width padded to a multiple of 4 where it is not one -- against a float64 restatement: the output
+    and the gradients of both inputs, fc.weight, attn_l, attn_r and bias.  Heads x width: a width that is a multiple
+    of 4, and two padded layouts (one head of 41 like Reddit's classes, two heads of 5)."""
+    for H, Fo in ((3, 40), (1, 41), (2, 5)):
+        _check_gatconv_training(H, Fo)
+
+
+def _check_gatconv_training(H, Fo):
     from bns_gcn_b200.module import gat
     dev = torch.device("cuda:0")
-    H, Fo, F_in = 3, 40, 24
-    case = _crafted(H, 77)
-    torch.manual_seed(0)
+    F_in = 24
+    case = _crafted(H, 77 + Fo)
+    torch.manual_seed(Fo)
     layer = gat.GATConv(F_in, Fo, H, 0.0, 0.0).to(dev).train()
     gen = torch.Generator().manual_seed(78)
-    h_src = torch.randn(case.n_u, F_in, generator=gen).to(dev)
-    d = torch.randn(N_IN, H, Fo, generator=gen).to(dev)
-    results = []
-    for fused_attention in (True, False):
-        monkeypatch.setattr(gat, "FUSED_ATTENTION", fused_attention)
-        layer.zero_grad(set_to_none=True)
-        hs = h_src.clone().requires_grad_(True)
-        hd = h_src[:N_IN].clone().requires_grad_(True)
-        out = layer(case.g, (hs, hd))
-        out.backward(d)
-        results.append([out.detach(), hs.grad, hd.grad] + [p.grad for p in layer.parameters()])
-    assert len(results[0]) == 7 and all(t is not None for t in results[0] + results[1])
-    for a, b in zip(*results):
-        assert torch.isfinite(b).all() and _rel(a, b) < 1e-5
+    with torch.no_grad():
+        layer.bias.copy_(torch.randn(H * Fo, generator=gen))          # (initialised to 0)
+    h_src = torch.randn(case.n_u, F_in, generator=gen)
+    h_dst = torch.randn(N_IN, F_in, generator=gen)
+    d = torch.randn(N_IN, H, Fo, generator=gen)
+    hs, hd = h_src.to(dev).requires_grad_(True), h_dst.to(dev).requires_grad_(True)
+    out = layer(case.g, (hs, hd))
+    out.backward(d.to(dev))
+    got = [out, hs.grad, hd.grad, layer.fc.weight.grad, layer.attn_l.grad, layer.attn_r.grad, layer.bias.grad]
+    # float64: fc and el / er under autograd; the attention's own gradients (d ft, d el, d er) from the restatement,
+    # carried back through fc and the projections as the gradient of <ft, d ft> + <el, d el> + <er, d er>
+    w, al, ar, b = (t.detach().double().cpu().requires_grad_(True)
+                    for t in (layer.fc.weight, layer.attn_l, layer.attn_r, layer.bias))
+    xs, xd = h_src.double().requires_grad_(True), h_dst.double().requires_grad_(True)
+    ft_src, ft_dst = xs @ w.t(), xd @ w.t()
+    el = (ft_src.view(-1, H, Fo) * al).sum(-1)
+    er = (ft_dst.view(-1, H, Fo) * ar).sum(-1)
+    rst, d_ft, d_el, d_er = gat_attention_reference(ft_src.detach(), el.detach(), er.detach(), case.u, case.v, N_IN, H,
+                                                    Fo, d.reshape(N_IN, H * Fo), SLOPE)[:4]
+    want_out = rst.view(-1, H, Fo) + b.detach().view(H, Fo)
+    ((ft_src * d_ft).sum() + (el * d_el).sum() + (er * d_er).sum()).backward()
+    want = [want_out, xs.grad, xd.grad, w.grad, al.grad, ar.grad, d.double().sum(0).reshape(-1)]
+    names = ["out", "d h_src", "d h_dst", "d fc.weight", "d attn_l", "d attn_r", "d bias"]
+    for name, g_, w_ in zip(names, got, want):
+        assert g_ is not None and g_.shape == w_.shape, (H, Fo, name)
+        assert _rel(g_, w_) < (2e-5 if name == "out" else 5e-5), (H, Fo, name, _rel(g_, w_))

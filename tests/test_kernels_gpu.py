@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.gat_reference import gat_attention_reference, gat_row_walk_nv
+from tests.gat_reference import gat_attention_reference
 
 pytestmark = pytest.mark.gpu
 
@@ -703,20 +703,17 @@ def _gat_case(H, Fo, seed, with_halo=True):
 
 GAT_ATTENTION_CASES = [(1, 64, True), (2, 8, True), (4, 16, False), (1, 256, True), (1, 100, True), (4, 128, True),
                        (3, 100, True), (8, 128, True), (5, 16, True), (8, 4, False), (1, 1024, True)]
-# every instantiation of the row-walk kernels, and heads above 4 (the upper half of their per-head registers and the
-# second Philox counter word of the dropout mask), stay covered when the list is edited
-assert {gat_row_walk_nv(H, Fo) for H, Fo, _ in GAT_ATTENTION_CASES} == {1, 2, 4, 8}
+# heads above 4 (the upper half of the per-head registers and the second Philox counter word of the dropout mask) stay
+# covered when the list is edited
 assert any(H > 4 for H, _, _ in GAT_ATTENTION_CASES)
 
 
-@pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
 @pytest.mark.parametrize("H,Fo,with_halo", GAT_ATTENTION_CASES)
-def test_fused_gat_attention_matches_the_per_entry_reference(built, monkeypatch, H, Fo, with_halo, rowwalk):
+def test_fused_gat_attention_matches_the_per_entry_reference(built, H, Fo, with_halo):
     """graph.GatAttention == the u_add_v / leaky_relu / edge_softmax / u_mul_e+sum algebra of dgl.nn.GATConv written with
-    torch ops on explicit entry lists (what module/gat.py's op-by-op path and oracle.GATConvRef do), forward and the
-    gradients with respect to ft, el and er; attention dropout off."""
+    torch ops on explicit entry lists (what oracle.GATConvRef does), forward and the gradients with respect to ft, el
+    and er; attention dropout off."""
     from bns_gcn_b200.graph import GatAttention
-    monkeypatch.setenv("BNS_GAT_ROWWALK", rowwalk)
     dev = torch.device("cuda:0")
     g, n_in, n_u, u, v, gen = _gat_case(H, Fo, 100 + H + Fo, with_halo)
     ft = torch.randn(n_u, H * Fo, generator=gen)
@@ -736,13 +733,11 @@ def test_fused_gat_attention_matches_the_per_entry_reference(built, monkeypatch,
     assert torch.all(out.detach().cpu()[deg == 0] == 0)
 
 
-@pytest.mark.parametrize("rowwalk", ["0", "1"], ids=["stages", "row-walk"])
-def test_fused_gat_attention_dropout_is_consistent_between_forward_and_backward(built, monkeypatch, rowwalk):
+def test_fused_gat_attention_dropout_is_consistent_between_forward_and_backward(built):
     """With attention dropout the layer is still linear in ft for fixed scores: <rst(ft), d> == <ft, d_ft(d)> holds only
     if the backward regenerates exactly the forward's Philox mask; the keep rate is 1 - p; a new offset gives a new mask."""
     from bns_gcn_b200 import ops
     from bns_gcn_b200.graph import GatAttention
-    monkeypatch.setenv("BNS_GAT_ROWWALK", rowwalk)
     dev = torch.device("cuda:0")
     H, Fo, p = 2, 32, 0.4
     g, n_in, n_u, u, v, gen = _gat_case(H, Fo, 7, True)
@@ -757,11 +752,6 @@ def test_fused_gat_attention_dropout_is_consistent_between_forward_and_backward(
     assert abs(lhs - rhs) <= 1e-4 * max(abs(lhs), 1.0), (lhs, rhs)
     out2 = GatAttention.apply(ft.detach(), el, er, g, H, Fo, 0.2, p, 3)
     assert torch.equal(out2, out.detach())
-    # the staged kernels and the one-launch row walk draw the SAME mask (Philox keyed by entry position and head)
-    monkeypatch.setenv("BNS_GAT_ROWWALK", "1" if rowwalk == "0" else "0")
-    other = GatAttention.apply(ft.detach().clone().requires_grad_(True), el, er, g, H, Fo, 0.2, p, 3)
-    assert _relerr(other.detach().cpu(), out.detach().cpu()) < 1e-5
-    monkeypatch.setenv("BNS_GAT_ROWWALK", rowwalk)
     ops.RNG.update(offset=12)
     assert not torch.equal(GatAttention.apply(ft.detach(), el, er, g, H, Fo, 0.2, p, 3), out.detach())
     # keep rate: compare the total attention mass of every row (sum of a' over its entries ~ 1) via ft = ones
