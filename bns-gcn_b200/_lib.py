@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -144,6 +144,12 @@ SIGNATURES = {
     "bns_dropout_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_float, c_uint64, c_uint64, c_void_p, c_void_p,
                                 c_int64, c_void_p]),
     "bns_scale_rows_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    # ---- ABI 4 ----
+    "bns_spmm_sum_bf16": (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_void_p,
+                                  c_void_p, c_void_p, c_int64, c_int64, c_int32, c_int, c_void_p, c_size_t, c_void_p]),
+    "bns_spmm_compact_bf16": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_void_p,
+                                      c_int64, c_void_p, c_int64, c_int32, c_int, c_void_p, c_size_t, c_void_p]),
+    "bns_cvt_rows_f32_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
 

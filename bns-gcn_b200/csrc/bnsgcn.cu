@@ -3,6 +3,7 @@
 // Hot kernels (all HBM/L2-bound f32 gather / scatter work; no tensor-core shaped math here):
 //   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers
 //   spmm_fixup_kernel  deterministic combine of rows longer than one chunk
+//   spmm_bf16_kernel   the same row-sum over a bf16 gather table (--agg-dtype bf16), f32 sums; cvt_rows_bf16_kernel
 //   gather / scatter   K3/K5      boundary pack and gradient scatter-add
 //   philox_key / take  K6         counter-based exactly-k sampling (with cub radix sort)
 //   p2p_put_rows       K3+C1      pack straight into the peer's receive slab over NVLink + flag
@@ -10,6 +11,7 @@
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 --shared -Xcompiler -fPIC
 #include "bnsgcn.h"
 
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -708,8 +710,9 @@ int64_t l2_bytes() {
     return v;
 }
 
-// Widest column slab (in floats: 256, 128, 64 or 32) whose source slab  x_rows * slab * 4 B  fits the L2 budget.
-int pick_slab(int64_t F, int64_t x_rows, int32_t forced) {
+// Widest column slab (in elements: 256, 128, 64 or 32) whose source slab  x_rows * slab * elem_bytes  fits the L2
+// budget (elem_bytes: 4 for f32 tables, 2 for the bf16 tables of bns_spmm_sum_bf16).
+int pick_slab(int64_t F, int64_t x_rows, int32_t forced, int elem_bytes = 4) {
     if (forced == 256 || forced == 128 || forced == 64 || forced == 32) return forced;
     const char *env = getenv("BNS_SPMM_SLAB");
     if (env) {
@@ -719,7 +722,7 @@ int pick_slab(int64_t F, int64_t x_rows, int32_t forced) {
     // Full rows while they fit comfortably, else 128 floats (a slab about the size of L2 still wins: the slab-major
     // order keeps the hot part resident and halves the index re-reads of 64), else 64; never 32.  When even a
     // 64-float slab cannot be L2-resident the gather is a pure HBM stream and the widest slab is best.
-    const double l2 = (double)l2_bytes(), bytes_per_col = (double)x_rows * 4.0;
+    const double l2 = (double)l2_bytes(), bytes_per_col = (double)x_rows * (double)elem_bytes;
     const int fmax = F >= 256 ? 256 : (F > 64 ? 128 : 64);
     if (fmax >= 256 && bytes_per_col * 256.0 <= 0.55 * l2) return 256;
     if (fmax >= 128 && bytes_per_col * 128.0 <= 1.0 * l2) return 128;
@@ -840,6 +843,321 @@ extern "C" int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64
     a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
     a.n_tiles = 1;
     return spmm_dispatch(a, x_rows > 0 ? x_rows : g->n_cols, 0, as_stream(stream));
+}
+
+// =================================================================================================
+// SpMM with a BF16 gather table (--agg-dtype bf16): X rows are bf16, everything else as spmm_kernel
+// =================================================================================================
+namespace {
+
+// Eight bf16 values of one 16-byte load, summed into eight f32 accumulators (bf16 -> f32 is exact: a shift).
+struct Bf16x8 {
+    uint4 u;
+    __device__ __forceinline__ void zero() { u = make_uint4(0u, 0u, 0u, 0u); }
+    __device__ __forceinline__ void load_ro(const uint16_t *p) { u = __ldg(reinterpret_cast<const uint4 *>(p)); }
+};
+__device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+
+struct Acc8 {
+    float v[8];
+    __device__ __forceinline__ void zero() {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.f;
+    }
+    __device__ __forceinline__ void add(const Bf16x8 &x) {
+        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] += bf_lo(w[i]); v[2 * i + 1] += bf_hi(w[i]); }
+    }
+    __device__ __forceinline__ void fma(const Bf16x8 &x, float s) {
+        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] = fmaf(bf_lo(w[i]), s, v[2 * i]); v[2 * i + 1] = fmaf(bf_hi(w[i]), s, v[2 * i + 1]); }
+    }
+    __device__ __forceinline__ void scale(float s) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] *= s;
+    }
+    __device__ __forceinline__ void add_shfl_xor(int off) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], off);
+    }
+    __device__ __forceinline__ void add_f32(const float *p) {
+        const float4 a = *reinterpret_cast<const float4 *>(p), b = *reinterpret_cast<const float4 *>(p + 4);
+        v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+    }
+    __device__ __forceinline__ void store(float *p) const {
+        *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
+        *reinterpret_cast<float4 *>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
+    }
+};
+
+// spmm_kernel with bf16 rows of X (ldx in elements): lane l of row group gi owns the 8 columns f0 + gl * 8 .. + 8, one
+// 16-byte load per gathered row, so a 256-wide slab is one 512-byte request per warp and each lane keeps 8 f32
+// accumulators (as the f32 kernel's 256-wide slab).  Work decomposition, column mapping, compaction, the partial sums
+// of split rows (f32, combined by spmm_fixup_kernel) and the epilogue are those of spmm_kernel.
+template <int G, bool MAP, bool CSCALE, bool GUARD>
+__global__ void __launch_bounds__(kThreads, 4) spmm_bf16_kernel(SpmmArgs a, const uint16_t *__restrict__ Xh) {
+    constexpr int NG = 32 / G;
+    constexpr int UNROLL = 8;
+    constexpr int SLAB = G * 8;
+    __shared__ int32_t s_col[kWarps][32];
+    __shared__ float s_sc[kWarps][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int gi = lane / G, gl = lane % G;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    const int64_t items = a.n_chunks * a.n_tiles;
+    for (int64_t item = (int64_t)blockIdx.x * kWarps + w; item < items; item += warps_total) {
+        const int64_t c = item % a.n_chunks;
+        const int fcol = (int)(item / a.n_chunks) * SLAB + gl * 8;
+        const bool fok = !GUARD || fcol < a.F;
+        const int32_t row = a.chunk_row[c];
+        int32_t orow = row;
+        if (a.row_map) {
+            orow = a.row_map[row];
+            if (orow < 0) continue;
+        }
+        const int64_t s = a.chunk_start[c];
+        int64_t e;
+        if (a.chunk_cnt) {
+            const int32_t cnt = a.chunk_cnt[c];
+            if (cnt == 0 && a.accumulate && a.chunk_part[c] < 0) continue;
+            e = s + cnt;
+        } else {
+            e = a.indptr[row + 1];
+            if (e > s + a.chunk_nnz) e = s + a.chunk_nnz;
+        }
+        Acc8 acc;
+        acc.zero();
+        for (int64_t k0 = s; k0 < e; k0 += 32) {
+            const int64_t k = k0 + lane;
+            int32_t col = -1;
+            float sc = 1.f;
+            if (k < e) {
+                col = ld_stream_i32(a.indices + k);
+                if (CSCALE) {
+                    if (a.col_scale) sc = __ldg(a.col_scale + col);
+                    if (a.edge_weight) sc *= __ldg(a.edge_weight + (a.edge_perm ? (int64_t)__ldg(a.edge_perm + k) : k) * a.edge_ld);
+                }
+                if (MAP) {
+                    if (col >= a.n_direct) col = __ldg(a.col_map + (col - a.n_direct));
+                }
+            }
+            int cnt;
+            if (MAP) {
+                const unsigned m = __ballot_sync(0xffffffffu, col >= 0);
+                cnt = __popc(m);
+                if (col >= 0) {
+                    const int pos = __popc(m & ((1u << lane) - 1u));
+                    s_col[w][pos] = col;
+                    if (CSCALE) s_sc[w][pos] = sc;
+                }
+            } else {
+                const int64_t rem = e - k0;
+                cnt = rem < 32 ? (int)rem : 32;
+                s_col[w][lane] = col;
+                if (CSCALE) s_sc[w][lane] = sc;
+            }
+            __syncwarp();
+            int j = 0;
+            for (; j + NG * UNROLL <= cnt; j += NG * UNROLL) {
+                Bf16x8 v[UNROLL];
+#pragma unroll
+                for (int u = 0; u < UNROLL; ++u) {
+                    if (fok) v[u].load_ro(Xh + (int64_t)s_col[w][j + u * NG + gi] * a.ldx + fcol); else v[u].zero();
+                }
+#pragma unroll
+                for (int u = 0; u < UNROLL; ++u) {
+                    if (CSCALE) acc.fma(v[u], s_sc[w][j + u * NG + gi]); else acc.add(v[u]);
+                }
+            }
+            for (; j < cnt; j += NG) {
+                const int jj = j + gi;
+                if (jj < cnt && fok) {
+                    Bf16x8 v;
+                    v.load_ro(Xh + (int64_t)s_col[w][jj] * a.ldx + fcol);
+                    if (CSCALE) acc.fma(v, s_sc[w][jj]); else acc.add(v);
+                }
+            }
+            __syncwarp();
+        }
+        if (NG > 1) {
+#pragma unroll
+            for (int off = 16; off >= G; off >>= 1) acc.add_shfl_xor(off);
+            if (gi != 0) continue;
+        }
+        if (!fok) continue;
+        const int32_t part = a.chunk_part[c];
+        if (part >= 0) {
+            acc.store(a.ws + (int64_t)part * a.ldws + fcol);
+        } else {
+            float *yr = a.Y + (int64_t)orow * a.ldy + fcol;
+            if (a.row_scale) acc.scale(a.row_scale[row]);
+            if (a.accumulate) acc.add_f32(yr);
+            acc.store(yr);
+        }
+    }
+}
+
+template <int G, bool MAP, bool CSCALE, bool GUARD>
+int launch_spmm_bf16(SpmmArgs a, const uint16_t *Xh, cudaStream_t st) {
+    static std::atomic<int> occ[kMaxDevices];
+    const int dev = current_device();
+    int blocks_per_sm = occ[dev].load(std::memory_order_relaxed);
+    if (blocks_per_sm == 0) {
+        int n = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spmm_bf16_kernel<G, MAP, CSCALE, GUARD>, kThreads, 0) !=
+                cudaSuccess || n < 1)
+            n = 2;
+        blocks_per_sm = n;
+        occ[dev].store(n, std::memory_order_relaxed);
+    }
+    constexpr int SLAB = G * 8;
+    a.n_tiles = (a.F + SLAB - 1) / SLAB;
+    const int64_t items = a.n_chunks * a.n_tiles;
+    int64_t want = (items + kWarps - 1) / kWarps;
+    int64_t cap = (int64_t)sm_count() * blocks_per_sm;
+    unsigned gx = (unsigned)(want < cap ? (want > 0 ? want : 1) : cap);
+    spmm_bf16_kernel<G, MAP, CSCALE, GUARD><<<gx, kThreads, 0, st>>>(a, Xh);
+    g_launches += a.n_split > 0 ? 2 : 1;
+    if (a.n_split > 0) {    // the partial sums are f32 rows: the f32 kernel's fix-up pass combines them
+        unsigned fx = (unsigned)((a.n_split + kWarps - 1) / kWarps);
+        spmm_fixup_kernel<4, 2, true><<<dim3(fx, (a.F + 255) / 256), kThreads, 0, st>>>(a);
+    }
+    return BNS_OK;
+}
+
+template <int G>
+int dispatch_bf16_flags(const SpmmArgs &a, const uint16_t *Xh, cudaStream_t st) {
+    const bool map = a.col_map != nullptr, cs = a.col_scale != nullptr || a.edge_weight != nullptr;
+    if ((a.F % (G * 8)) != 0) {
+        if (map && cs) return launch_spmm_bf16<G, true, true, true>(a, Xh, st);
+        if (map) return launch_spmm_bf16<G, true, false, true>(a, Xh, st);
+        if (cs) return launch_spmm_bf16<G, false, true, true>(a, Xh, st);
+        return launch_spmm_bf16<G, false, false, true>(a, Xh, st);
+    }
+    if (map && cs) return launch_spmm_bf16<G, true, true, false>(a, Xh, st);
+    if (map) return launch_spmm_bf16<G, true, false, false>(a, Xh, st);
+    if (cs) return launch_spmm_bf16<G, false, true, false>(a, Xh, st);
+    return launch_spmm_bf16<G, false, false, false>(a, Xh, st);
+}
+
+int spmm_bf16_dispatch(const SpmmArgs &a, const uint16_t *Xh, int64_t x_rows, int32_t slab_hint, cudaStream_t st) {
+    int slab = pick_slab(a.F, x_rows, slab_hint, sizeof(uint16_t));
+    while (slab > 32 && slab / 2 >= a.F) slab >>= 1;
+    switch (slab) {
+        case 256: dispatch_bf16_flags<32>(a, Xh, st); break;
+        case 128: dispatch_bf16_flags<16>(a, Xh, st); break;
+        case 64:  dispatch_bf16_flags<8>(a, Xh, st); break;
+        default:  dispatch_bf16_flags<4>(a, Xh, st); break;
+    }
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// the 16-byte gathers and the 2 x 16-byte stores of the bf16 kernel
+#define BNS_BF16_LAYOUT(fn)                                                                                            \
+    BNS_REQUIRE(F % 8 == 0 && ldx % 8 == 0 && ldy % 4 == 0 &&                                                          \
+                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
+                fn ": needs F %% 8 == 0, ldx %% 8 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "   \
+                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
+
+__global__ void __launch_bounds__(kThreads) cvt_rows_bf16_kernel(const float *__restrict__ src, int64_t lds,
+                                                                 uint16_t *__restrict__ dst, int64_t ldd, int64_t n_rows,
+                                                                 int64_t F, bool vec) {
+    const int64_t per_row = vec ? F / 4 : F, total = n_rows * per_row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / per_row, c = i - r * per_row;
+        if (vec) {
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(src + r * lds) + c);
+            uint2 o;
+            o.x = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.x)) |
+                  ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.y)) << 16);
+            o.y = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.z)) |
+                  ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.w)) << 16);
+            reinterpret_cast<uint2 *>(dst + r * ldd)[c] = o;
+        } else {
+            dst[r * ldd + c] = __bfloat16_as_ushort(__float2bfloat16_rn(__ldg(src + r * lds + c)));
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
+                                 const float *row_scale, const float *col_scale, const float *edge_weight,
+                                 const int32_t *row_map, const int32_t *col_map, int64_t n_direct, int64_t x_rows,
+                                 int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes, void *stream) {
+    BNS_REQUIRE(g, "bns_spmm_sum_bf16: NULL graph");
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_sum_bf16: bad feature width %lld", (long long)F);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(Y, "bns_spmm_sum_bf16: NULL output matrix");
+    BNS_REQUIRE(X || g->nnz == 0, "bns_spmm_sum_bf16: NULL input matrix");
+    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_sum_bf16: leading dimension smaller than F");
+    BNS_BF16_LAYOUT("bns_spmm_sum_bf16");
+    const size_t need = bns_spmm_workspace_bytes(g, F);
+    if (need > 0 && (ws == nullptr || ws_bytes < need))
+        return fail(BNS_E_WORKSPACE, "bns_spmm_sum_bf16: workspace %zu bytes < %zu needed", ws_bytes, need);
+    if (col_map == nullptr) n_direct = g->n_cols;
+    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_bf16: n_direct out of range");
+    if (x_rows <= 0) x_rows = g->n_cols;
+    SpmmArgs a;
+    a.indptr = g->indptr; a.indices = g->indices;
+    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = nullptr;
+    a.split_row = g->split_row; a.split_part = g->split_part;
+    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
+    a.X = nullptr; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
+    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
+    a.edge_perm = nullptr; a.edge_ld = 1;
+    a.n_direct = (int32_t)n_direct; a.accumulate = accumulate ? 1 : 0;
+    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
+    a.n_tiles = 1;
+    return spmm_bf16_dispatch(a, X, x_rows, slab_hint, as_stream(stream));
+}
+
+extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
+                                     const int32_t *chunk_cnt, const uint16_t *X, int64_t ldx, int64_t F, float *Y,
+                                     int64_t ldy, const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate,
+                                     void *ws, size_t ws_bytes, void *stream) {
+    BNS_REQUIRE(g && cidx && chunk_cnt, "bns_spmm_compact_bf16: NULL argument");
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_compact_bf16: bad feature width %lld", (long long)F);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(Y && (X || g->nnz == 0), "bns_spmm_compact_bf16: NULL matrix");
+    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_compact_bf16: leading dimension smaller than F");
+    BNS_BF16_LAYOUT("bns_spmm_compact_bf16");
+    const size_t need = bns_spmm_workspace_bytes(g, F);
+    if (need > 0 && (ws == nullptr || ws_bytes < need))
+        return fail(BNS_E_WORKSPACE, "bns_spmm_compact_bf16: workspace %zu bytes < %zu needed", ws_bytes, need);
+    SpmmArgs a;
+    a.indptr = g->indptr; a.indices = cidx;
+    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = chunk_cnt;
+    a.split_row = g->split_row; a.split_part = g->split_part;
+    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
+    a.X = nullptr; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
+    a.row_scale = row_scale; a.col_scale = nullptr; a.edge_weight = cw; a.row_map = nullptr; a.col_map = nullptr;
+    a.edge_perm = nullptr; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
+    a.n_direct = (int32_t)g->n_cols; a.accumulate = accumulate ? 1 : 0;
+    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
+    a.n_tiles = 1;
+    return spmm_bf16_dispatch(a, X, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+}
+
+extern "C" int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *dst, int64_t ldd, int64_t n_rows, int64_t F,
+                                     void *stream) {
+    BNS_REQUIRE(n_rows >= 0 && F >= 0 && lds >= F && ldd >= F, "bns_cvt_rows_f32_bf16: bad shape");
+    if (n_rows == 0 || F == 0) return BNS_OK;
+    BNS_REQUIRE(src && dst, "bns_cvt_rows_f32_bf16: NULL matrix");
+    const bool vec = F % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 16 == 0 &&
+                     reinterpret_cast<uintptr_t>(dst) % 8 == 0;
+    const int64_t work = n_rows * (vec ? F / 4 : F);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const int64_t want = (work + kThreads - 1) / kThreads;
+    cvt_rows_bf16_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, dst, ldd,
+                                                                                                   n_rows, F, vec);
+    g_launches += 1;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
 }
 
 // =================================================================================================

@@ -311,22 +311,30 @@ class PPLinearFn(torch.autograd.Function):
         return dx, None, None, None, None, None
 
 
-def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready) -> torch.Tensor:
+def _gather_table(x: torch.Tensor, bf16: bool) -> torch.Tensor:
+    """What an aggregation pass gathers: ``x`` itself, or (``--agg-dtype bf16``) its rows rounded to bf16."""
+    return ops.cvt_rows_bf16(x) if bf16 else x
+
+
+def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf16: bool = False) -> torch.Tensor:
     """``rs * (A_in x_u[:n_in] + A_out[:, sampled] x_u[n_in:])`` -- the inner pass first (it needs local rows only), the
-    halo pass after the exchange's event."""
-    y = ops.spmm_auto(g.a_in, x_u[:g.n_in], row_scale=rs)
+    halo pass after the exchange's event.  ``bf16``: both passes gather bf16 copies of the rows (f32 sums)."""
+    y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16), row_scale=rs)
     if ready is not None:
         torch.cuda.current_stream(x_u.device).wait_event(ready)
     if g.a_out is not None and x_u.shape[0] > g.n_in:
-        halo_aggregate(g, x_u[g.n_in:], y, rs, None)
+        halo_aggregate(g, _gather_table(x_u[g.n_in:], bf16), y, rs, None)
     return y
 
 
-def _aggregate_t(g: PartitionGraph, dys: torch.Tensor, n_u: int, cs_in=None, cs_halo=None, after_halo=None) -> torch.Tensor:
+def _aggregate_t(g: PartitionGraph, dys: torch.Tensor, n_u: int, cs_in=None, cs_halo=None, after_halo=None,
+                 bf16: bool = False) -> torch.Tensor:
     """``cs * (A^T dys)`` over the epoch's graph: ``[n_u, F]`` (inner rows, then the sampled halo rows); ``cs``: GCN's
     per-source scale (1/sqrt(out_deg)), applied as the row scale of the transposed products.  The halo rows come first;
-    ``after_halo(du)`` is called as soon as they are final (the gradient return trip starts there)."""
+    ``after_halo(du)`` is called as soon as they are final (the gradient return trip starts there).  ``bf16``: both
+    passes gather one bf16 copy of ``dys``."""
     du = torch.empty(n_u, dys.shape[1], dtype=torch.float32, device=dys.device)
+    dys = _gather_table(dys, bf16)
     if n_u > g.n_in:
         tail = du[g.n_in:]
         tail.zero_()
@@ -373,7 +381,7 @@ class SageConvFn(torch.autograd.Function):
                 halo_aggregate(g, t[n_in:], out, rs, None)                      # ... + (A_out t_halo) / deg
             ctx.save_for_backward(h_u)
         else:
-            ah = _aggregate(g, h_u, rs, ready)                                  # [n_in, in]
+            ah = _aggregate(g, h_u, rs, ready, g.agg_bf16)                      # [n_in, in]
             t = dense.tc_mm_tn(ah, W2, arena.padded(b2))
             out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t)
             ctx.save_for_backward(h_u, ah)
@@ -409,7 +417,7 @@ class SageConvFn(torch.autograd.Function):
             h_u, ah = ctx.saved_tensors
             n_u = h_u.shape[0]
             dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs)          # (dout W2) / deg
-            du = _aggregate_t(g, dys, n_u, after_halo=begin)
+            du = _aggregate_t(g, dys, n_u, after_halo=begin, bf16=g.agg_bf16)
             dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1))
             dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2))
         inner = du[:n_in]
@@ -446,11 +454,12 @@ class GcnConvFn(torch.autograd.Function):
             out = scale_rows(s, rs, bias=bp)                                                          # / in_norm + b
             ctx.save_for_backward(h_u)
         else:
-            y = ops.spmm_auto(g.a_in, scale_rows(h_u[:n_in], cs_in), row_scale=rs)
+            bf16 = g.agg_bf16
+            y = ops.spmm_auto(g.a_in, _gather_table(scale_rows(h_u[:n_in], cs_in), bf16), row_scale=rs)
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             if has_halo:
-                halo_aggregate(g, h_u[n_in:], y, rs, cs_halo)
+                halo_aggregate(g, _gather_table(h_u[n_in:], bf16), y, rs, cs_halo)
             out = dense.tc_mm_tn(y, W, bp)
             ctx.save_for_backward(y)
         ctx.n_u = h_u.shape[0]
@@ -474,7 +483,7 @@ class GcnConvFn(torch.autograd.Function):
             (y,) = ctx.saved_tensors
             dense.tc_mm_nt(dout, y, out=a.grad_padded(w))
             dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs)           # (dout W) / in_norm
-            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo)
+            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, bf16=g.agg_bf16)
         return du, None, None, None, None, None, None, None, None
 
 

@@ -65,6 +65,12 @@ def build_parser():
                         help="NEW: with --eval, every rank evaluates its own nodes on its partition (the whole halo "
                              "exchanged layer by layer) instead of rank 0 evaluating the full graph alone; the full "
                              "graph is never built.  Transductive runs only")
+    parser.add_argument(*_spellings("agg-dtype"), default="f32", choices=["f32", "bf16"],
+                        help="NEW: element type of the rows the wide (hidden-width) aggregation passes gather.  bf16 "
+                             "rounds them to bf16 (nearest even) before each pass -- h_u forward, the transposed "
+                             "passes' input gradient backward -- and sums in f32: half the gathered bytes, and results "
+                             "that no longer match the reference to 1e-4.  Only with the fused training step "
+                             "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
     return parser
 
 

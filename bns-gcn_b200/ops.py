@@ -125,8 +125,13 @@ def spmm(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *,
          row_scale: Optional[torch.Tensor] = None, col_scale: Optional[torch.Tensor] = None,
          row_map: Optional[torch.Tensor] = None, col_map: Optional[torch.Tensor] = None, n_direct: int = 0,
          accumulate: bool = False, slab: int = 0, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``bns_spmm_sum_f32``: ``out[orow(r)] (+)= row_scale[r] * sum_k col_scale[c_k] * x[xrow(c_k)]``."""
-    _req(x, torch.float32, "x")
+    """``bns_spmm_sum_f32``: ``out[orow(r)] (+)= row_scale[r] * sum_k col_scale[c_k] * x[xrow(c_k)]``.  A bf16 ``x``
+    (``cvt_rows_bf16``) takes ``bns_spmm_sum_bf16``: the same sum, accumulated and written in f32."""
+    bf16 = x.dtype == torch.bfloat16
+    if not bf16:
+        _req(x, torch.float32, "x")
+    elif not x.is_cuda:
+        raise _lib.BnsError("x must be a CUDA tensor (there is no CPU path)")
     if x.dim() != 2 or x.stride(1) != 1:
         raise _lib.BnsError("x must be a row-major 2-D tensor")
     F = x.shape[1]
@@ -147,15 +152,16 @@ def spmm(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *,
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(torch.cuda.current_stream(x.device))
+    fn, name = (lib.bns_spmm_sum_bf16, "bns_spmm_sum_bf16") if bf16 else (lib.bns_spmm_sum_f32, "bns_spmm_sum_f32")
     with torch.cuda.device(x.device):
-        check(lib.bns_spmm_sum_f32(g._h, x.data_ptr(), x.stride(0), F, out.data_ptr(), out.stride(0),
-                                   _ptr(row_scale), _ptr(col_scale), _ptr(edge_weight), _ptr(row_map), _ptr(col_map),
-                                   n_direct, x.shape[0], slab, 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()),
-              "bns_spmm_sum_f32")
+        check(fn(g._h, x.data_ptr(), x.stride(0), F, out.data_ptr(), out.stride(0),
+                 _ptr(row_scale), _ptr(col_scale), _ptr(edge_weight), _ptr(row_map), _ptr(col_map),
+                 n_direct, x.shape[0], slab, 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()),
+              name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(x.device))
         # SURVEY.md §8(d): every distinct operand byte once -- row offsets, column ids, source rows, output rows
-        alg = 8 * (g.n_rows + 1) + 4 * g.nnz + 4 * F * x.shape[0] + 4 * F * out.shape[0]
+        alg = 8 * (g.n_rows + 1) + 4 * g.nnz + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
         # entries whose source row is really gathered: all of them, or (sampled halo) the mapped fraction
         live = g.nnz
         if col_map is not None and g.n_cols > n_direct:
@@ -176,15 +182,15 @@ BLOCK_MIN_AVG_DEGREE = 64
 BLOCK_MAX = 4
 
 
-def plan_col_blocks(g: DeviceGraph, F: int) -> int:
-    """Number of source-row blocks for width ``F`` (1 = no blocking)."""
+def plan_col_blocks(g: DeviceGraph, F: int, elem_bytes: int = 4) -> int:
+    """Number of source-row blocks for width ``F`` (1 = no blocking); ``elem_bytes``: 4 for an f32 table, 2 for bf16."""
     import os
     forced = os.environ.get("BNS_SPMM_COLBLOCKS")
     if forced:
         return max(1, int(forced))
     if F < 128 or g.n_rows == 0 or g.nnz / max(g.n_rows, 1) < BLOCK_MIN_AVG_DEGREE:
         return 1
-    b = -(-g.n_cols * 512 // BLOCK_TABLE_BYTES)
+    b = -(-g.n_cols * 128 * elem_bytes // BLOCK_TABLE_BYTES)     # a 128-column slab of every source row
     return b if 1 < b <= BLOCK_MAX else 1
 
 
@@ -209,7 +215,7 @@ def spmm_auto(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = Non
     per block, each accumulating into ``out``.  Counts as ONE launch in bench.py's roofline bookkeeping."""
     global PROFILE
     F = x.shape[1]
-    nb = plan_col_blocks(g, F)
+    nb = plan_col_blocks(g, F, x.element_size())
     if nb <= 1:
         return spmm(g, x, out, row_scale=row_scale, n_out_rows=n_out_rows, accumulate=accumulate, col_scale=col_scale)
     blocks = g.__dict__.get("_col_blocks")
@@ -227,7 +233,7 @@ def spmm_auto(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = Non
                  col_scale=None if col_scale is None else col_scale[c0:c1])
         if prof is not None:
             ev1.record(torch.cuda.current_stream(x.device))
-            alg = 8 * (g.n_rows + 1) + 4 * g.nnz + 4 * F * x.shape[0] + 4 * F * out.shape[0]
+            alg = 8 * (g.n_rows + 1) + 4 * g.nnz + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
             prof.append((ev0, ev1, alg, g.nnz, F, g.nnz))
     finally:
         PROFILE = prof
@@ -261,9 +267,12 @@ def spmm_compact(c: CompactedCols, x: torch.Tensor, out: torch.Tensor, *, row_sc
                  accumulate: bool = False, slab: int = 0, live_nnz: Optional[int] = None,
                  weights: Optional[torch.Tensor] = None, head: int = 0) -> torch.Tensor:
     """``bns_spmm_compact_f32``: the SpMM over the compacted (sampled) entries only.  ``weights`` ``[nnz, heads]`` at
-    the COMPACTED positions (GAT's dropped attention, column ``head``) replaces the compaction's own per-entry weights."""
+    the COMPACTED positions (GAT's dropped attention, column ``head``) replaces the compaction's own per-entry weights.
+    A bf16 ``x`` takes ``bns_spmm_compact_bf16``."""
     g = c.g
-    _req(x, torch.float32, "x")
+    bf16 = x.dtype == torch.bfloat16
+    if not bf16:
+        _req(x, torch.float32, "x")
     _req(out, torch.float32, "out")
     if x.dim() != 2 or x.stride(1) != 1 or out.stride(1) != 1 or out.shape[1] != x.shape[1]:
         raise _lib.BnsError("x / out must be row-major [*, F]")
@@ -275,15 +284,16 @@ def spmm_compact(c: CompactedCols, x: torch.Tensor, out: torch.Tensor, *, row_sc
         ev0.record(torch.cuda.current_stream(x.device))
     with torch.cuda.device(x.device):
         cw_ptr, cw_ld = (_ptr(c.cw), 1) if weights is None else (weights.data_ptr() + 4 * head, weights.stride(0))
-        check(lib.bns_spmm_compact_f32(g._h, c.cidx.data_ptr(), cw_ptr, cw_ld, c.chunk_cnt.data_ptr(), x.data_ptr(), x.stride(0),
-                                       F, out.data_ptr(), out.stride(0), _ptr(row_scale), x.shape[0], slab,
-                                       1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()),
-              "bns_spmm_compact_f32")
+        fn, name = ((lib.bns_spmm_compact_bf16, "bns_spmm_compact_bf16") if bf16 else
+                    (lib.bns_spmm_compact_f32, "bns_spmm_compact_f32"))
+        check(fn(g._h, c.cidx.data_ptr(), cw_ptr, cw_ld, c.chunk_cnt.data_ptr(), x.data_ptr(), x.stride(0),
+                 F, out.data_ptr(), out.stride(0), _ptr(row_scale), x.shape[0], slab,
+                 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()), name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(x.device))
         live = int(g.nnz * min(1.0, x.shape[0] / max(g.n_cols, 1))) if live_nnz is None else live_nnz
         # algorithmic bytes of the SAMPLED product: its live entries, the rows of X it can reference, the output rows
-        alg = 8 * (g.n_rows + 1) + 4 * live + 4 * F * x.shape[0] + 4 * F * out.shape[0]
+        alg = 8 * (g.n_rows + 1) + 4 * live + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
         prof.append((ev0, ev1, alg, live, F, live))
     return out
 
@@ -373,6 +383,24 @@ def copy_rows(src: torch.Tensor, dst: torch.Tensor, n_rows: int) -> None:
     with torch.cuda.device(src.device):
         check(lib.bns_copy_rows_f32(src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), n_rows,
                                     src.shape[1], _stream_ptr()), "bns_copy_rows_f32")
+
+
+def cvt_rows_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``bns_cvt_rows_f32_bf16``: ``src`` rounded to bf16 (nearest even), into ``out`` or a new ``[rows, F]`` matrix whose
+    row stride is a multiple of 8 elements (16 bytes: what the bf16 SpMM gathers)."""
+    _req(src, torch.float32, "src")
+    if src.dim() != 2 or src.stride(1) != 1:
+        raise _lib.BnsError("src must be a row-major 2-D tensor")
+    n, F = src.shape
+    if out is None:
+        out = torch.empty(n, (F + 7) // 8 * 8, dtype=torch.bfloat16, device=src.device)[:, :F]
+    _req(out, torch.bfloat16, "out")
+    if out.shape != src.shape or out.stride(1) != 1:
+        raise _lib.BnsError("out must be row-major with the shape of src")
+    with torch.cuda.device(src.device):
+        check(lib.bns_cvt_rows_f32_bf16(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0), n, F, _stream_ptr()),
+              "bns_cvt_rows_f32_bf16")
+    return out
 
 
 class BoundarySampler:

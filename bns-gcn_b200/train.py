@@ -347,6 +347,38 @@ def _fused_eligible(args, layer_size, dev) -> bool:
     return widths_ok and len(layer_size) >= 3
 
 
+def check_agg_dtype(args, layer_size, dev) -> bool:
+    """Whether ``--agg-dtype bf16`` is on.  It only exists on the fused training step: any configuration that step does
+    not take raises ``ValueError`` naming why, rather than training in f32 behind the user's back."""
+    import os
+    from .module import dense
+    mode = getattr(args, 'agg_dtype', 'f32')
+    if mode == 'f32':
+        return False
+    if mode != 'bf16':
+        raise ValueError(f"--agg-dtype {mode!r}: expected 'f32' or 'bf16'")
+    why = []
+    if os.environ.get("BNS_FUSED", "1") == "0":
+        why.append("BNS_FUSED=0 turns the fused training step off")
+    if args.model not in ('graphsage', 'gcn'):
+        why.append(f"--model {args.model} (only graphsage and gcn have the fused step)")
+    if not args.use_pp:
+        why.append("no --use-pp")
+    if args.n_linear != 0:
+        why.append(f"--n-linear {args.n_linear}")
+    if args.norm != 'layer':
+        why.append(f"--norm {args.norm}")
+    if dev.type != "cuda" or dense.MODE != "tc":
+        why.append("no CUDA device with the wgmma GEMMs")
+    if any(w % 8 for w in layer_size[1:-1]):
+        why.append(f"hidden width {args.n_hidden} is not a multiple of 8 (bf16 rows are gathered 8 at a time)")
+    if not why and not _fused_eligible(args, layer_size, dev):
+        why.append("the layer widths do not fit the fused step")
+    if why:
+        raise ValueError("--agg-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
+    return True
+
+
 def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     """Everything ``run`` does before its epoch loop (train.py:300-383)."""
     rank, size = _rank_size()
@@ -357,6 +389,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     part.want_positions = args.model == 'gat'          # the fused attention keeps per-entry values at CSR positions
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
+    part.agg_bf16 = check_agg_dtype(args, layer_size, dev)
     _, _, _, node_dict, boundary = move_to_cuda(graph, in_graph, out_graph, node_dict, boundary, dev)
     print(f'Process {rank} has {graph.num_nodes()} nodes, {graph.num_edges()} edges '
           f'{in_graph.n_rows} inner nodes, and {in_graph.nnz} inner edges.')

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 3
+#define BNS_ABI_VERSION 4
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -310,6 +310,24 @@ int bns_spmm_compact_f32(const bns_graph_t *g, const int32_t *cidx, const float 
                          const int32_t *chunk_cnt, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                          const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes,
                          void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 4: BF16 gather tables (--agg-dtype bf16).  bns_spmm_sum_bf16 / bns_spmm_compact_bf16 are bns_spmm_sum_f32 /
+ * bns_spmm_compact_f32 with X stored as bf16 bit patterns (ldx in elements): every other operand, the accumulation
+ * (f32, same entry order) and Y stay f32.  X is read as 16-byte vectors of 8 elements: F % 8 == 0, ldx % 8 == 0,
+ * ldy % 4 == 0 and 16-byte aligned X, Y, else BNS_E_INVALID (there is no scalar path).  The column slab is sized from
+ * x_rows * slab * 2 bytes; the workspace is the f32 one (bns_spmm_workspace_bytes).
+ * bns_cvt_rows_f32_bf16: dst[r, :F] = bf16(src[r, :F]), round to nearest even (NaN stays NaN, subnormals are kept).
+ * ----------------------------------------------------------------------------------------------*/
+int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X /*bf16*/, int64_t ldx, int64_t F, float *Y, int64_t ldy,
+                      const float *row_scale, const float *col_scale, const float *edge_weight, const int32_t *row_map,
+                      const int32_t *col_map, int64_t n_direct, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws,
+                      size_t ws_bytes, void *stream);
+int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld, const int32_t *chunk_cnt,
+                          const uint16_t *X /*bf16*/, int64_t ldx, int64_t F, float *Y, int64_t ldy, const float *row_scale,
+                          int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes, void *stream);
+int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *dst /*bf16*/, int64_t ldd, int64_t n_rows, int64_t F,
+                          void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K10 fused: the attention of dgl.nn.GATConv (module/model.py:96-132; DGL 0.9 python/dgl/nn/pytorch/conv/gatconv.py):
