@@ -212,6 +212,11 @@ def test_dense_split_k_plan_is_sane_without_a_gpu(built):
         kb = (R + 31) // 32
         assert 1 <= splits <= kb
         assert (kb + splits - 1) // splits <= 48 + 5, (R, n1, n2, splits)      # <= 48 up to the -10 % wave rounding
+    # contractions of more than 1,024 x 48 k-blocks (the papers100M per-rank rows): never above 48 k-blocks per slice
+    for R, n1, n2 in [(111_059_956 // 8, 256, 256), (111_059_956 // 8, 44, 256), (2_000_000, 256, 1204)]:
+        kb = (R + 31) // 32
+        splits = f(R, n1, n2) // (n1 * n2 * 4)
+        assert splits >= (kb + 47) // 48 > 1024, (R, n1, n2, splits)
     assert _lib.lib.bns_colsum_workspace_bytes(256) == 132 * 4 * 64 * 16
 
 
