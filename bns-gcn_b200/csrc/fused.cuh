@@ -511,12 +511,101 @@ __global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDe
     }
 }
 
+// ---- bf16 boundary exchange (--comm-dtype bf16): 8 elements per lane and 16-byte access, no scalar path ----
+
+__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
+    return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(lo)) |
+           ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(hi)) << 16);
+}
+__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+
+// bf16(src[0:8] / div) as one 16-byte word (the division in f32, then one rounding)
+__device__ __forceinline__ uint4 div_round8(const float *src, float div) {
+    const float4 a = *reinterpret_cast<const float4 *>(src), b = *reinterpret_cast<const float4 *>(src + 4);
+    uint4 o;
+    o.x = bf16x2_rn(__fdiv_rn(a.x, div), __fdiv_rn(a.y, div));
+    o.y = bf16x2_rn(__fdiv_rn(a.z, div), __fdiv_rn(a.w, div));
+    o.z = bf16x2_rn(__fdiv_rn(b.x, div), __fdiv_rn(b.y, div));
+    o.w = bf16x2_rn(__fdiv_rn(b.z, div), __fdiv_rn(b.w, div));
+    return o;
+}
+
+// (a, b) += widen(r) / div, each element as the f32 siblings add it
+__device__ __forceinline__ void add_div8(float4 &a, float4 &b, uint4 r, float div) {
+    a.x += __fdiv_rn(bf16_lo(r.x), div); a.y += __fdiv_rn(bf16_hi(r.x), div);
+    a.z += __fdiv_rn(bf16_lo(r.y), div); a.w += __fdiv_rn(bf16_hi(r.y), div);
+    b.x += __fdiv_rn(bf16_lo(r.z), div); b.y += __fdiv_rn(bf16_hi(r.z), div);
+    b.z += __fdiv_rn(bf16_lo(r.w), div); b.w += __fdiv_rn(bf16_hi(r.w), div);
+}
+
+// p2p_put_all_kernel with the remote rows stored as bf16 (remote / ld_remote in bf16 elements)
+__global__ void __launch_bounds__(kThreads) p2p_put_all_bf16_kernel(PutAllDev a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
+        int s = 0;
+        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
+        const int64_t local = i - a.row_begin[s];
+        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
+        const float *src = a.H + r * a.ldh;
+        uint16_t *d = reinterpret_cast<uint16_t *>(a.remote[s]) + local * a.ld_remote;
+        for (int f = lane * 8; f < a.F; f += 256) *reinterpret_cast<uint4 *>(d + f) = div_round8(src + f, a.div[s]);
+    }
+    __threadfence_system();
+    __syncthreads();
+    __shared__ bool s_last;
+    if (threadIdx.x == 0) {
+        const unsigned int done = atomicAdd(a.ticket, 1u);
+        s_last = (done == gridDim.x - 1);
+        if (s_last) atomicExch(a.ticket, 0u);
+    }
+    __syncthreads();
+    if (s_last && (int)threadIdx.x < a.n_seg) {
+        __threadfence_system();
+        st_release_sys(a.flag[threadIdx.x], a.flag_value + (a.flag_value_dev ? *a.flag_value_dev : 0ull));
+    }
+}
+
+// scatter_rows_all_kernel reading bf16 recv rows (ld_recv in bf16 elements): same order, same per-element arithmetic
+__global__ void __launch_bounds__(kThreads) scatter_rows_all_bf16_kernel(ScatterAllDev a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < a.n_rows; row += warps_total) {
+        int32_t mine = -1;
+        if (lane < a.n_seg) mine = a.inv[lane][row];
+        if (__ballot_sync(0xffffffffu, mine >= 0) == 0u) continue;
+        float *g = a.G + row * a.ldg;
+        for (int f0 = 0; f0 < a.F; f0 += 256) {                 // warp-uniform: every lane takes every shuffle
+            const int f = f0 + lane * 8;
+            const bool on = f < a.F;
+            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+            if (on) {
+                v0 = *reinterpret_cast<const float4 *>(g + f);
+                v1 = *reinterpret_cast<const float4 *>(g + f + 4);
+            }
+            for (int s = 0; s < a.n_seg; ++s) {
+                const int32_t k = __shfl_sync(0xffffffffu, mine, s);
+                if (k < 0 || !on) continue;
+                const uint16_t *r = reinterpret_cast<const uint16_t *>(a.recv[s]) + (int64_t)k * a.ld_recv + f;
+                add_div8(v0, v1, *reinterpret_cast<const uint4 *>(r), a.div[s]);
+            }
+            if (on) {
+                *reinterpret_cast<float4 *>(g + f) = v0;
+                *reinterpret_cast<float4 *>(g + f + 4) = v1;
+            }
+        }
+    }
+}
+
 }  // namespace
 
 namespace {
 // see bns_p2p_create: a kernel's first launch loads its code, which synchronises the context -- never while a flag wait spins
 void preload_exchange_kernels() {
     cudaFuncAttributes fa;
+    cudaFuncGetAttributes(&fa, p2p_put_all_bf16_kernel);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_bf16_kernel);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<true>);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<false>);
     cudaFuncGetAttributes(&fa, p2p_put_ids_kernel);
@@ -641,6 +730,179 @@ extern "C" int bns_scatter_rows_all_f32(float *G, int64_t ldg, int64_t n_rows, i
     a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
     if (vec) scatter_rows_all_kernel<true><<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
     else scatter_rows_all_kernel<false><<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_p2p_put_all_bf16(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
+                                    int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
+                                    uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
+    BNS_REQUIRE(p && segs, "bns_p2p_put_all_bf16: NULL argument");
+    BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "bns_p2p_put_all_bf16: too many segments");
+    BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "bns_p2p_put_all_bf16: bad flag index");
+    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "bns_p2p_put_all_bf16: bad ticket index");
+    BNS_REQUIRE(F > 0 && ldh >= F && ld_remote >= F, "bns_p2p_put_all_bf16: bad shape");
+    BNS_REQUIRE(F % 8 == 0 && ldh % 8 == 0 && ld_remote % 8 == 0,
+                "bns_p2p_put_all_bf16: F, ldh and ld_remote must be multiples of 8 (F %lld, ldh %lld, ld_remote %lld)",
+                (long long)F, (long long)ldh, (long long)ld_remote);
+    if (segs->n_seg == 0) return BNS_OK;
+    PutAllDev a;
+    a.n_seg = segs->n_seg;
+    for (int s = 0; s <= segs->n_seg; ++s) a.row_begin[s] = segs->row_begin[s];
+    for (int s = 0; s < segs->n_seg; ++s) {
+        const int peer = segs->peer[s];
+        const int64_t k = segs->row_begin[s + 1] - segs->row_begin[s];
+        BNS_REQUIRE(peer >= 0 && peer < p->world && peer != p->rank, "bns_p2p_put_all_bf16: bad peer %d", peer);
+        BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "bns_p2p_put_all_bf16: peer %d not connected", peer);
+        BNS_REQUIRE(k >= 0, "bns_p2p_put_all_bf16: negative row count");
+        BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "bns_p2p_put_all_bf16: division by zero");
+        BNS_REQUIRE(segs->remote_off[s] % 16 == 0 &&
+                        segs->remote_off[s] + (size_t)k * ld_remote * 2 <= p->peer_slab_bytes[peer],
+                    "bns_p2p_put_all_bf16: remote range of segment %d outside peer %d's slab or not 16-byte aligned", s,
+                    peer);
+        a.remote[s] = reinterpret_cast<float *>(p->peer_slab[peer] + segs->remote_off[s]);
+        a.flag[s] = p->peer_flags[peer] + flag_index;
+        a.src_begin[s] = segs->src_begin[s];
+        a.div[s] = k == 0 ? 1.f : segs->div[s];
+    }
+    const int64_t total = segs->row_begin[segs->n_seg];
+    BNS_REQUIRE(total == 0 || H, "bns_p2p_put_all_bf16: NULL source");
+    BNS_REQUIRE((reinterpret_cast<uintptr_t>(H) & 15u) == 0, "bns_p2p_put_all_bf16: source not 16-byte aligned");
+    a.H = H; a.ldh = ldh; a.F = (int32_t)F; a.idx = idx_cat; a.ld_remote = ld_remote;
+    a.flag_value = flag_value; a.flag_value_dev = reinterpret_cast<const unsigned long long *>(flag_value_dev);
+    a.ticket = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(p->flags) + align256((size_t)p->n_flags * 8)) + ticket_index;
+    p2p_put_all_bf16_kernel<<<rows_grid(total), kThreads, 0, as_stream(stream)>>>(a);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_scatter_rows_all_bf16(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
+                                         const int32_t *const *inv, const uint16_t *const *recv, int64_t ld_recv,
+                                         const float *div, void *stream) {
+    BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "bns_scatter_rows_all_bf16: too many segments");
+    if (n_seg == 0 || n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(G && inv && recv && div && F > 0 && ldg >= F && ld_recv >= F, "bns_scatter_rows_all_bf16: bad argument");
+    BNS_REQUIRE(F % 8 == 0 && ldg % 4 == 0 && ld_recv % 8 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0,
+                "bns_scatter_rows_all_bf16: needs F %% 8 == 0, ldg %% 4 == 0, ld_recv %% 8 == 0 and a 16-byte aligned G "
+                "(F %lld, ldg %lld, ld_recv %lld)", (long long)F, (long long)ldg, (long long)ld_recv);
+    ScatterAllDev a;
+    a.n_seg = n_seg;
+    for (int s = 0; s < n_seg; ++s) {
+        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f && (reinterpret_cast<uintptr_t>(recv[s]) & 15u) == 0,
+                    "bns_scatter_rows_all_bf16: bad segment %d (NULL, misaligned or division by zero)", s);
+        a.inv[s] = inv[s]; a.recv[s] = reinterpret_cast<const float *>(recv[s]); a.div[s] = div[s];
+    }
+    a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
+    scatter_rows_all_bf16_kernel<<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// ---- the staged transport's pack (K3) and scatter (K5) with a bf16 wire side, and the exact widening ----
+namespace {
+
+// out[i] = bf16(H[idx[i]] / div): one warp per row
+__global__ void __launch_bounds__(kThreads) gather_div_bf16_kernel(const float *__restrict__ H, int64_t ldh,
+                                                                   uint16_t *__restrict__ out, int64_t ldo,
+                                                                   const int64_t *__restrict__ idx, int64_t k, int32_t F,
+                                                                   float div) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
+        const float *s = H + idx[i] * ldh;
+        uint16_t *d = out + i * ldo;
+        for (int f = lane * 8; f < F; f += 256) *reinterpret_cast<uint4 *>(d + f) = div_round8(s + f, div);
+    }
+}
+
+// G[idx[i]] += widen(src[i]) / div: one warp per row (the ids of one call are distinct)
+__global__ void __launch_bounds__(kThreads) scatter_add_div_bf16_kernel(const uint16_t *__restrict__ src, int64_t lds,
+                                                                        float *G, int64_t ldg,
+                                                                        const int64_t *__restrict__ idx, int64_t k,
+                                                                        int32_t F, float div) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
+        const uint16_t *s = src + i * lds;
+        float *d = G + idx[i] * ldg;
+        for (int f = lane * 8; f < F; f += 256) {
+            float4 v0 = *reinterpret_cast<const float4 *>(d + f), v1 = *reinterpret_cast<const float4 *>(d + f + 4);
+            add_div8(v0, v1, *reinterpret_cast<const uint4 *>(s + f), div);
+            *reinterpret_cast<float4 *>(d + f) = v0;
+            *reinterpret_cast<float4 *>(d + f + 4) = v1;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) cvt_rows_bf16_f32_kernel(const uint16_t *__restrict__ src, int64_t lds,
+                                                                     float *__restrict__ dst, int64_t ldd, int64_t n_rows,
+                                                                     int64_t F, bool vec) {
+    const int64_t per_row = vec ? F / 4 : F, total = n_rows * per_row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / per_row, c = i - r * per_row;
+        if (vec) {
+            const uint2 w = __ldg(reinterpret_cast<const uint2 *>(src + r * lds) + c);
+            reinterpret_cast<float4 *>(dst + r * ldd)[c] = make_float4(bf16_lo(w.x), bf16_hi(w.x), bf16_lo(w.y), bf16_hi(w.y));
+        } else {
+            dst[r * ldd + c] = __uint_as_float((uint32_t)__ldg(src + r * lds + c) << 16);
+        }
+    }
+}
+
+inline bool bf16_rows_ok(const void *f32, const void *b16, int64_t F, int64_t ld32, int64_t ld16) {
+    return F % 8 == 0 && ld32 % 8 == 0 && ld16 % 8 == 0 &&
+           ((reinterpret_cast<uintptr_t>(f32) | reinterpret_cast<uintptr_t>(b16)) % 16) == 0;
+}
+
+}  // namespace
+
+extern "C" int bns_gather_div_bf16(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
+                                   uint16_t *out, int64_t ldo, void *stream) {
+    BNS_REQUIRE(k >= 0 && F > 0, "bns_gather_div_bf16: bad size");
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(H && out && idx, "bns_gather_div_bf16: NULL pointer");
+    BNS_REQUIRE(ldh >= F && ldo >= F, "bns_gather_div_bf16: leading dimension smaller than F");
+    BNS_REQUIRE(div != 0.f, "bns_gather_div_bf16: division by zero");
+    BNS_REQUIRE(bf16_rows_ok(H, out, F, ldh, ldo),
+                "bns_gather_div_bf16: needs F, ldh, ldo multiples of 8 and 16-byte aligned H, out (F %lld, ldh %lld, "
+                "ldo %lld)", (long long)F, (long long)ldh, (long long)ldo);
+    gather_div_bf16_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
+                                        const uint16_t *src, int64_t lds, void *stream) {
+    BNS_REQUIRE(k >= 0 && F > 0, "bns_scatter_add_div_bf16: bad size");
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(G && src && idx, "bns_scatter_add_div_bf16: NULL pointer");
+    BNS_REQUIRE(ldg >= F && lds >= F, "bns_scatter_add_div_bf16: leading dimension smaller than F");
+    BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_bf16: division by zero");
+    BNS_REQUIRE(bf16_rows_ok(G, src, F, ldg, lds),
+                "bns_scatter_add_div_bf16: needs F, ldg, lds multiples of 8 and 16-byte aligned G, src (F %lld, "
+                "ldg %lld, lds %lld)", (long long)F, (long long)ldg, (long long)lds);
+    scatter_add_div_bf16_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_cvt_rows_bf16_f32(const uint16_t *src, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
+                                     void *stream) {
+    BNS_REQUIRE(n_rows >= 0 && F >= 0 && lds >= F && ldd >= F, "bns_cvt_rows_bf16_f32: bad shape");
+    if (n_rows == 0 || F == 0) return BNS_OK;
+    BNS_REQUIRE(src && dst, "bns_cvt_rows_bf16_f32: NULL matrix");
+    const bool vec = F % 4 == 0 && lds % 4 == 0 && ldd % 4 == 0 && reinterpret_cast<uintptr_t>(src) % 8 == 0 &&
+                     reinterpret_cast<uintptr_t>(dst) % 16 == 0;
+    const int64_t work = n_rows * (vec ? F / 4 : F);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const int64_t want = (work + kThreads - 1) / kThreads;
+    cvt_rows_bf16_f32_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, dst, ldd,
+                                                                                                       n_rows, F, vec);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

@@ -316,15 +316,41 @@ def _gather_table(x: torch.Tensor, bf16: bool) -> torch.Tensor:
     return ops.cvt_rows_bf16(x) if bf16 else x
 
 
-def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf16: bool = False) -> torch.Tensor:
+def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf16: bool = False,
+               halo: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``rs * (A_in x_u[:n_in] + A_out[:, sampled] x_u[n_in:])`` -- the inner pass first (it needs local rows only), the
-    halo pass after the exchange's event.  ``bf16``: both passes gather bf16 copies of the rows (f32 sums)."""
+    halo pass after the exchange's event.  ``bf16``: both passes gather bf16 copies of the rows (f32 sums).  ``halo``:
+    the halo rows as they arrived in bf16 (``--comm-dtype bf16``; ``x_u`` is then the inner rows alone), gathered as
+    they are."""
     y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16), row_scale=rs)
     if ready is not None:
         torch.cuda.current_stream(x_u.device).wait_event(ready)
-    if g.a_out is not None and x_u.shape[0] > g.n_in:
+    if halo is not None:
+        if g.a_out is not None and halo.shape[0]:
+            halo_aggregate(g, halo, y, rs, None)
+    elif g.a_out is not None and x_u.shape[0] > g.n_in:
         halo_aggregate(g, _gather_table(x_u[g.n_in:], bf16), y, rs, None)
     return y
+
+
+def _halo_rows(h_u: torch.Tensor, n_in: int, halo: Optional[torch.Tensor]) -> torch.Tensor:
+    """The f32 halo rows a narrow layer transforms: ``h_u[n_in:]``, or (``--comm-dtype bf16``) the received bf16 rows
+    widened into a matrix of their own -- the inner rows stay where they are."""
+    return h_u[n_in:] if halo is None else ops.cvt_rows_f32(halo)
+
+
+def _weight_grad(dt: torch.Tensor, saved, n_in: int, out: torch.Tensor) -> None:
+    """``dt^T h_u`` into ``out``.  ``saved``: ``(h_u,)``, or ``(h_in, h_halo)`` when the halo rows are kept apart
+    (``--comm-dtype bf16``): the inner rows' product, then the halo rows' product added (one f32 add per element)."""
+    if len(saved) == 1:
+        dense.tc_mm_nt(dt, saved[0], out=out)
+        return
+    h_in, h_halo = saved
+    dense.tc_mm_nt(dt[:n_in], h_in, out=out)
+    if h_halo.shape[0]:
+        part = dense.tc_mm_nt(dt[n_in:], h_halo)
+        rows = torch.arange(out.shape[0], dtype=torch.int64, device=out.device)
+        ops.scatter_add_div(out, rows, part, 1.0)                      # x / 1 is x: an exact row-wise add
 
 
 def _aggregate_t(g: PartitionGraph, dys: torch.Tensor, n_u: int, cs_in=None, cs_halo=None, after_halo=None,
@@ -358,10 +384,11 @@ class SageConvFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, h_u, w1, b1, w2, b2, g: PartitionGraph, rs, ready, arena: ParamArena, narrow_first: bool,
-                exchange=None):
+                exchange=None, halo=None):
         """``exchange = (Buffer, layer)`` when ``h_u`` came out of ``Buffer.update``: the backward then hands the halo
-        rows of its gradient to ``Buffer.begin_backward`` as soon as they are final."""
-        ctx.exchange = exchange
+        rows of its gradient to ``Buffer.begin_backward`` as soon as they are final.  ``halo``: the received halo rows in
+        bf16 (``--comm-dtype bf16``); ``h_u`` is then the inner rows alone, and so is the returned gradient."""
+        ctx.exchange, ctx.inner_only = exchange, halo is not None
         n_in = g.n_in
         h_u = h_u.contiguous()
         W1, W2 = arena.padded(w1), arena.padded(w2)
@@ -369,22 +396,24 @@ class SageConvFn(torch.autograd.Function):
         if narrow_first:
             # transform, then aggregate; the local rows go first -- their GEMM and the inner-edge pass need nothing from
             # the peers and hide the exchange -- the halo rows after the exchange's event
-            n_u = h_u.shape[0]
+            n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
             t = gather_friendly(n_u, W2.shape[0], h_u.device)                   # [n_u, out_p]
             dense.tc_mm_tn(h_in, W2, out=t[:n_in])
             out = dense.tc_mm_tn(h_in, W1, arena.bias_sum(b1, b2))              # linear1(h) + b1 + b2 ...
             ops.spmm_auto(g.a_in, t[:n_in], out, row_scale=rs, accumulate=True)  # ... + (A_in t) / deg
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
+            h_halo = _halo_rows(h_u, n_in, halo)
             if g.a_out is not None and n_u > n_in:
-                dense.tc_mm_tn(h_u[n_in:], W2, out=t[n_in:])
+                dense.tc_mm_tn(h_halo, W2, out=t[n_in:])
                 halo_aggregate(g, t[n_in:], out, rs, None)                      # ... + (A_out t_halo) / deg
-            ctx.save_for_backward(h_u)
+            ctx.save_for_backward(*((h_u,) if halo is None else (h_in, h_halo)))
         else:
-            ah = _aggregate(g, h_u, rs, ready, g.agg_bf16)                      # [n_in, in]
+            ah = _aggregate(g, h_u, rs, ready, g.agg_bf16, halo)                # [n_in, in]
             t = dense.tc_mm_tn(ah, W2, arena.padded(b2))
             out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t)
             ctx.save_for_backward(h_u, ah)
+        ctx.n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
         ctx.g, ctx.rs, ctx.arena, ctx.narrow = g, rs, arena, narrow_first
         ctx.params = (w1, b1, w2, b2)
         return out
@@ -401,28 +430,27 @@ class SageConvFn(torch.autograd.Function):
             buf, layer = ctx.exchange
             begin = lambda du_: buf.begin_backward(layer, du_)      # noqa: E731
         if ctx.narrow:
-            (h_u,) = ctx.saved_tensors
-            n_u = h_u.shape[0]
+            saved = ctx.saved_tensors
+            h_in, n_u = saved[0][:n_in], ctx.n_u
             dys = scale_rows(dout, rs, out=gather_friendly(n_in, dout.shape[1], dout.device))
             dt = _aggregate_t(g, dys, n_u)                                      # [n_u, out_p]
-            du = torch.empty(n_u, h_u.shape[1], dtype=torch.float32, device=dout.device)
+            du = torch.empty(n_u, h_in.shape[1], dtype=torch.float32, device=dout.device)
             if n_u > n_in:                                                      # halo rows first: they travel ...
                 dense.tc_mm_tn(dt[n_in:], a.transposed(w2), out=du[n_in:])
             if begin is not None:
                 begin(du)
             dense.tc_mm_tn(dt[:n_in], a.transposed(w2), out=du[:n_in])          # ... while the local rows are computed
-            dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1))
-            dense.tc_mm_nt(dt, h_u, out=a.grad_padded(w2))
+            dense.tc_mm_nt(dout, h_in, out=a.grad_padded(w1))
+            _weight_grad(dt, saved, n_in, a.grad_padded(w2))
         else:
             h_u, ah = ctx.saved_tensors
-            n_u = h_u.shape[0]
             dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs)          # (dout W2) / deg
-            du = _aggregate_t(g, dys, n_u, after_halo=begin, bf16=g.agg_bf16)
+            du = _aggregate_t(g, dys, ctx.n_u, after_halo=begin, bf16=g.agg_bf16)
             dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1))
             dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2))
         inner = du[:n_in]
         dense.tc_mm_tn(dout, a.transposed(w1), addend=inner, out=inner)         # += dout W1, in place
-        return du, None, None, None, None, None, None, None, None, None, None
+        return inner if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None, None
 
 
 class GcnConvFn(torch.autograd.Function):
@@ -435,34 +463,39 @@ class GcnConvFn(torch.autograd.Function):
     compaction as per-entry weights (``PartitionGraph.halo_col_scale``)."""
 
     @staticmethod
-    def forward(ctx, h_u, w, b, g: PartitionGraph, rs, cs_u, ready, arena: ParamArena, narrow_first: bool):
+    def forward(ctx, h_u, w, b, g: PartitionGraph, rs, cs_u, ready, arena: ParamArena, narrow_first: bool,
+                exchange=None, halo=None):
+        """``exchange`` / ``halo``: as for ``SageConvFn`` (``--comm-dtype bf16``)."""
+        ctx.exchange, ctx.inner_only = exchange, halo is not None
         n_in = g.n_in
         h_u = h_u.contiguous()
         W, bp = arena.padded(w), arena.padded(b)
         cs_in, cs_halo = cs_u[:n_in], cs_u[n_in:]
-        has_halo = g.a_out is not None and h_u.shape[0] > n_in
+        n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
+        has_halo = g.a_out is not None and n_u > n_in
         if narrow_first:
-            t = gather_friendly(h_u.shape[0], W.shape[0], h_u.device)                                 # [n_u, out_p]
+            t = gather_friendly(n_u, W.shape[0], h_u.device)                                          # [n_u, out_p]
             dense.tc_mm_tn(h_u[:n_in], W, out=t[:n_in])                                               # local rows first
             ts = scale_rows(t[:n_in], cs_in, out=gather_friendly(n_in, W.shape[0], h_u.device))
             s = ops.spmm_auto(g.a_in, ts)                                                             # raw sums
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
+            h_halo = _halo_rows(h_u, n_in, halo)
             if has_halo:
-                dense.tc_mm_tn(h_u[n_in:], W, out=t[n_in:])
+                dense.tc_mm_tn(h_halo, W, out=t[n_in:])
                 halo_aggregate(g, t[n_in:], s, None, cs_halo)
             out = scale_rows(s, rs, bias=bp)                                                          # / in_norm + b
-            ctx.save_for_backward(h_u)
+            ctx.save_for_backward(*((h_u,) if halo is None else (h_u[:n_in], h_halo)))
         else:
             bf16 = g.agg_bf16
             y = ops.spmm_auto(g.a_in, _gather_table(scale_rows(h_u[:n_in], cs_in), bf16), row_scale=rs)
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             if has_halo:
-                halo_aggregate(g, _gather_table(h_u[n_in:], bf16), y, rs, cs_halo)
+                halo_aggregate(g, halo if halo is not None else _gather_table(h_u[n_in:], bf16), y, rs, cs_halo)
             out = dense.tc_mm_tn(y, W, bp)
             ctx.save_for_backward(y)
-        ctx.n_u = h_u.shape[0]
+        ctx.n_u = n_u
         ctx.g, ctx.rs, ctx.cs, ctx.arena, ctx.narrow, ctx.params = g, rs, (cs_in, cs_halo), arena, narrow_first, (w, b)
         return out
 
@@ -473,18 +506,23 @@ class GcnConvFn(torch.autograd.Function):
         w, b = ctx.params
         dout = dout.contiguous()
         dense.colsum(dout, out=a.grad_padded(b))
+        begin = None
+        if ctx.exchange is not None:
+            buf, layer = ctx.exchange
+            begin = lambda du_: buf.begin_backward(layer, du_)      # noqa: E731
         if ctx.narrow:
-            (h_u,) = ctx.saved_tensors
             dys = scale_rows(dout, rs, out=gather_friendly(g.n_in, dout.shape[1], dout.device))
             dt = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo)                  # [n_u, out_p]
-            dense.tc_mm_nt(dt, h_u, out=a.grad_padded(w))
+            _weight_grad(dt, ctx.saved_tensors, g.n_in, a.grad_padded(w))
             du = dense.tc_mm_tn(dt, a.transposed(w))                            # [n_u, in]
+            if begin is not None:
+                begin(du)
         else:
             (y,) = ctx.saved_tensors
             dense.tc_mm_nt(dout, y, out=a.grad_padded(w))
             dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs)           # (dout W) / in_norm
-            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, bf16=g.agg_bf16)
-        return du, None, None, None, None, None, None, None, None
+            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, after_halo=begin, bf16=g.agg_bf16)
+        return du[:g.n_in] if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None
 
 
 def sage_layer_eligible(layer, feat: torch.Tensor) -> bool:

@@ -11,6 +11,11 @@ Same surface -- ``init_buffer(num_in, ratio, f_send_shape, f_recv_shape, layer_s
   buffer through a peer-mapped pointer (NVLink 5 / NVSwitch) and raises a flag there (``bns_p2p_put_rows_f32`` /
   ``bns_p2p_wait_flag``): K3 + C1 fused, no staging copy, no NCCL launch.
 
+``comm_dtype='bf16'`` (``--comm-dtype bf16``, fused GraphSAGE / GCN step only): the sender rounds each boundary row
+``H[selected]/ratio`` -- and each returned gradient row -- to bf16 once, so the wire and the receiving slab carry half
+the bytes.  ``update`` then returns the inner rows ``[n_in, F]`` (f32, as given) with the received halo rows attached
+as ``_bns_halo`` (bf16 ``[recv_total, F]``), and the halo gradient travels only through ``begin_backward``.
+
 The exchange runs on ``self._comm_stream``; with ``update(..., overlap=True)`` the caller's stream does not wait
 for it -- the aggregation op waits on ``h_u._bns_ready`` right before it touches the halo rows, so the transfer
 hides behind the inner-edge SpMM.  ``Comm(s)`` is measured with CUDA events on that stream.
@@ -37,6 +42,41 @@ class _DevArray:
                                          "version": 2, "strides": None}
 
 
+def _a256(n: int) -> int:
+    return (n + 255) // 256 * 256
+
+
+def slab_layout(n_in, recv_total, send_total, width, n_comm_layers, comm_dtype='f32') -> dict:
+    """Byte layout of one rank's peer-mapped slab.  Per communicating layer: a forward region -- the ``n_in`` inner f32
+    rows, then the ``recv_total`` received halo rows -- and a backward region of the ``send_total`` gradient rows this
+    rank gets back; the received id lists close the slab.  With bf16 the halo and backward rows are bf16 and every
+    sub-region starts on 256 bytes.  ``*_bytes``: the size of each region (one layer)."""
+    if comm_dtype == 'bf16':
+        inner, halo, bwd = _a256(n_in * width * 4), _a256(max(recv_total, 1) * width * 2), _a256(max(send_total, 1) * width * 2)
+        stride = inner + halo + bwd
+        fwd_off = [l * stride for l in range(n_comm_layers)]
+        halo_off = [o + inner for o in fwd_off]
+        bwd_off = [o + halo for o in halo_off]
+        ids_off = n_comm_layers * stride
+    else:
+        row = width * 4
+        inner, halo, bwd = n_in * row, recv_total * row, max(send_total, 1) * row
+        fwd_off = [l * (inner + halo + bwd) for l in range(n_comm_layers)]
+        halo_off = [o + inner for o in fwd_off]
+        bwd_off = [o + inner + halo for o in fwd_off]
+        ids_off = _a256(n_comm_layers * (inner + halo + bwd))
+    return {"fwd_off": fwd_off, "halo_off": halo_off, "bwd_off": bwd_off, "ids_off": ids_off,
+            "slab_bytes": ids_off + max(recv_total, 1) * 8, "inner_bytes": inner, "halo_bytes": halo, "bwd_bytes": bwd}
+
+
+def wire_bytes(send_total, recv_total, F, comm_dtype='f32') -> dict:
+    """Feature bytes one rank moves per communicating layer and epoch: forward it sends its ``send_total`` sampled rows
+    and receives ``recv_total`` halo rows; backward the reverse."""
+    e = 2 if comm_dtype == 'bf16' else 4
+    return {"fwd_send": send_total * F * e, "fwd_recv": recv_total * F * e,
+            "bwd_send": recv_total * F * e, "bwd_recv": send_total * F * e}
+
+
 class Buffer(object):
 
     def __init__(self):
@@ -58,6 +98,7 @@ class Buffer(object):
         self.seq_dev = None
         self.seq_base = 0
         self._maps = None
+        self._bf16 = False
 
     # helper/feature_buffer.py:23-33
     def __init_pl_pr(self):
@@ -74,9 +115,11 @@ class Buffer(object):
         self._n_u = tot
 
     def init_buffer(self, num_in, ratio, f_send_shape, f_recv_shape, layer_size, use_pp=False, backend='nccl',
-                    device=None):
+                    device=None, comm_dtype='f32'):
         if use_pp is False:
             raise NotImplementedError            # helper/feature_buffer.py:36-37
+        if comm_dtype not in ('f32', 'bf16'):
+            raise ValueError(f"comm_dtype {comm_dtype!r}: expected 'f32' or 'bf16'")
         c = ctx.comm()
         # captured now: backward runs on autograd's device thread, where thread-local lookups would miss
         self._comm, self._timer = c, comm_timer._get()
@@ -101,6 +144,10 @@ class Buffer(object):
             raise RuntimeError("Buffer needs a CUDA device: there is no CPU exchange path")
         width = self._layer_size[1]              # the reference sizes every slab with layer_size[1] (:54-55)
         self._width = width
+        self._bf16 = comm_dtype == 'bf16'
+        if self._bf16 and width % 8:
+            raise ValueError(f"comm_dtype bf16: exchanged width {width} is not a multiple of 8")
+        wire = torch.bfloat16 if self._bf16 else torch.float32
         self._comm_stream = torch.cuda.Stream(self._device)
         self._send_begin, tot = [], 0
         for j in range(self._size):
@@ -109,29 +156,32 @@ class Buffer(object):
         self._send_total = tot
         if backend == 'nccl':
             self._send_buf = [None if j == self._rank else
-                              torch.zeros(self._send_shape[j], width, device=self._device) for j in range(self._size)]
+                              torch.zeros(self._send_shape[j], width, dtype=wire, device=self._device)
+                              for j in range(self._size)]
             self._b_recv = [None if j == self._rank else
-                            torch.zeros(self._send_shape[j], width, device=self._device) for j in range(self._size)]
+                            torch.zeros(self._send_shape[j], width, dtype=wire, device=self._device)
+                            for j in range(self._size)]
+            # bf16: the halo gradient rows are rounded into this buffer before they are sent (f32 sends them in place)
+            self._b_send = (torch.zeros(max(self._n_u - num_in, 1), width, dtype=wire, device=self._device)
+                            if self._bf16 else None)
         else:
             self.__init_p2p(c, width)
 
     # ---- p2p slabs -------------------------------------------------------------------------------
     def __init_p2p(self, c, width):
         n_comm_layers = max(self._n_layers - 1, 1)
-        fwd_rows, bwd_rows = self._n_u, max(self._send_total, 1)
-        row_bytes = width * 4
         if self._size - 1 > MAX_PEERS:
             raise RuntimeError(f"p2p transport: at most {MAX_PEERS + 1} partitions (BNS_MAX_PEERS)")
-        self._fwd_off = [l * (fwd_rows + bwd_rows) * row_bytes for l in range(n_comm_layers)]
-        self._bwd_off = [o + fwd_rows * row_bytes for o in self._fwd_off]
-        # after the feature regions: the received id lists of the epoch (data_transfer NODE), int64 [sum of recv sizes]
-        self._ids_off = (n_comm_layers * (fwd_rows + bwd_rows) * row_bytes + 255) // 256 * 256
         self._hop_begin, tot = [], 0
         for j in range(self._size):
             self._hop_begin.append(tot)
             tot += 0 if j == self._rank else self._recv_shape[j]
         self._recv_total = tot
-        slab_bytes = self._ids_off + max(tot, 1) * 8
+        # after the feature regions: the received id lists of the epoch (data_transfer NODE), int64 [sum of recv sizes]
+        lay = slab_layout(self._num_in, tot, self._send_total, width, n_comm_layers, 'bf16' if self._bf16 else 'f32')
+        self._fwd_off, self._halo_off, self._bwd_off, self._ids_off = (lay["fwd_off"], lay["halo_off"], lay["bwd_off"],
+                                                                       lay["ids_off"])
+        slab_bytes = lay["slab_bytes"]
         self._n_comm_layers = n_comm_layers
         n_flags = (n_comm_layers * 2 + 1) * self._size          # (layer, direction, source) + (ids, source)
         # completion tickets of the all-peer puts: size + 2 (layer - 1) forward, + 1 backward, size + 2 n_comm_layers
@@ -144,7 +194,8 @@ class Buffer(object):
         check(lib.bns_p2p_local(h, ctypes.byref(slab), ctypes.byref(flags), ctypes.byref(nbytes)), "bns_p2p_local")
         self._slab_ptr = slab.value
         # publish: where peers must write inside MY slab (row offsets of their segment) + how to map my memory
-        my = {"fwd_off": self._fwd_off, "bwd_off": self._bwd_off, "pl": self._pl, "send_begin": self._send_begin,
+        my = {"fwd_off": self._fwd_off, "halo_off": self._halo_off, "bwd_off": self._bwd_off, "pl": self._pl,
+              "send_begin": self._send_begin,
               "ids_off": self._ids_off, "hop_begin": self._hop_begin, "slab_bytes": nbytes.value}
         if c.kind == "thread":
             my["ptrs"] = (slab.value, flags.value)
@@ -282,7 +333,10 @@ class Buffer(object):
     def _flag(self, layer, backward, src):
         return ((layer - 1) * 2 + (1 if backward else 0)) * self._size + src
 
-    def _slab_view(self, byte_off, rows):
+    def _slab_view(self, byte_off, rows, bf16=False):
+        if bf16:
+            return torch.as_tensor(_DevArray(self._slab_ptr + byte_off, (rows, self._width), "<i2"),
+                                   device=self._device).view(torch.bfloat16)
         return torch.as_tensor(_DevArray(self._slab_ptr + byte_off, (rows, self._width)), device=self._device)
 
     def input_slot(self, layer, rows, width):
@@ -313,6 +367,8 @@ class Buffer(object):
         if overlap:
             res._bns_ready = self._last_ready
         res._bns_exchange = (self, layer)          # lets a fused consumer start the gradient return trip early
+        if self._bf16:
+            res._bns_halo = self._last_halo        # the received rows, bf16: the layer gathers / widens them itself
         return res
 
     def _forward(self, layer, feat, overlap):
@@ -322,12 +378,20 @@ class Buffer(object):
         feat = feat.contiguous()
         main, cs = torch.cuda.current_stream(self._device), self._comm_stream
         ready = torch.cuda.Event()
-        if self._backend == 'nccl':
+        bf16, halo = self._bf16, None
+        if self._p2p is not None and F != self._width:
+            raise RuntimeError("p2p transport needs equal hidden widths")
+        if bf16:
+            # the inner rows go on as they are (no concat); the halo rows land in a bf16 table of their own
+            h_u, n_halo = feat, self._n_u - self._num_in
+            if self._backend == 'nccl':
+                halo = torch.empty(n_halo, F, dtype=torch.bfloat16, device=self._device)
+            else:
+                halo = self._slab_view(self._halo_off[layer - 1], max(n_halo, 1), bf16=True)[:n_halo]
+        elif self._backend == 'nccl':
             h_u = torch.empty(self._n_u, F, device=self._device)
         else:
-            h_u = self._slab_view(self._fwd_off[layer - 1], self._n_u)[:, :F] if F == self._width else None
-            if h_u is None:
-                raise RuntimeError("p2p transport needs equal hidden widths")
+            h_u = self._slab_view(self._fwd_off[layer - 1], self._n_u)[:, :F]
         if feat.data_ptr() != h_u.data_ptr():                          # (written in place by the producer: input_slot)
             ops.copy_rows(feat, h_u, self._num_in)                     # K4: the only copy of the concat
         start = torch.cuda.Event()
@@ -342,9 +406,10 @@ class Buffer(object):
                         if j == self._rank:
                             continue
                         send[j] = self._send_buf[j][:, :F] if F == self._width else \
-                            torch.empty(self._send_shape[j], F, device=self._device)
+                            torch.empty(self._send_shape[j], F, dtype=self._send_buf[j].dtype, device=self._device)
                         ops.gather_div(feat, self._selected[j], self._ratio[j], out=send[j])      # K3
-                        recv[j] = h_u[self._pl[j]:self._pr[j]]
+                        recv[j] = (halo[self._pl[j] - self._num_in:self._pr[j] - self._num_in] if bf16 else
+                                   h_u[self._pl[j]:self._pr[j]])
                     self._comm.alltoall(send, recv, tag=16 + layer)                               # C1/C2
                 else:
                     seq, seq_dev = self._seq_args(layer, False)
@@ -356,14 +421,18 @@ class Buffer(object):
                         segs.row_begin[s_] = tot
                         tot += self._send_shape[j]
                         segs.peer[s_] = j
-                        segs.remote_off[s_] = lay["fwd_off"][layer - 1] + lay["pl"][self._rank] * self._width * 4
+                        if bf16:
+                            segs.remote_off[s_] = lay["halo_off"][layer - 1] + lay["hop_begin"][self._rank] * self._width * 2
+                        else:
+                            segs.remote_off[s_] = lay["fwd_off"][layer - 1] + lay["pl"][self._rank] * self._width * 4
                         segs.div[s_] = float(self._ratio[j]) if self._send_shape[j] else 1.0
                     segs.row_begin[segs.n_seg] = tot
                     sel_cat = self._selected_cat
-                    check(lib.bns_p2p_put_all_f32(self._p2p, ctypes.byref(segs), self._width, feat.data_ptr(), feat.stride(0),
-                                                  F, sel_cat.data_ptr() if tot else None,
-                                                  self._flag(layer, False, self._rank), self._size + (layer - 1) * 2, seq,
-                                                  seq_dev, cs.cuda_stream), "bns_p2p_put_all_f32")
+                    put = "bns_p2p_put_all_bf16" if bf16 else "bns_p2p_put_all_f32"
+                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), self._width, feat.data_ptr(), feat.stride(0),
+                                            F, sel_cat.data_ptr() if tot else None,
+                                            self._flag(layer, False, self._rank), self._size + (layer - 1) * 2, seq,
+                                            seq_dev, cs.cuda_stream), put)
                     for j in self._peers:
                         self._post_put_event(j, 2000 + 2 * layer, cs)
                     for j in self._peers:
@@ -374,10 +443,10 @@ class Buffer(object):
             ready.record(cs)
         if not self.graph_mode:
             feat.record_stream(cs)
-            h_u.record_stream(cs)
+            (halo if bf16 else h_u).record_stream(cs)
         if not overlap:
             main.wait_event(ready)
-        self._last_ready = ready
+        self._last_ready, self._last_halo = ready, halo
         return h_u
 
     # ---- backward (the grad hook) -------------------------------------------------------------------
@@ -400,10 +469,18 @@ class Buffer(object):
         with torch.cuda.stream(cs):
             with self._timer_ctx(f'backward_{layer}', cs):
                 if self._backend == 'nccl':
-                    send = [None if j == self._rank else grad[self._pl[j]:self._pr[j]] for j in range(self._size)]
+                    # bf16: the sender rounds its halo gradient rows once, then sends them per peer
+                    rows = grad
+                    if self._bf16:
+                        halo = grad[self._num_in:]
+                        rows = (ops.cvt_rows_bf16(halo, out=self._b_send[:halo.shape[0]]) if F == self._width else
+                                ops.cvt_rows_bf16(halo))
+                    b0 = self._num_in if self._bf16 else 0
+                    send = [None if j == self._rank else rows[self._pl[j] - b0:self._pr[j] - b0] for j in range(self._size)]
                     recv = [None if j == self._rank else
                             (self._b_recv[j][:, :F] if F == self._width else
-                             torch.empty(self._send_shape[j], F, device=self._device)) for j in range(self._size)]
+                             torch.empty(self._send_shape[j], F, dtype=self._b_recv[j].dtype, device=self._device))
+                            for j in range(self._size)]
                     self._comm.alltoall(send, recv, tag=64 + layer)
                 else:
                     seq, seq_dev = self._seq_args(layer, True)
@@ -415,14 +492,15 @@ class Buffer(object):
                         segs.row_begin[s_] = tot
                         tot += self._recv_shape[j]
                         segs.peer[s_] = j
-                        segs.remote_off[s_] = lay["bwd_off"][layer - 1] + lay["send_begin"][self._rank] * self._width * 4
+                        segs.remote_off[s_] = (lay["bwd_off"][layer - 1] +
+                                               lay["send_begin"][self._rank] * self._width * (2 if self._bf16 else 4))
                         segs.src_begin[s_] = self._pl[j]
                         segs.div[s_] = 1.0
                     segs.row_begin[segs.n_seg] = tot
-                    check(lib.bns_p2p_put_all_f32(self._p2p, ctypes.byref(segs), self._width, grad.data_ptr(), grad.stride(0),
-                                                  F, None, self._flag(layer, True, self._rank),
-                                                  self._size + (layer - 1) * 2 + 1, seq, seq_dev, cs.cuda_stream),
-                          "bns_p2p_put_all_f32")
+                    put = "bns_p2p_put_all_bf16" if self._bf16 else "bns_p2p_put_all_f32"
+                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), self._width, grad.data_ptr(), grad.stride(0),
+                                            F, None, self._flag(layer, True, self._rank),
+                                            self._size + (layer - 1) * 2 + 1, seq, seq_dev, cs.cuda_stream), put)
                     for j in self._peers:
                         self._post_put_event(j, 2001 + 2 * layer, cs)
                     for j in self._peers:
@@ -431,7 +509,7 @@ class Buffer(object):
                     check(lib.bns_p2p_wait_all(self._p2p, len(self._peers), idx, seq, seq_dev, cs.cuda_stream),
                           "bns_p2p_wait_all")
                     recv = [None] * self._size
-                    bwd = self._slab_view(self._bwd_off[layer - 1], max(self._send_total, 1))
+                    bwd = self._slab_view(self._bwd_off[layer - 1], max(self._send_total, 1), bf16=self._bf16)
                     for j in self._peers:
                         recv[j] = bwd[self._send_begin[j]:self._send_begin[j] + self._send_shape[j], :F]
             done.record(cs)
@@ -450,6 +528,9 @@ class Buffer(object):
         begun, self._begun = getattr(self, "_begun", None), None
         if begun is not None and begun[0] == layer and begun[1] == grad.data_ptr():
             done, recv = begun[2]                     # the producer already sent the halo rows (begin_backward)
+        elif self._bf16:
+            raise RuntimeError("comm_dtype bf16: the layer that consumed the exchange must hand its halo gradient to "
+                               "Buffer.begin_backward (the fused GraphSAGE / GCN layers do)")
         else:
             done, recv = self._exchange_backward(layer, grad)
         main.wait_event(done)
@@ -465,11 +546,13 @@ class Buffer(object):
                 n = len(order)
                 inv = (ctypes.c_void_p * n)(*[self._inv[j].data_ptr() for j in order])
                 base = self._slab_ptr + self._bwd_off[layer - 1]
-                rcv = (ctypes.c_void_p * n)(*[base + self._send_begin[j] * self._width * 4 for j in order])
+                esz = 2 if self._bf16 else 4
+                rcv = (ctypes.c_void_p * n)(*[base + self._send_begin[j] * self._width * esz for j in order])
                 div = (ctypes.c_float * n)(*[float(self._ratio[j]) for j in order])
+                fn = "bns_scatter_rows_all_bf16" if self._bf16 else "bns_scatter_rows_all_f32"
                 with torch.cuda.device(self._device):
-                    check(lib.bns_scatter_rows_all_f32(inner.data_ptr(), inner.stride(0), self._num_in, F, n, inv, rcv,
-                                                       self._width, div, main.cuda_stream), "bns_scatter_rows_all_f32")
+                    check(getattr(lib, fn)(inner.data_ptr(), inner.stride(0), self._num_in, F, n, inv, rcv,
+                                           self._width, div, main.cuda_stream), fn)
         if trace is not None:
             trace[f"grad_h{layer}"] = inner.detach().clone()
         return inner

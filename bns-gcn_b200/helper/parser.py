@@ -71,6 +71,11 @@ def build_parser():
                              "passes' input gradient backward -- and sums in f32: half the gathered bytes, and results "
                              "that no longer match the reference to 1e-4.  Only with the fused training step "
                              "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+    parser.add_argument(*_spellings("comm-dtype"), default="f32", choices=["f32", "bf16"],
+                        help="NEW: element type of the boundary rows the training exchange moves.  bf16 rounds each "
+                             "sampled row H[selected]/ratio, and each returned halo gradient row, to bf16 (nearest even) "
+                             "at the sender: half the wire and slab bytes; the receiver widens and sums in f32.  Only "
+                             "with the fused training step (GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
     return parser
 
 

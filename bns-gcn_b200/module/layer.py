@@ -84,8 +84,11 @@ class GCNLayer(nn.Module):
                 return _f.PPLinearFn.apply(feat, self.linear.weight, self.linear.bias, arena, p, seed)
             out_f, in_f = self.linear.out_features, self.linear.in_features
             narrow = AGGREGATE_AFTER_TRANSFORM and out_f < in_f
+            # --comm-dtype bf16: the halo rows arrive apart from feat, and their gradient returns through the exchange
+            halo = getattr(feat, '_bns_halo', None)
             out = _f.GcnConvFn.apply(feat, self.linear.weight, self.linear.bias, graph, graph.recip(in_norm),
-                                     graph.recip(out_norm), getattr(feat, '_bns_ready', None), arena, narrow)
+                                     graph.recip(out_norm), getattr(feat, '_bns_ready', None), arena, narrow,
+                                     None if halo is None else getattr(feat, '_bns_exchange', None), halo)
             holder.value = out
             return out if out.shape[1] == out_f else out[:, :out_f]
         if self.training:
@@ -138,7 +141,7 @@ class GraphSAGELayer(nn.Module):
             narrow = AGGREGATE_AFTER_TRANSFORM and out_f < in_f
             out = _f.SageConvFn.apply(feat, self.linear1.weight, self.linear1.bias, self.linear2.weight,
                                       self.linear2.bias, graph, graph.recip(in_norm), getattr(feat, '_bns_ready', None),
-                                      arena, narrow, getattr(feat, '_bns_exchange', None))
+                                      arena, narrow, getattr(feat, '_bns_exchange', None), getattr(feat, '_bns_halo', None))
             holder.value = out                  # [n_in, ceil4(out_features)]
             return out if out.shape[1] == out_f else out[:, :out_f]
         if self.training:

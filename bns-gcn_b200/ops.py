@@ -355,27 +355,33 @@ class AggregateSum(torch.autograd.Function):
 
 
 def gather_div(h: torch.Tensor, idx: torch.Tensor, div: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``out[i] = h[idx[i]] / div`` (helper/feature_buffer.py:117)."""
+    """``out[i] = h[idx[i]] / div`` (helper/feature_buffer.py:117).  A bf16 ``out`` (``--comm-dtype bf16``) receives the
+    f32 quotient rounded to nearest even (``bns_gather_div_bf16``)."""
     _req(h, torch.float32, "h")
     _req(idx, torch.int64, "idx")
     k, F = idx.numel(), h.shape[1]
     if out is None:
         out = torch.empty(k, F, dtype=torch.float32, device=h.device)
+    fn = "bns_gather_div_bf16" if out.dtype == torch.bfloat16 else "bns_gather_div_f32"
+    if fn == "bns_gather_div_f32":
+        _req(out, torch.float32, "out")
     with torch.cuda.device(h.device):
-        check(lib.bns_gather_div_f32(h.data_ptr(), h.stride(0), F, idx.data_ptr(), k, float(div), out.data_ptr(),
-                                     out.stride(0), _stream_ptr()), "bns_gather_div_f32")
+        check(getattr(lib, fn)(h.data_ptr(), h.stride(0), F, idx.data_ptr(), k, float(div), out.data_ptr(),
+                               out.stride(0), _stream_ptr()), fn)
     return out
 
 
 def scatter_add_div(g: torch.Tensor, idx: torch.Tensor, src: torch.Tensor, div: float) -> torch.Tensor:
-    """``g[idx[i]] += src[i] / div`` in place (helper/feature_buffer.py:129)."""
+    """``g[idx[i]] += src[i] / div`` in place (helper/feature_buffer.py:129).  A bf16 ``src`` (``--comm-dtype bf16``)
+    is widened exactly before the f32 division and sum (``bns_scatter_add_div_bf16``)."""
     _req(g, torch.float32, "g")
-    _req(src, torch.float32, "src")
+    fn = "bns_scatter_add_div_bf16" if src.dtype == torch.bfloat16 else "bns_scatter_add_div_f32"
+    if fn == "bns_scatter_add_div_f32":
+        _req(src, torch.float32, "src")
     _req(idx, torch.int64, "idx")
     with torch.cuda.device(g.device):
-        check(lib.bns_scatter_add_div_f32(g.data_ptr(), g.stride(0), g.shape[1], idx.data_ptr(), idx.numel(),
-                                          float(div), src.data_ptr(), src.stride(0), _stream_ptr()),
-              "bns_scatter_add_div_f32")
+        check(getattr(lib, fn)(g.data_ptr(), g.stride(0), g.shape[1], idx.data_ptr(), idx.numel(), float(div),
+                               src.data_ptr(), src.stride(0), _stream_ptr()), fn)
     return g
 
 
@@ -400,6 +406,23 @@ def cvt_rows_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torc
     with torch.cuda.device(src.device):
         check(lib.bns_cvt_rows_f32_bf16(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0), n, F, _stream_ptr()),
               "bns_cvt_rows_f32_bf16")
+    return out
+
+
+def cvt_rows_f32(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``bns_cvt_rows_bf16_f32``: bf16 rows widened to f32 (exact), into ``out`` or a new ``[rows, F]`` matrix."""
+    _req(src, torch.bfloat16, "src")
+    if src.dim() != 2 or src.stride(1) != 1:
+        raise _lib.BnsError("src must be a row-major 2-D tensor")
+    n, F = src.shape
+    if out is None:
+        out = torch.empty(n, F, dtype=torch.float32, device=src.device)
+    _req(out, torch.float32, "out")
+    if out.shape != src.shape or out.stride(1) != 1:
+        raise _lib.BnsError("out must be row-major with the shape of src")
+    with torch.cuda.device(src.device):
+        check(lib.bns_cvt_rows_bf16_f32(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0), n, F, _stream_ptr()),
+              "bns_cvt_rows_bf16_f32")
     return out
 
 

@@ -379,6 +379,40 @@ def check_agg_dtype(args, layer_size, dev) -> bool:
     return True
 
 
+def check_comm_dtype(args, layer_size, dev) -> str:
+    """The element type of the boundary rows on the wire: ``'f32'``, or ``'bf16'`` (``--comm-dtype bf16``), which only
+    exists on the fused training step -- its layers take the halo rows as bf16 and hand their halo gradient back to the
+    exchange.  Any configuration that step does not take raises ``ValueError`` naming every reason."""
+    import os
+    from .module import dense
+    mode = getattr(args, 'comm_dtype', 'f32')
+    if mode == 'f32':
+        return mode
+    if mode != 'bf16':
+        raise ValueError(f"--comm-dtype {mode!r}: expected 'f32' or 'bf16'")
+    why = []
+    if os.environ.get("BNS_FUSED", "1") == "0":
+        why.append("BNS_FUSED=0 turns the fused training step off")
+    if args.model not in ('graphsage', 'gcn'):
+        why.append(f"--model {args.model} (only graphsage and gcn have the fused step)")
+    if not args.use_pp:
+        why.append("no --use-pp")
+    if args.n_linear != 0:
+        why.append(f"--n-linear {args.n_linear}")
+    if args.norm != 'layer':
+        why.append(f"--norm {args.norm}")
+    if dev.type != "cuda" or dense.MODE != "tc":
+        why.append("no CUDA device with the wgmma GEMMs")
+    bad = sorted({w for w in layer_size[1:-1] if w % 8})
+    if bad:
+        why.append(f"exchanged width {', '.join(map(str, bad))} is not a multiple of 8 (bf16 rows move 8 at a time)")
+    if not why and not _fused_eligible(args, layer_size, dev):
+        why.append("the layer widths do not fit the fused step")
+    if why:
+        raise ValueError("--comm-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
+    return mode
+
+
 def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     """Everything ``run`` does before its epoch loop (train.py:300-383)."""
     rank, size = _rank_size()
@@ -390,6 +424,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
     part.agg_bf16 = check_agg_dtype(args, layer_size, dev)
+    comm_dtype = check_comm_dtype(args, layer_size, dev)
     _, _, _, node_dict, boundary = move_to_cuda(graph, in_graph, out_graph, node_dict, boundary, dev)
     print(f'Process {rank} has {graph.num_nodes()} nodes, {graph.num_edges()} edges '
           f'{in_graph.n_rows} inner nodes, and {in_graph.nnz} inner edges.')
@@ -421,7 +456,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     recv_size = get_recv_size(node_dict, args.sampling_rate)
     ctx.buffer.init_buffer(in_graph.n_rows, ratio, send_size, recv_size,
                            layer_size[:args.n_layers - args.n_linear], use_pp=args.use_pp, backend=args.backend,
-                           device=dev)
+                           device=dev, comm_dtype=comm_dtype)
     if size > 1 and ctx.buffer._get()._p2p is not None:
         # slot map + the inverse maps of the gradient scatter in ONE allocation (one memset + one kernel per epoch)
         n_slot = max(graph.n_halo, 1)

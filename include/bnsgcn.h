@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 4
+#define BNS_ABI_VERSION 5
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -425,6 +425,33 @@ int bns_scatter_rows_all_f32(float *G, int64_t ldg, int64_t n_rows, int64_t F, i
                              const int32_t *const *inv /*host array of device pointers*/,
                              const float *const *recv /*host array of device pointers*/, int64_t ld_recv,
                              const float *div /*host*/, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 5: the boundary exchange with a bf16 wire side (--comm-dtype bf16).  Every division stays f32; the sender rounds
+ * its quotient once to bf16 (nearest even, NaN stays NaN, subnormals kept: bns_cvt_rows_f32_bf16's rule) and the
+ * receiver widens each row exactly before it divides and adds in f32.
+ * bns_p2p_put_all_bf16: bns_p2p_put_all_f32 with the remote rows stored as bf16 (ld_remote in bf16 elements); same
+ *     segments, flags and tickets.  F, ldh and ld_remote multiples of 8, H 16-byte aligned, every remote_off a multiple
+ *     of 16, else BNS_E_INVALID (there is no scalar path).
+ * bns_scatter_rows_all_bf16: bns_scatter_rows_all_f32 reading bf16 recv rows (ld_recv in elements), same order and
+ *     same per-element arithmetic.  F % 8 == 0, ldg % 4 == 0, ld_recv % 8 == 0, 16-byte aligned G and recv rows.
+ * bns_gather_div_bf16 / bns_scatter_add_div_bf16: bns_gather_div_f32 / bns_scatter_add_div_f32 (the staged transport's
+ *     pack and scatter) with a bf16 out / src.  F and both leading dimensions multiples of 8, 16-byte aligned matrices.
+ * bns_cvt_rows_bf16_f32: dst[r, :F] = (float)src[r, :F], exact.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_p2p_put_all_bf16(bns_p2p_t *p, const bns_put_all *segs /*host*/, int64_t ld_remote, const float *H, int64_t ldh,
+                         int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index, uint64_t flag_value,
+                         const uint64_t *flag_value_dev, void *stream);
+int bns_scatter_rows_all_bf16(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
+                              const int32_t *const *inv /*host array of device pointers*/,
+                              const uint16_t *const *recv /*host array of device pointers, bf16*/, int64_t ld_recv,
+                              const float *div /*host*/, void *stream);
+int bns_gather_div_bf16(const float *H, int64_t ldh, int64_t F, const int64_t *idx /*device [k]*/, int64_t k, float div,
+                        uint16_t *out /*bf16*/, int64_t ldo, void *stream);
+int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *idx /*device [k]*/, int64_t k, float div,
+                             const uint16_t *src /*bf16*/, int64_t lds, void *stream);
+int bns_cvt_rows_bf16_f32(const uint16_t *src /*bf16*/, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
+                          void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Loss and its gradient in one launch.  Replaces train.py:406-408 for the two losses of train.py:358-361:
