@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -159,6 +159,11 @@ SIGNATURES = {
     "bns_scatter_add_div_bf16": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float, c_void_p, c_int64,
                                          c_void_p]),
     "bns_cvt_rows_bf16_f32": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
+    # ---- ABI 6 ----
+    "bns_dense_tn_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                  c_int64, c_int64, c_int64, c_int64, c_void_p]),
+    "bns_dense_nt_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
+                                  c_void_p, c_size_t, c_void_p]),
 }
 
 

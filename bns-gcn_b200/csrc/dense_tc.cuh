@@ -50,6 +50,16 @@ constexpr int BAR_BYTES = 256;
 constexpr int SMEM_BYTES = kStages * RAW_BYTES + kOpBufs * OP_BYTES + BAR_BYTES + 1024;   // + slack to align to 1024
 constexpr int MN_BOX_BYTES = BK * 128;          // MN-major: one TMA box = BK rows x 32 floats
 static_assert(SMEM_BYTES <= 227 * 1024, "exceeds the shared memory of one block");
+// bf16 pipeline (bns_dense_*_bf16): same raw ring geometry and TMA boxes; the operand buffer holds one bf16 copy of the
+// A and B tiles (BK bf16 = 64 bytes per row, 64-byte swizzle), a quarter of hi + lo, so the freed space goes to a deeper
+// raw ring.
+constexpr int WG_K_BF = 16;                     // wgmma .bf16: 16 elements (32 bytes) of contraction per instruction
+constexpr int kStagesBf = 6;
+constexpr int A_BF_BYTES = BM * BK * 2;         // 8 KB
+constexpr int OP_BF_BYTES = A_BF_BYTES + BN * BK * 2;
+constexpr int SMEM_BF_BYTES = kStagesBf * RAW_BYTES + kOpBufs * OP_BF_BYTES + BAR_BYTES + 1024;
+static_assert(SMEM_BF_BYTES <= 227 * 1024, "exceeds the shared memory of one block");
+static_assert(2 * kStagesBf * 8 <= BAR_BYTES, "barrier region too small");
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -181,14 +191,97 @@ __device__ __forceinline__ void split_stage(const uint8_t *raw, uint8_t *op, int
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes -> visible to wgmma's async reads
 }
 
+// ---- bf16 operands ----
+// wgmma descriptor, K-major with 64-byte swizzle (layout type 2): 8-row groups of 64-byte rows, SBO = 512; the second
+// 16-wide k-step of a row starts 32 bytes further.
+__device__ __forceinline__ uint64_t smem_desc_sw64(uint32_t addr) {
+    return (uint64_t)((addr >> 4) & 0x3FFFu) | ((uint64_t)1 << 16) | ((uint64_t)(512 >> 4) << 32) | (2ull << 62);
+}
+
+// d[64 x 128] += A[64 x 16] * B[128 x 16]^T, bf16 operands, f32 accumulators
+__device__ __forceinline__ void wgmma_bf16(float (&d)[64], uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(1)
+        : "memory");
+}
+
+// The 2 wgmmas of one BK-wide k-block for consumer warpgroup wg.
+__device__ __forceinline__ void mma_kblock_bf16(float (&d)[64], uint32_t op, uint32_t wg) {
+    const uint32_t a = op + wg * (64 * 64), b = op + A_BF_BYTES;
+#pragma unroll
+    for (int k = 0; k < BK / WG_K_BF; ++k) wgmma_bf16(d, smem_desc_sw64(a + 32 * k), smem_desc_sw64(b + 32 * k));
+}
+
+// two f32 -> bf16x2, round to nearest even (NaN stays NaN, +-Inf stays +-Inf); lo lands in the low half (lower address)
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+
+// Consumer warpgroup wg's share of the rounding: rows [64 wg, 64 wg + 64) of the A and of the B tile of raw stage `raw`
+// -> bf16 operand buffer `op`, K-major with the 64-byte swizzle (16-byte chunk c of row r at chunk c ^ ((r / 2) % 4)).
+// A unit is 8 contraction elements of one row (one 16-byte bf16 chunk); lanes walk consecutive rows, so the raw reads
+// (as in split_stage) and the 16-byte stores of each quarter-warp hit 8 distinct bank groups.
+template <bool kMN>
+__device__ __forceinline__ void cvt_stage(const uint8_t *raw, uint8_t *op, int wg, int t) {
+#pragma unroll
+    for (int part = 0; part < 2; ++part) {           // 0: A, 1: B
+        const uint8_t *src = raw + part * A_BYTES;
+        uint8_t *dst = op + part * A_BF_BYTES;
+#pragma unroll
+        for (int j = 0; j < (64 * BK / 8) / 128; ++j) {
+            const int idx = t + 128 * j;
+            const int r = 64 * wg + (idx & 63), c = idx >> 6;
+            float e[8];
+            if (!kMN) {
+                const float4 x0 = *reinterpret_cast<const float4 *>(src + r * 128 + (((2 * c) ^ (r & 7)) << 4));
+                const float4 x1 = *reinterpret_cast<const float4 *>(src + r * 128 + (((2 * c + 1) ^ (r & 7)) << 4));
+                e[0] = x0.x; e[1] = x0.y; e[2] = x0.z; e[3] = x0.w; e[4] = x1.x; e[5] = x1.y; e[6] = x1.z; e[7] = x1.w;
+            } else {
+                const uint8_t *box = src + (r >> 5) * MN_BOX_BYTES;
+                const int mm = r & 31;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int k = 8 * c + q;
+                    e[q] = *reinterpret_cast<const float *>(box + k * 128 + ((((mm >> 2) ^ (k & 7))) << 4) + (mm & 3) * 4);
+                }
+            }
+            const uint4 o = make_uint4(pack_bf16x2(e[0], e[1]), pack_bf16x2(e[2], e[3]), pack_bf16x2(e[4], e[5]),
+                                       pack_bf16x2(e[6], e[7]));
+            *reinterpret_cast<uint4 *>(dst + r * 64 + ((c ^ ((r >> 1) & 3)) << 4)) = o;
+        }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+// The whole pipeline, shared by the 3xTF32 and the bf16 kernels (kBf16 picks the ring depth, the operand buffer and
+// its conversion, and the wgmma form).
 // Persistent: gridDim.x = min(work items, SMs); a work item = (output tile, contraction slice).  All roles walk the same
 // item sequence; the raw ring and its phases run on across items.
-template <bool kMN>
-__global__ void __launch_bounds__(kThreadsTc, 1)
-gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-              float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
-              const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
-              int tiles_n, int tiles, int splits) {
+template <bool kMN, bool kBf16>
+__device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtensorMap &map_b, float *__restrict__ C,
+                                          int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
+                                          const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale,
+                                          int M, int N, int num_kb, int tiles_n, int tiles, int splits) {
+    constexpr int kStages = kBf16 ? kStagesBf : tc::kStages;
+    constexpr int OP_BYTES = kBf16 ? OP_BF_BYTES : tc::OP_BYTES;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -254,7 +347,10 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
     auto split_kblock = [&](uint32_t g) {
         const uint32_t s = g % kStages;
         mbar_wait(full_bar(s), (g / kStages) & 1u);
-        split_stage<kMN>(base_ptr + s * RAW_BYTES, base_ptr + kStages * RAW_BYTES + (g & 1u) * OP_BYTES, wg, t);
+        if constexpr (kBf16)
+            cvt_stage<kMN>(base_ptr + s * RAW_BYTES, base_ptr + kStages * RAW_BYTES + (g & 1u) * OP_BYTES, wg, t);
+        else
+            split_stage<kMN>(base_ptr + s * RAW_BYTES, base_ptr + kStages * RAW_BYTES + (g & 1u) * OP_BYTES, wg, t);
     };
     auto publish_kblock = [&](uint32_t g) {
         consumers_sync();
@@ -272,8 +368,13 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
         for (int i = 0; i < nkb; ++i, ++g) {
             const uint32_t op = ops + (g & 1u) * OP_BYTES;
             wgmma_fence();
-            if (i % kAcc == 0) mma_kblock(acc0, op, wg);
-            else mma_kblock(acc1, op, wg);
+            if constexpr (kBf16) {
+                if (i % kAcc == 0) mma_kblock_bf16(acc0, op, wg);
+                else mma_kblock_bf16(acc1, op, wg);
+            } else {
+                if (i % kAcc == 0) mma_kblock(acc0, op, wg);
+                else mma_kblock(acc1, op, wg);
+            }
             wgmma_commit();
             if (i + 1 < nkb) split_kblock(g + 1);            // CUDA cores: next k-block while the tensor cores run
             wgmma_wait_all();
@@ -312,6 +413,28 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
         }
     }
 #undef BNS_TC_ITEM
+}
+
+template <bool kMN>
+__global__ void __launch_bounds__(kThreadsTc, 1)
+gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+              float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
+              const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
+              int tiles_n, int tiles, int splits) {
+    gemm_body<kMN, false>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, M, N, num_kb, tiles_n, tiles,
+                          splits);
+}
+
+// The same GEMM with the operands rounded to bf16 (nearest even) in shared memory: one m64n128k16 wgmma per 16
+// contraction elements instead of 3 x 2 m64n128k8 .tf32.  Not f32-accurate (8-bit mantissa operands, f32 sums).
+template <bool kMN>
+__global__ void __launch_bounds__(kThreadsTc, 1)
+gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                 float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
+                 const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
+                 int tiles_n, int tiles, int splits) {
+    gemm_body<kMN, true>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, M, N, num_kb, tiles_n, tiles,
+                         splits);
 }
 
 // out[r, c] = sum_s ws[s][r, c]  in split order (deterministic); ws slices are contiguous [rows, cols].  Above
@@ -379,50 +502,54 @@ inline int make_map(CUtensorMap *m, const float *ptr, int64_t inner, int64_t row
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-template <bool kMN>
+template <bool kMN, bool kBf16>
 int configure() {
     static std::atomic<int> done[kMaxDevices];      // the attribute is per function AND per device
     const int dev = current_device();
     if (!done[dev].load(std::memory_order_acquire)) {
-        BNS_CUDA(cudaFuncSetAttribute(gemm3x_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
+        if (kBf16)
+            BNS_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BF_BYTES));
+        else
+            BNS_CUDA(cudaFuncSetAttribute(gemm3x_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
         done[dev].store(1, std::memory_order_release);
     }
     return BNS_OK;
 }
 
-}  // namespace tc
-
-// C[M, N] = A[M, K] * B[N, K]^T (+ bias[N]) (+ addend[M, N])
-extern "C" int bns_dense_tn_3xtf32(const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias,
-                                   const float *addend, int64_t ldadd, const float *row_scale, float *C, int64_t ldc, int64_t M,
-                                   int64_t N, int64_t K, void *stream) {
-    BNS_REQUIRE(A && B && C, "bns_dense_tn_3xtf32: NULL argument");
-    BNS_REQUIRE(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "bns_dense_tn_3xtf32: bad shape");
-    BNS_REQUIRE(lda >= K && ldb >= K && ldc >= N, "bns_dense_tn_3xtf32: leading dimension smaller than the row");
-    BNS_REQUIRE(lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0 && tc::aligned16(A) && tc::aligned16(B) && tc::aligned16(C) &&
-                    (!bias || tc::aligned16(bias)) && (!addend || (tc::aligned16(addend) && ldadd % 4 == 0 && ldadd >= N)),
-                "bns_dense_tn_3xtf32: operands must be 16-byte aligned with leading dimensions that are multiples of 4");
+// C[M, N] = A[M, K] * B[N, K]^T (+ bias[N]) (+ addend[M, N]); `fn` names the entry point in error messages
+template <bool kBf16>
+int dense_tn(const char *fn, const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias, const float *addend,
+             int64_t ldadd, const float *row_scale, float *C, int64_t ldc, int64_t M, int64_t N, int64_t K, void *stream) {
+    BNS_REQUIRE(A && B && C, "%s: NULL argument", fn);
+    BNS_REQUIRE(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "%s: bad shape", fn);
+    BNS_REQUIRE(lda >= K && ldb >= K && ldc >= N, "%s: leading dimension smaller than the row", fn);
+    BNS_REQUIRE(lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0 && aligned16(A) && aligned16(B) && aligned16(C) &&
+                    (!bias || aligned16(bias)) && (!addend || (aligned16(addend) && ldadd % 4 == 0 && ldadd >= N)),
+                "%s: operands must be 16-byte aligned with leading dimensions that are multiples of 4", fn);
     CUtensorMap ma, mb;
-    int rc = tc::make_map(&ma, A, K, M, lda, tc::BK, tc::BM);
+    int rc = make_map(&ma, A, K, M, lda, BK, BM);
     if (rc) return rc;
-    rc = tc::make_map(&mb, B, K, N, ldb, tc::BK, tc::BN);
+    rc = make_map(&mb, B, K, N, ldb, BK, BN);
     if (rc) return rc;
-    rc = tc::configure<false>();
+    rc = configure<false, kBf16>();
     if (rc) return rc;
-    const int tiles_m = (int)((M + tc::BM - 1) / tc::BM), tiles_n = (int)((N + tc::BN - 1) / tc::BN);
-    const int num_kb = (int)((K + tc::BK - 1) / tc::BK);
+    const int tiles_m = (int)((M + BM - 1) / BM), tiles_n = (int)((N + BN - 1) / BN);
+    const int num_kb = (int)((K + BK - 1) / BK);
     const int64_t tiles64 = tiles_m * (int64_t)tiles_n;
-    BNS_REQUIRE(tiles64 < (1ll << 31), "bns_dense_tn_3xtf32: too many tiles");
+    BNS_REQUIRE(tiles64 < (1ll << 31), "%s: too many tiles", fn);
     const int tiles = (int)tiles64;
     dim3 grid((unsigned)(tiles < sm_count() ? tiles : sm_count()), 1, 1);
-    tc::gemm3x_kernel<false><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
-                                                                                        row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
+    if (kBf16)
+        gemm_bf16_kernel<false><<<grid, kThreadsTc, SMEM_BF_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
+                                                                                      row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
+    else
+        gemm3x_kernel<false><<<grid, kThreadsTc, SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
+                                                                                row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
 }
 
-namespace tc {
 inline int nt_splits(int64_t R, int64_t N1, int64_t N2) {
     const int64_t tiles = ((N1 + BM - 1) / BM) * ((N2 + BN - 1) / BN);
     const int64_t num_kb = (R + BK - 1) / BK;
@@ -450,7 +577,67 @@ inline int nt_splits(int64_t R, int64_t N1, int64_t N2) {
     s = best;
     return (int)s;
 }
+
+// C[N1, N2] = A[R, N1]^T * B[R, N2]; both precisions use the same slice plan and workspace
+template <bool kBf16>
+int dense_nt(const char *fn, const float *A, int64_t lda, const float *B, int64_t ldb, float *C, int64_t ldc, int64_t R,
+             int64_t N1, int64_t N2, void *ws, size_t ws_bytes, void *stream) {
+    BNS_REQUIRE(A && B && C, "%s: NULL argument", fn);
+    BNS_REQUIRE(R > 0 && N1 > 0 && N2 > 0 && R < (1ll << 31) && N1 < (1ll << 31) && N2 < (1ll << 31), "%s: bad shape", fn);
+    BNS_REQUIRE(lda >= N1 && ldb >= N2 && ldc >= N2, "%s: leading dimension smaller than the row", fn);
+    BNS_REQUIRE(lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0 && N2 % 4 == 0 && aligned16(A) && aligned16(B) && aligned16(C),
+                "%s: operands must be 16-byte aligned, leading dimensions and N2 multiples of 4", fn);
+    const int splits = nt_splits(R, N1, N2);
+    const size_t need = splits > 1 ? (size_t)splits * (size_t)N1 * (size_t)N2 * sizeof(float) : 0;
+    if (need > ws_bytes || (need && (!ws || !aligned16(ws))))
+        return fail(BNS_E_WORKSPACE, "%s: workspace %zu < %zu bytes", fn, ws_bytes, need);
+    CUtensorMap ma, mb;
+    int rc = make_map(&ma, A, N1, R, lda, 32, BK);
+    if (rc) return rc;
+    rc = make_map(&mb, B, N2, R, ldb, 32, BK);
+    if (rc) return rc;
+    rc = configure<true, kBf16>();
+    if (rc) return rc;
+    const int tiles_m = (int)((N1 + BM - 1) / BM), tiles_n = (int)((N2 + BN - 1) / BN);
+    const int num_kb = (int)((R + BK - 1) / BK);
+    const int tiles = tiles_m * tiles_n;
+    const int64_t work = (int64_t)tiles * splits;
+    BNS_REQUIRE(work < (1ll << 31), "%s: too many work items", fn);
+    dim3 grid((unsigned)(work < sm_count() ? work : sm_count()), 1, 1);
+    cudaStream_t st = as_stream(stream);
+    float *w = splits == 1 ? C : static_cast<float *>(ws);
+    const int64_t ldw = splits == 1 ? ldc : N2, slice = splits == 1 ? 0 : N1 * N2;
+    if (kBf16)
+        gemm_bf16_kernel<true><<<grid, kThreadsTc, SMEM_BF_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
+                                                                        (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
+    else
+        gemm3x_kernel<true><<<grid, kThreadsTc, SMEM_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
+                                                                  (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
+    if (splits == 1) {
+        ++g_launches;
+    } else {
+        const int64_t total4 = N1 * N2 / 4;
+        splitk_reduce_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float4 *>(w), total4, splits,
+                                                                               N2 / 4, C, ldc, total4);
+        g_launches += 2;
+    }
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
 }  // namespace tc
+
+extern "C" int bns_dense_tn_3xtf32(const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias,
+                                   const float *addend, int64_t ldadd, const float *row_scale, float *C, int64_t ldc, int64_t M,
+                                   int64_t N, int64_t K, void *stream) {
+    return tc::dense_tn<false>("bns_dense_tn_3xtf32", A, lda, B, ldb, bias, addend, ldadd, row_scale, C, ldc, M, N, K, stream);
+}
+
+extern "C" int bns_dense_tn_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias,
+                                 const float *addend, int64_t ldadd, const float *row_scale, float *C, int64_t ldc, int64_t M,
+                                 int64_t N, int64_t K, void *stream) {
+    return tc::dense_tn<true>("bns_dense_tn_bf16", A, lda, B, ldb, bias, addend, ldadd, row_scale, C, ldc, M, N, K, stream);
+}
 
 extern "C" size_t bns_dense_nt_workspace_bytes(int64_t R, int64_t N1, int64_t N2) {
     if (R <= 0 || N1 <= 0 || N2 <= 0) return 0;
@@ -458,44 +645,12 @@ extern "C" size_t bns_dense_nt_workspace_bytes(int64_t R, int64_t N1, int64_t N2
     return s > 1 ? (size_t)s * (size_t)N1 * (size_t)N2 * sizeof(float) : 0;
 }
 
-// C[N1, N2] = A[R, N1]^T * B[R, N2]
 extern "C" int bns_dense_nt_3xtf32(const float *A, int64_t lda, const float *B, int64_t ldb, float *C, int64_t ldc,
                                    int64_t R, int64_t N1, int64_t N2, void *ws, size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(A && B && C, "bns_dense_nt_3xtf32: NULL argument");
-    BNS_REQUIRE(R > 0 && N1 > 0 && N2 > 0 && R < (1ll << 31) && N1 < (1ll << 31) && N2 < (1ll << 31), "bns_dense_nt_3xtf32: bad shape");
-    BNS_REQUIRE(lda >= N1 && ldb >= N2 && ldc >= N2, "bns_dense_nt_3xtf32: leading dimension smaller than the row");
-    BNS_REQUIRE(lda % 4 == 0 && ldb % 4 == 0 && ldc % 4 == 0 && N2 % 4 == 0 && tc::aligned16(A) && tc::aligned16(B) && tc::aligned16(C),
-                "bns_dense_nt_3xtf32: operands must be 16-byte aligned, leading dimensions and N2 multiples of 4");
-    const int splits = tc::nt_splits(R, N1, N2);
-    const size_t need = splits > 1 ? (size_t)splits * (size_t)N1 * (size_t)N2 * sizeof(float) : 0;
-    if (need > ws_bytes || (need && (!ws || !tc::aligned16(ws))))
-        return fail(BNS_E_WORKSPACE, "bns_dense_nt_3xtf32: workspace %zu < %zu bytes", ws_bytes, need);
-    CUtensorMap ma, mb;
-    int rc = tc::make_map(&ma, A, N1, R, lda, 32, tc::BK);
-    if (rc) return rc;
-    rc = tc::make_map(&mb, B, N2, R, ldb, 32, tc::BK);
-    if (rc) return rc;
-    rc = tc::configure<true>();
-    if (rc) return rc;
-    const int tiles_m = (int)((N1 + tc::BM - 1) / tc::BM), tiles_n = (int)((N2 + tc::BN - 1) / tc::BN);
-    const int num_kb = (int)((R + tc::BK - 1) / tc::BK);
-    const int tiles = tiles_m * tiles_n;
-    const int64_t work = (int64_t)tiles * splits;
-    BNS_REQUIRE(work < (1ll << 31), "bns_dense_nt_3xtf32: too many work items");
-    dim3 grid((unsigned)(work < sm_count() ? work : sm_count()), 1, 1);
-    cudaStream_t st = as_stream(stream);
-    float *w = splits == 1 ? C : static_cast<float *>(ws);
-    const int64_t ldw = splits == 1 ? ldc : N2, slice = splits == 1 ? 0 : N1 * N2;
-    tc::gemm3x_kernel<true><<<grid, tc::kThreadsTc, tc::SMEM_BYTES, st>>>(ma, mb, w, ldw, slice, nullptr, nullptr, 0, nullptr,
-                                                                         (int)N1, (int)N2, num_kb, tiles_n, tiles, splits);
-    if (splits == 1) {
-        ++g_launches;
-    } else {
-        const int64_t total4 = N1 * N2 / 4;
-        tc::splitk_reduce_kernel<<<(unsigned)((total4 + 255) / 256), 256, 0, st>>>(reinterpret_cast<const float4 *>(w), total4, splits,
-                                                                                   N2 / 4, C, ldc, total4);
-        g_launches += 2;
-    }
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
+    return tc::dense_nt<false>("bns_dense_nt_3xtf32", A, lda, B, ldb, C, ldc, R, N1, N2, ws, ws_bytes, stream);
+}
+
+extern "C" int bns_dense_nt_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, float *C, int64_t ldc,
+                                 int64_t R, int64_t N1, int64_t N2, void *ws, size_t ws_bytes, void *stream) {
+    return tc::dense_nt<true>("bns_dense_nt_bf16", A, lda, B, ldb, C, ldc, R, N1, N2, ws, ws_bytes, stream);
 }

@@ -87,6 +87,9 @@ class ParamArena:
         self._entries: List[DeriveEntry] = []
         self._table: Optional[torch.Tensor] = None
         self._keep: List[torch.Tensor] = []
+        # --dense-dtype bf16: every GEMM of the fused layers rounds its operands to bf16 inside the kernel (f32 sums);
+        # per run, never global: ranks that are threads of one process may differ
+        self.dense_bf16 = False
 
     def __deepcopy__(self, memo):
         """A copied model (evaluate.py's snapshots) owns plain parameter tensors and takes the op-by-op path."""
@@ -286,7 +289,7 @@ class PPLinearFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, arena: ParamArena, p: float, seed: int):
         xd = dropout(x, p, seed)
-        y = dense.tc_mm_tn(xd, arena.padded(weight), None if bias is None else arena.padded(bias))
+        y = dense.tc_mm_tn(xd, arena.padded(weight), None if bias is None else arena.padded(bias), bf16=arena.dense_bf16)
         ctx.save_for_backward(xd)
         ctx.arena, ctx.weight, ctx.bias, ctx.p, ctx.seed = arena, weight, bias, p, seed
         ctx.rng = (ops.RNG["seed"], ops.RNG["offset"], ops.RNG["offset_dev"])
@@ -299,10 +302,10 @@ class PPLinearFn(torch.autograd.Function):
         dy = dy.contiguous()
         if ctx.bias is not None:
             dense.colsum(dy, out=a.grad_padded(ctx.bias))
-        dense.tc_mm_nt(dy, xd, out=a.grad_padded(ctx.weight))
+        dense.tc_mm_nt(dy, xd, out=a.grad_padded(ctx.weight), bf16=a.dense_bf16)
         dx = None
         if ctx.needs_input_grad[0]:
-            dx = dense.tc_mm_tn(dy, a.transposed(ctx.weight))
+            dx = dense.tc_mm_tn(dy, a.transposed(ctx.weight), bf16=a.dense_bf16)
             if ctx.p > 0.0:                     # d dropout: the same mask, regenerated
                 keep = ops.RNG["seed"], ops.RNG["offset"], ops.RNG["offset_dev"]
                 ops.RNG.update(seed=ctx.rng[0], offset=ctx.rng[1], offset_dev=ctx.rng[2])
@@ -339,16 +342,17 @@ def _halo_rows(h_u: torch.Tensor, n_in: int, halo: Optional[torch.Tensor]) -> to
     return h_u[n_in:] if halo is None else ops.cvt_rows_f32(halo)
 
 
-def _weight_grad(dt: torch.Tensor, saved, n_in: int, out: torch.Tensor) -> None:
+def _weight_grad(dt: torch.Tensor, saved, n_in: int, out: torch.Tensor, bf16: bool) -> None:
     """``dt^T h_u`` into ``out``.  ``saved``: ``(h_u,)``, or ``(h_in, h_halo)`` when the halo rows are kept apart
-    (``--comm-dtype bf16``): the inner rows' product, then the halo rows' product added (one f32 add per element)."""
+    (``--comm-dtype bf16``): the inner rows' product, then the halo rows' product added (one f32 add per element).
+    ``bf16``: the products of ``--dense-dtype bf16``."""
     if len(saved) == 1:
-        dense.tc_mm_nt(dt, saved[0], out=out)
+        dense.tc_mm_nt(dt, saved[0], out=out, bf16=bf16)
         return
     h_in, h_halo = saved
-    dense.tc_mm_nt(dt[:n_in], h_in, out=out)
+    dense.tc_mm_nt(dt[:n_in], h_in, out=out, bf16=bf16)
     if h_halo.shape[0]:
-        part = dense.tc_mm_nt(dt[n_in:], h_halo)
+        part = dense.tc_mm_nt(dt[n_in:], h_halo, bf16=bf16)
         rows = torch.arange(out.shape[0], dtype=torch.int64, device=out.device)
         ops.scatter_add_div(out, rows, part, 1.0)                      # x / 1 is x: an exact row-wise add
 
@@ -392,26 +396,27 @@ class SageConvFn(torch.autograd.Function):
         n_in = g.n_in
         h_u = h_u.contiguous()
         W1, W2 = arena.padded(w1), arena.padded(w2)
+        bf = arena.dense_bf16
         h_in = h_u[:n_in]
         if narrow_first:
             # transform, then aggregate; the local rows go first -- their GEMM and the inner-edge pass need nothing from
             # the peers and hide the exchange -- the halo rows after the exchange's event
             n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
             t = gather_friendly(n_u, W2.shape[0], h_u.device)                   # [n_u, out_p]
-            dense.tc_mm_tn(h_in, W2, out=t[:n_in])
-            out = dense.tc_mm_tn(h_in, W1, arena.bias_sum(b1, b2))              # linear1(h) + b1 + b2 ...
+            dense.tc_mm_tn(h_in, W2, out=t[:n_in], bf16=bf)
+            out = dense.tc_mm_tn(h_in, W1, arena.bias_sum(b1, b2), bf16=bf)     # linear1(h) + b1 + b2 ...
             ops.spmm_auto(g.a_in, t[:n_in], out, row_scale=rs, accumulate=True)  # ... + (A_in t) / deg
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             h_halo = _halo_rows(h_u, n_in, halo)
             if g.a_out is not None and n_u > n_in:
-                dense.tc_mm_tn(h_halo, W2, out=t[n_in:])
+                dense.tc_mm_tn(h_halo, W2, out=t[n_in:], bf16=bf)
                 halo_aggregate(g, t[n_in:], out, rs, None)                      # ... + (A_out t_halo) / deg
             ctx.save_for_backward(*((h_u,) if halo is None else (h_in, h_halo)))
         else:
             ah = _aggregate(g, h_u, rs, ready, g.agg_bf16, halo)                # [n_in, in]
-            t = dense.tc_mm_tn(ah, W2, arena.padded(b2))
-            out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t)
+            t = dense.tc_mm_tn(ah, W2, arena.padded(b2), bf16=bf)
+            out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t, bf16=bf)
             ctx.save_for_backward(h_u, ah)
         ctx.n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
         ctx.g, ctx.rs, ctx.arena, ctx.narrow = g, rs, arena, narrow_first
@@ -423,6 +428,7 @@ class SageConvFn(torch.autograd.Function):
         g, rs, a = ctx.g, ctx.rs, ctx.arena
         w1, b1, w2, b2 = ctx.params
         n_in = g.n_in
+        bf = a.dense_bf16
         dout = dout.contiguous()
         dense.colsum(dout, out=a.grad_padded(b1), out2=a.grad_padded(b2))
         begin = None
@@ -436,20 +442,20 @@ class SageConvFn(torch.autograd.Function):
             dt = _aggregate_t(g, dys, n_u)                                      # [n_u, out_p]
             du = torch.empty(n_u, h_in.shape[1], dtype=torch.float32, device=dout.device)
             if n_u > n_in:                                                      # halo rows first: they travel ...
-                dense.tc_mm_tn(dt[n_in:], a.transposed(w2), out=du[n_in:])
+                dense.tc_mm_tn(dt[n_in:], a.transposed(w2), out=du[n_in:], bf16=bf)
             if begin is not None:
                 begin(du)
-            dense.tc_mm_tn(dt[:n_in], a.transposed(w2), out=du[:n_in])          # ... while the local rows are computed
-            dense.tc_mm_nt(dout, h_in, out=a.grad_padded(w1))
-            _weight_grad(dt, saved, n_in, a.grad_padded(w2))
+            dense.tc_mm_tn(dt[:n_in], a.transposed(w2), out=du[:n_in], bf16=bf)  # ... while the local rows are computed
+            dense.tc_mm_nt(dout, h_in, out=a.grad_padded(w1), bf16=bf)
+            _weight_grad(dt, saved, n_in, a.grad_padded(w2), bf)
         else:
             h_u, ah = ctx.saved_tensors
-            dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs)          # (dout W2) / deg
+            dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs, bf16=bf)  # (dout W2) / deg
             du = _aggregate_t(g, dys, ctx.n_u, after_halo=begin, bf16=g.agg_bf16)
-            dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1))
-            dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2))
+            dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1), bf16=bf)
+            dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2), bf16=bf)
         inner = du[:n_in]
-        dense.tc_mm_tn(dout, a.transposed(w1), addend=inner, out=inner)         # += dout W1, in place
+        dense.tc_mm_tn(dout, a.transposed(w1), addend=inner, out=inner, bf16=bf)  # += dout W1, in place
         return inner if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None, None
 
 
@@ -470,19 +476,20 @@ class GcnConvFn(torch.autograd.Function):
         n_in = g.n_in
         h_u = h_u.contiguous()
         W, bp = arena.padded(w), arena.padded(b)
+        bf = arena.dense_bf16
         cs_in, cs_halo = cs_u[:n_in], cs_u[n_in:]
         n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
         has_halo = g.a_out is not None and n_u > n_in
         if narrow_first:
             t = gather_friendly(n_u, W.shape[0], h_u.device)                                          # [n_u, out_p]
-            dense.tc_mm_tn(h_u[:n_in], W, out=t[:n_in])                                               # local rows first
+            dense.tc_mm_tn(h_u[:n_in], W, out=t[:n_in], bf16=bf)                                      # local rows first
             ts = scale_rows(t[:n_in], cs_in, out=gather_friendly(n_in, W.shape[0], h_u.device))
             s = ops.spmm_auto(g.a_in, ts)                                                             # raw sums
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             h_halo = _halo_rows(h_u, n_in, halo)
             if has_halo:
-                dense.tc_mm_tn(h_halo, W, out=t[n_in:])
+                dense.tc_mm_tn(h_halo, W, out=t[n_in:], bf16=bf)
                 halo_aggregate(g, t[n_in:], s, None, cs_halo)
             out = scale_rows(s, rs, bias=bp)                                                          # / in_norm + b
             ctx.save_for_backward(*((h_u,) if halo is None else (h_u[:n_in], h_halo)))
@@ -493,7 +500,7 @@ class GcnConvFn(torch.autograd.Function):
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             if has_halo:
                 halo_aggregate(g, halo if halo is not None else _gather_table(h_u[n_in:], bf16), y, rs, cs_halo)
-            out = dense.tc_mm_tn(y, W, bp)
+            out = dense.tc_mm_tn(y, W, bp, bf16=bf)
             ctx.save_for_backward(y)
         ctx.n_u = n_u
         ctx.g, ctx.rs, ctx.cs, ctx.arena, ctx.narrow, ctx.params = g, rs, (cs_in, cs_halo), arena, narrow_first, (w, b)
@@ -504,6 +511,7 @@ class GcnConvFn(torch.autograd.Function):
         g, rs, a = ctx.g, ctx.rs, ctx.arena
         cs_in, cs_halo = ctx.cs
         w, b = ctx.params
+        bf = a.dense_bf16
         dout = dout.contiguous()
         dense.colsum(dout, out=a.grad_padded(b))
         begin = None
@@ -513,14 +521,14 @@ class GcnConvFn(torch.autograd.Function):
         if ctx.narrow:
             dys = scale_rows(dout, rs, out=gather_friendly(g.n_in, dout.shape[1], dout.device))
             dt = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo)                  # [n_u, out_p]
-            _weight_grad(dt, ctx.saved_tensors, g.n_in, a.grad_padded(w))
-            du = dense.tc_mm_tn(dt, a.transposed(w))                            # [n_u, in]
+            _weight_grad(dt, ctx.saved_tensors, g.n_in, a.grad_padded(w), bf)
+            du = dense.tc_mm_tn(dt, a.transposed(w), bf16=bf)                   # [n_u, in]
             if begin is not None:
                 begin(du)
         else:
             (y,) = ctx.saved_tensors
-            dense.tc_mm_nt(dout, y, out=a.grad_padded(w))
-            dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs)           # (dout W) / in_norm
+            dense.tc_mm_nt(dout, y, out=a.grad_padded(w), bf16=bf)
+            dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs, bf16=bf)  # (dout W) / in_norm
             du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, after_halo=begin, bf16=g.agg_bf16)
         return du[:g.n_in] if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None
 

@@ -76,6 +76,13 @@ def build_parser():
                              "sampled row H[selected]/ratio, and each returned halo gradient row, to bf16 (nearest even) "
                              "at the sender: half the wire and slab bytes; the receiver widens and sums in f32.  Only "
                              "with the fused training step (GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+    parser.add_argument(*_spellings("dense-dtype"), default="f32", choices=["f32", "bf16"],
+                        help="NEW: operand precision of the training step's dense layers.  f32 runs the f32-accurate "
+                             "3xTF32 tensor-core scheme; bf16 rounds every GEMM operand to bf16 (nearest even) inside "
+                             "the kernel and sums in f32: one bf16 tensor-core product instead of three TF32 ones, and "
+                             "results that no longer match the reference to 1e-4.  Master weights, gradients, the "
+                             "all-reduce, Adam, the loss and evaluation stay f32.  Only with the fused training step "
+                             "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
     return parser
 
 

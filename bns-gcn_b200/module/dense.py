@@ -170,10 +170,14 @@ def tc_eligible(x: torch.Tensor, weight: torch.Tensor, bias=None) -> bool:
                                   and bias.data_ptr() % 16 == 0)))
 
 
-def tc_mm_tn(a: torch.Tensor, b: torch.Tensor, bias=None, addend=None, row_scale=None, out=None) -> torch.Tensor:
+def tc_mm_tn(a: torch.Tensor, b: torch.Tensor, bias=None, addend=None, row_scale=None, out=None,
+             bf16: bool = False) -> torch.Tensor:
     """``(a @ b.T (+ bias) (+ addend)) (* row_scale[:, None])``: a [M, K], b [N, K], addend [M, >= N]
-    (``bns_dense_tn_3xtf32``).  ``out`` may alias ``addend`` (in-place accumulation into a gradient buffer)."""
+    (``bns_dense_tn_3xtf32``).  ``out`` may alias ``addend`` (in-place accumulation into a gradient buffer).
+    ``bf16``: the products of ``bns_dense_tn_bf16`` instead -- a and b rounded to bf16 inside the kernel, f32 sums and
+    epilogue (``--dense-dtype bf16``)."""
     from .._lib import check, lib
+    fn_name = "bns_dense_tn_bf16" if bf16 else "bns_dense_tn_3xtf32"
     M, K = a.shape
     N = b.shape[0]
     if out is None:
@@ -183,12 +187,12 @@ def tc_mm_tn(a: torch.Tensor, b: torch.Tensor, bias=None, addend=None, row_scale
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(torch.cuda.current_stream(a.device))
     with torch.cuda.device(a.device):
-        check(lib.bns_dense_tn_3xtf32(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0),
-                                      None if bias is None else bias.data_ptr(),
-                                      None if addend is None else addend.data_ptr(),
-                                      0 if addend is None else addend.stride(0),
-                                      None if row_scale is None else row_scale.data_ptr(), out.data_ptr(), out.stride(0), M, N, K,
-                                      torch.cuda.current_stream().cuda_stream), "bns_dense_tn_3xtf32")
+        check(getattr(lib, fn_name)(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0),
+                                    None if bias is None else bias.data_ptr(),
+                                    None if addend is None else addend.data_ptr(),
+                                    0 if addend is None else addend.stride(0),
+                                    None if row_scale is None else row_scale.data_ptr(), out.data_ptr(), out.stride(0), M, N, K,
+                                    torch.cuda.current_stream().cuda_stream), fn_name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(a.device))
         prof.append((ev0, ev1, 2.0 * M * N * K, 4.0 * (M * K + N * K + M * N * (2 if addend is not None else 1))))
@@ -231,9 +235,11 @@ def colsum(x: torch.Tensor, out=None, out2=None) -> torch.Tensor:
     return out
 
 
-def tc_mm_nt(a: torch.Tensor, b: torch.Tensor, out=None) -> torch.Tensor:
-    """``a.T @ b``: a [R, N1], b [R, N2] -> [N1, N2], contraction over the rows (``bns_dense_nt_3xtf32``)."""
+def tc_mm_nt(a: torch.Tensor, b: torch.Tensor, out=None, bf16: bool = False) -> torch.Tensor:
+    """``a.T @ b``: a [R, N1], b [R, N2] -> [N1, N2], contraction over the rows (``bns_dense_nt_3xtf32``).  ``bf16``:
+    ``bns_dense_nt_bf16`` (operands rounded to bf16 inside the kernel, same split-K plan and workspace)."""
     from .._lib import check, lib
+    fn_name = "bns_dense_nt_bf16" if bf16 else "bns_dense_nt_3xtf32"
     R, N1 = a.shape
     N2 = b.shape[1]
     if out is None:
@@ -245,9 +251,8 @@ def tc_mm_nt(a: torch.Tensor, b: torch.Tensor, out=None) -> torch.Tensor:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(torch.cuda.current_stream(a.device))
     with torch.cuda.device(a.device):
-        check(lib.bns_dense_nt_3xtf32(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr(), out.stride(0),
-                                      R, N1, N2, ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream),
-              "bns_dense_nt_3xtf32")
+        check(getattr(lib, fn_name)(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0), out.data_ptr(), out.stride(0),
+                                    R, N1, N2, ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream), fn_name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(a.device))
         prof.append((ev0, ev1, 2.0 * R * N1 * N2, 4.0 * (R * N1 + R * N2 + N1 * N2)))

@@ -347,16 +347,12 @@ def _fused_eligible(args, layer_size, dev) -> bool:
     return widths_ok and len(layer_size) >= 3
 
 
-def check_agg_dtype(args, layer_size, dev) -> bool:
-    """Whether ``--agg-dtype bf16`` is on.  It only exists on the fused training step: any configuration that step does
-    not take raises ``ValueError`` naming why, rather than training in f32 behind the user's back."""
+def _fused_step_refusals(args, layer_size, dev, width_why=None) -> list:
+    """Every reason why the fused training step does not run for this configuration (empty: it runs); the bf16 modes
+    of ``--agg-dtype`` / ``--comm-dtype`` / ``--dense-dtype`` only exist there.  ``width_why``: the mode's own width
+    rule, when it is broken."""
     import os
     from .module import dense
-    mode = getattr(args, 'agg_dtype', 'f32')
-    if mode == 'f32':
-        return False
-    if mode != 'bf16':
-        raise ValueError(f"--agg-dtype {mode!r}: expected 'f32' or 'bf16'")
     why = []
     if os.environ.get("BNS_FUSED", "1") == "0":
         why.append("BNS_FUSED=0 turns the fused training step off")
@@ -370,10 +366,25 @@ def check_agg_dtype(args, layer_size, dev) -> bool:
         why.append(f"--norm {args.norm}")
     if dev.type != "cuda" or dense.MODE != "tc":
         why.append("no CUDA device with the wgmma GEMMs")
-    if any(w % 8 for w in layer_size[1:-1]):
-        why.append(f"hidden width {args.n_hidden} is not a multiple of 8 (bf16 rows are gathered 8 at a time)")
+    if width_why:
+        why.append(width_why)
     if not why and not _fused_eligible(args, layer_size, dev):
         why.append("the layer widths do not fit the fused step")
+    return why
+
+
+def check_agg_dtype(args, layer_size, dev) -> bool:
+    """Whether ``--agg-dtype bf16`` is on.  It only exists on the fused training step: any configuration that step does
+    not take raises ``ValueError`` naming why, rather than training in f32 behind the user's back."""
+    mode = getattr(args, 'agg_dtype', 'f32')
+    if mode == 'f32':
+        return False
+    if mode != 'bf16':
+        raise ValueError(f"--agg-dtype {mode!r}: expected 'f32' or 'bf16'")
+    width_why = None
+    if any(w % 8 for w in layer_size[1:-1]):
+        width_why = f"hidden width {args.n_hidden} is not a multiple of 8 (bf16 rows are gathered 8 at a time)"
+    why = _fused_step_refusals(args, layer_size, dev, width_why)
     if why:
         raise ValueError("--agg-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
     return True
@@ -383,34 +394,40 @@ def check_comm_dtype(args, layer_size, dev) -> str:
     """The element type of the boundary rows on the wire: ``'f32'``, or ``'bf16'`` (``--comm-dtype bf16``), which only
     exists on the fused training step -- its layers take the halo rows as bf16 and hand their halo gradient back to the
     exchange.  Any configuration that step does not take raises ``ValueError`` naming every reason."""
-    import os
-    from .module import dense
     mode = getattr(args, 'comm_dtype', 'f32')
     if mode == 'f32':
         return mode
     if mode != 'bf16':
         raise ValueError(f"--comm-dtype {mode!r}: expected 'f32' or 'bf16'")
-    why = []
-    if os.environ.get("BNS_FUSED", "1") == "0":
-        why.append("BNS_FUSED=0 turns the fused training step off")
-    if args.model not in ('graphsage', 'gcn'):
-        why.append(f"--model {args.model} (only graphsage and gcn have the fused step)")
-    if not args.use_pp:
-        why.append("no --use-pp")
-    if args.n_linear != 0:
-        why.append(f"--n-linear {args.n_linear}")
-    if args.norm != 'layer':
-        why.append(f"--norm {args.norm}")
-    if dev.type != "cuda" or dense.MODE != "tc":
-        why.append("no CUDA device with the wgmma GEMMs")
+    width_why = None
     bad = sorted({w for w in layer_size[1:-1] if w % 8})
     if bad:
-        why.append(f"exchanged width {', '.join(map(str, bad))} is not a multiple of 8 (bf16 rows move 8 at a time)")
-    if not why and not _fused_eligible(args, layer_size, dev):
-        why.append("the layer widths do not fit the fused step")
+        width_why = f"exchanged width {', '.join(map(str, bad))} is not a multiple of 8 (bf16 rows move 8 at a time)"
+    why = _fused_step_refusals(args, layer_size, dev, width_why)
     if why:
         raise ValueError("--comm-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
     return mode
+
+
+def check_dense_dtype(args, layer_size, dev) -> bool:
+    """Whether ``--dense-dtype bf16`` is on: every GEMM of the fused layers (forward, input and weight gradients) takes
+    its operands rounded to bf16 inside the kernel, with f32 sums.  It only exists on the fused training step; any
+    configuration that step does not take raises ``ValueError`` naming every reason."""
+    mode = getattr(args, 'dense_dtype', 'f32')
+    if mode == 'f32':
+        return False
+    if mode != 'bf16':
+        raise ValueError(f"--dense-dtype {mode!r}: expected 'f32' or 'bf16'")
+    k0 = 2 * layer_size[0] if args.model == 'graphsage' else layer_size[0]      # as _fused_eligible
+    bad = sorted(({k0} if k0 % 4 else set()) | {w for w in layer_size[1:-1] if w % 4 or w > 1024})
+    width_why = None
+    if bad or len(layer_size) < 3:
+        width_why = (f"layer widths {', '.join(map(str, bad))} do not fit the fused step (multiples of 4, hidden at most "
+                     f"1024)" if bad else "fewer than two layers")
+    why = _fused_step_refusals(args, layer_size, dev, width_why)
+    if why:
+        raise ValueError("--dense-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
+    return True
 
 
 def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
@@ -425,6 +442,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
     part.agg_bf16 = check_agg_dtype(args, layer_size, dev)
     comm_dtype = check_comm_dtype(args, layer_size, dev)
+    dense_bf16 = check_dense_dtype(args, layer_size, dev)
     _, _, _, node_dict, boundary = move_to_cuda(graph, in_graph, out_graph, node_dict, boundary, dev)
     print(f'Process {rank} has {graph.num_nodes()} nodes, {graph.num_edges()} edges '
           f'{in_graph.n_rows} inner nodes, and {in_graph.nnz} inner edges.')
@@ -443,6 +461,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     if _fused_eligible(args, layer_size, dev):
         from . import fused
         arena = fused.ParamArena(model)
+        arena.dense_bf16 = dense_bf16
         model._arena = arena
         ctx.reducer.init_arena(arena)
     else:

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 5
+#define BNS_ABI_VERSION 6
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -452,6 +452,19 @@ int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *id
                              const uint16_t *src /*bf16*/, int64_t lds, void *stream);
 int bns_cvt_rows_bf16_f32(const uint16_t *src /*bf16*/, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
                           void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 6: the dense layers with bf16 tensor-core products (--dense-dtype bf16).  Same operands (f32 in HBM), shapes,
+ * alignment rules, epilogue, split-K plan and workspace (bns_dense_nt_workspace_bytes) as bns_dense_tn_3xtf32 /
+ * bns_dense_nt_3xtf32, and the same BNS_E_INVALID / BNS_E_WORKSPACE returns.  The kernels round each operand element
+ * once to bf16 (nearest even; NaN stays NaN, +-Inf stays +-Inf) in shared memory and accumulate the products in f32:
+ * C = bf16(A) bf16(B)^T (+ bias) (+ addend) (* row_scale), the epilogue in f32.  Not f32-accurate: for runs that have
+ * opted out of the 1e-4 parity bar.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_dense_tn_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, const float *bias, const float *addend,
+                      int64_t ldadd, const float *row_scale, float *C, int64_t ldc, int64_t M, int64_t N, int64_t K, void *stream);
+int bns_dense_nt_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, float *C, int64_t ldc, int64_t R, int64_t N1,
+                      int64_t N2, void *ws, size_t ws_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Loss and its gradient in one launch.  Replaces train.py:406-408 for the two losses of train.py:358-361:
