@@ -1,10 +1,10 @@
 // bnsgcn.cu -- sm_90a kernels + the C ABI of include/bnsgcn.h.
 //
 // Hot kernels (all HBM/L2-bound f32 gather / scatter work; no tensor-core shaped math here):
-//   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers
+//   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers; f32 or bf16
+//                                 (--agg-dtype bf16) gather tables, f32 sums; cvt_rows_bf16_kernel
 //   spmm_fixup_kernel  deterministic combine of rows longer than one chunk
-//   spmm_bf16_kernel   the same row-sum over a bf16 gather table (--agg-dtype bf16), f32 sums; cvt_rows_bf16_kernel
-//   gather / scatter   K3/K5      boundary pack and gradient scatter-add
+//   gather / scatter   K3/K5      boundary pack and gradient scatter-add, f32 or bf16 (--comm-dtype bf16) wire rows
 //   philox_key / take  K6         counter-based exactly-k sampling (with cub radix sort)
 //   p2p_put_rows       K3+C1      pack straight into the peer's receive slab over NVLink + flag
 //
@@ -397,7 +397,7 @@ struct SpmmArgs {
     const int32_t *split_part;
     int64_t n_chunks, n_split;
     int32_t chunk_nnz;
-    const float *X;
+    const void *X;              // rows of the lane's element type (f32, or bf16 for Bf16x8); ldx in elements
     int64_t ldx;
     float *Y;
     int64_t ldy;
@@ -416,14 +416,53 @@ struct SpmmArgs {
     int64_t n_tiles;     // column slabs of the kernel's SLAB width covering F
 };
 
+// bf16 <-> f32: the widening is exact (a shift); the narrowing rounds to nearest even
+__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
+__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
+__device__ __forceinline__ uint16_t bf16_rn(float x) { return __bfloat16_as_ushort(__float2bfloat16_rn(x)); }
+__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
+    return (uint32_t)bf16_rn(lo) | ((uint32_t)bf16_rn(hi) << 16);
+}
+
+// bf16(src[0:8] / div) as one 16-byte word (the division in f32, then one rounding)
+__device__ __forceinline__ uint4 div_round8(const float *src, float div) {
+    const float4 a = *reinterpret_cast<const float4 *>(src), b = *reinterpret_cast<const float4 *>(src + 4);
+    uint4 o;
+    o.x = bf16x2_rn(__fdiv_rn(a.x, div), __fdiv_rn(a.y, div));
+    o.y = bf16x2_rn(__fdiv_rn(a.z, div), __fdiv_rn(a.w, div));
+    o.z = bf16x2_rn(__fdiv_rn(b.x, div), __fdiv_rn(b.y, div));
+    o.w = bf16x2_rn(__fdiv_rn(b.z, div), __fdiv_rn(b.w, div));
+    return o;
+}
+
+// v[0:8] += widen(r) / div, each element as the f32 lanes add it
+__device__ __forceinline__ void add_div8(float *v, uint4 r, float div) {
+    v[0] += __fdiv_rn(bf16_lo(r.x), div); v[1] += __fdiv_rn(bf16_hi(r.x), div);
+    v[2] += __fdiv_rn(bf16_lo(r.y), div); v[3] += __fdiv_rn(bf16_hi(r.y), div);
+    v[4] += __fdiv_rn(bf16_lo(r.z), div); v[5] += __fdiv_rn(bf16_hi(r.z), div);
+    v[6] += __fdiv_rn(bf16_lo(r.w), div); v[7] += __fdiv_rn(bf16_hi(r.w), div);
+}
+
+// Lane types: what one lane of a row-wise kernel holds.  Vec<4> is one 16-byte f32 vector, Vec<1> the scalar path
+// for rows that are not 16-byte aligned, Bf16x8 eight bf16 values of one 16-byte load widened into eight f32 sums.
+// T / kN: element type and count of one lane's slice of a row in X (SpMM) or on the wire (exchange).  In: what one
+// gather loads.  The sums, the partial sums of split rows and Y are f32 for every lane type.
+// min_blocks(NV, G, MAP && !CSCALE): the second argument of spmm_kernel's __launch_bounds__.
+//   div_round(s, div)  s / div rounded to T, as one Wire word;   load_div / add_div(r, div)  sums (+)= widen(r) / div
 template <int W> struct Vec;
 template <> struct Vec<4> {
+    using T = float;
+    using In = Vec;
+    using Wire = float4;
+    static constexpr int kN = 4;
+    static constexpr int min_blocks(int nv, int, bool) { return nv <= 1 ? 5 : 4; }
     float4 v;
     __device__ __forceinline__ void zero() { v = make_float4(0.f, 0.f, 0.f, 0.f); }
     __device__ __forceinline__ void load_ro(const float *p) { v = __ldg(reinterpret_cast<const float4 *>(p)); }
     __device__ __forceinline__ void load(const float *p) { v = *reinterpret_cast<const float4 *>(p); }
     __device__ __forceinline__ void store(float *p) const { *reinterpret_cast<float4 *>(p) = v; }
     __device__ __forceinline__ void add(const Vec &o) { v.x += o.v.x; v.y += o.v.y; v.z += o.v.z; v.w += o.v.w; }
+    __device__ __forceinline__ void add_f32(const float *p) { Vec o; o.load(p); add(o); }
     __device__ __forceinline__ void fma(const Vec &o, float s) {
         v.x = fmaf(o.v.x, s, v.x); v.y = fmaf(o.v.y, s, v.y); v.z = fmaf(o.v.z, s, v.z); v.w = fmaf(o.v.w, s, v.w);
     }
@@ -432,17 +471,90 @@ template <> struct Vec<4> {
         v.x += __shfl_xor_sync(0xffffffffu, v.x, off); v.y += __shfl_xor_sync(0xffffffffu, v.y, off);
         v.z += __shfl_xor_sync(0xffffffffu, v.z, off); v.w += __shfl_xor_sync(0xffffffffu, v.w, off);
     }
+    __device__ __forceinline__ void load_div(const float *r, float div) {
+        v = *reinterpret_cast<const float4 *>(r);
+        v.x = __fdiv_rn(v.x, div); v.y = __fdiv_rn(v.y, div); v.z = __fdiv_rn(v.z, div); v.w = __fdiv_rn(v.w, div);
+    }
+    __device__ __forceinline__ void add_div(const float *r, float div) { Vec x; x.load_div(r, div); add(x); }
+    __device__ __forceinline__ static float4 div_round(const float *s, float div) { Vec x; x.load_div(s, div); return x.v; }
 };
 template <> struct Vec<1> {
+    using T = float;
+    using In = Vec;
+    using Wire = float;
+    static constexpr int kN = 1;
+    static constexpr int min_blocks(int nv, int, bool) { return nv <= 1 ? 5 : 4; }
     float v;
     __device__ __forceinline__ void zero() { v = 0.f; }
     __device__ __forceinline__ void load_ro(const float *p) { v = __ldg(p); }
     __device__ __forceinline__ void load(const float *p) { v = *p; }
     __device__ __forceinline__ void store(float *p) const { *p = v; }
     __device__ __forceinline__ void add(const Vec &o) { v += o.v; }
+    __device__ __forceinline__ void add_f32(const float *p) { Vec o; o.load(p); add(o); }
     __device__ __forceinline__ void fma(const Vec &o, float s) { v = fmaf(o.v, s, v); }
     __device__ __forceinline__ void scale(float s) { v *= s; }
     __device__ __forceinline__ void add_shfl_xor(int off) { v += __shfl_xor_sync(0xffffffffu, v, off); }
+    __device__ __forceinline__ void load_div(const float *r, float div) { v = __fdiv_rn(*r, div); }
+    __device__ __forceinline__ void add_div(const float *r, float div) { v += __fdiv_rn(*r, div); }
+    __device__ __forceinline__ static float div_round(const float *s, float div) { return __fdiv_rn(*s, div); }
+};
+struct Bf16x8 {
+    using T = uint16_t;
+    using Wire = uint4;
+    static constexpr int kN = 8;
+    // 6 blocks per SM for the column-mapped plain sums with 4-lane row groups (32-column slabs): they fit 40 registers,
+    // and the 5 blocks that 43-44 registers leave cost 13 % there (measured on an H100 80GB HBM3 at 700 W)
+    static constexpr int min_blocks(int, int g, bool map_sum) { return g == 4 && map_sum ? 6 : 4; }
+    struct In {
+        uint4 u;
+        __device__ __forceinline__ void zero() { u = make_uint4(0u, 0u, 0u, 0u); }
+        __device__ __forceinline__ void load_ro(const uint16_t *p) { u = __ldg(reinterpret_cast<const uint4 *>(p)); }
+    };
+    float v[8];
+    __device__ __forceinline__ void zero() {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.f;
+    }
+    __device__ __forceinline__ void load(const float *p) {
+        const float4 a = *reinterpret_cast<const float4 *>(p), b = *reinterpret_cast<const float4 *>(p + 4);
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+    }
+    __device__ __forceinline__ void store(float *p) const {
+        *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
+        *reinterpret_cast<float4 *>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
+    }
+    __device__ __forceinline__ void add(const In &x) {
+        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] += bf16_lo(w[i]); v[2 * i + 1] += bf16_hi(w[i]); }
+    }
+    __device__ __forceinline__ void add_f32(const float *p) {
+        const float4 a = *reinterpret_cast<const float4 *>(p), b = *reinterpret_cast<const float4 *>(p + 4);
+        v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
+    }
+    __device__ __forceinline__ void fma(const In &x, float s) {
+        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] = fmaf(bf16_lo(w[i]), s, v[2 * i]); v[2 * i + 1] = fmaf(bf16_hi(w[i]), s, v[2 * i + 1]); }
+    }
+    __device__ __forceinline__ void scale(float s) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] *= s;
+    }
+    __device__ __forceinline__ void add_shfl_xor(int off) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], off);
+    }
+    __device__ __forceinline__ void load_div(const uint16_t *r, float div) {
+        const uint4 u = *reinterpret_cast<const uint4 *>(r);
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) { v[2 * i] = __fdiv_rn(bf16_lo(w[i]), div); v[2 * i + 1] = __fdiv_rn(bf16_hi(w[i]), div); }
+    }
+    __device__ __forceinline__ static uint4 div_round(const float *s, float div) { return div_round8(s, div); }
+    __device__ __forceinline__ void add_div(const uint16_t *r, float div) {
+        add_div8(v, *reinterpret_cast<const uint4 *>(r), div);
+    }
 };
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -458,8 +570,9 @@ __device__ __forceinline__ int32_t ld_stream_i32(const int32_t *p) {
 }
 
 // One warp per chunk of <= chunk_nnz entries of one row.  Lane l owns columns
-//   f0 + (l + 32 t) * W .. + W   for t < NV   (W = 4: one 16-byte vector, W = 1: scalar path)
-// so a warp reads each gathered row as NV fully coalesced 512-byte (W=4) requests.
+//   f0 + (l + 32 t) * W .. + W   for t < NV   (W = L::kN: 4 for one 16-byte f32 vector, 1 for the scalar path,
+//                                              8 for one 16-byte load of bf16 rows)
+// so a warp reads each gathered row as NV fully coalesced 512-byte (16-byte lanes) requests.
 // Column ids of 32 entries are fetched with one coalesced load, mapped (col_map: sampled halo ->
 // slab row, -1 = skip), compacted through shared memory and then consumed UNROLL at a time so that
 // UNROLL*NV independent 16-byte gathers are in flight per lane.
@@ -470,8 +583,10 @@ __device__ __forceinline__ int32_t ld_stream_i32(const int32_t *p) {
 // slab-major, so at any moment all resident warps gather from the same slab.  For narrow slabs a warp is
 // split into 32/G row groups of G lanes that walk different entries of the chunk concurrently (every lane
 // still issues 16-byte loads) and are summed with shuffles at the end.
-template <int W, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
-__global__ void __launch_bounds__(kThreads, (NV <= 1 ? 5 : 4)) spmm_kernel(SpmmArgs a) {
+template <class L, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
+__global__ void __launch_bounds__(kThreads, L::min_blocks(NV, G, MAP && !CSCALE)) spmm_kernel(SpmmArgs a) {
+    using T = typename L::T;
+    constexpr int W = L::kN;
     constexpr int NG = 32 / G;                               // entries walked concurrently by one warp
     constexpr int UNROLL = (NV <= 2) ? 8 / NV : 2;           // independent 16-byte gathers in flight per lane
     constexpr int SLAB = G * W * NV;
@@ -508,7 +623,7 @@ __global__ void __launch_bounds__(kThreads, (NV <= 1 ? 5 : 4)) spmm_kernel(SpmmA
             e = a.indptr[row + 1];
             if (e > s + a.chunk_nnz) e = s + a.chunk_nnz;
         }
-        Vec<W> acc[NV];
+        L acc[NV];
 #pragma unroll
         for (int t = 0; t < NV; ++t) acc[t].zero();
         for (int64_t k0 = s; k0 < e; k0 += 32) {
@@ -543,10 +658,10 @@ __global__ void __launch_bounds__(kThreads, (NV <= 1 ? 5 : 4)) spmm_kernel(SpmmA
             __syncwarp();
             int j = 0;
             for (; j + NG * UNROLL <= cnt; j += NG * UNROLL) {       // full steps: no predication
-                Vec<W> v[UNROLL][NV];
+                typename L::In v[UNROLL][NV];
 #pragma unroll
                 for (int u = 0; u < UNROLL; ++u) {
-                    const float *xr = a.X + (int64_t)s_col[w][j + u * NG + gi] * a.ldx;
+                    const T *xr = static_cast<const T *>(a.X) + (int64_t)s_col[w][j + u * NG + gi] * a.ldx;
 #pragma unroll
                     for (int t = 0; t < NV; ++t) {
                         if (fok[t]) v[u][t].load_ro(xr + fcol[t]); else v[u][t].zero();
@@ -564,12 +679,12 @@ __global__ void __launch_bounds__(kThreads, (NV <= 1 ? 5 : 4)) spmm_kernel(SpmmA
             for (; j < cnt; j += NG) {                               // tail: one entry per row group
                 const int jj = j + gi;
                 if (jj < cnt) {
-                    const float *xr = a.X + (int64_t)s_col[w][jj] * a.ldx;
+                    const T *xr = static_cast<const T *>(a.X) + (int64_t)s_col[w][jj] * a.ldx;
                     const float cs = CSCALE ? s_sc[w][jj] : 1.f;
 #pragma unroll
                     for (int t = 0; t < NV; ++t) {
                         if (fok[t]) {
-                            Vec<W> v;
+                            typename L::In v;
                             v.load_ro(xr + fcol[t]);
                             if (CSCALE) acc[t].fma(v, cs); else acc[t].add(v);
                         }
@@ -598,11 +713,7 @@ __global__ void __launch_bounds__(kThreads, (NV <= 1 ? 5 : 4)) spmm_kernel(SpmmA
             for (int t = 0; t < NV; ++t) {
                 if (!fok[t]) continue;
                 if (a.row_scale) acc[t].scale(rs);
-                if (a.accumulate) {
-                    Vec<W> old;
-                    old.load(yr + fcol[t]);
-                    acc[t].add(old);
-                }
+                if (a.accumulate) acc[t].add_f32(yr + fcol[t]);
                 acc[t].store(yr + fcol[t]);
             }
         }
@@ -647,54 +758,50 @@ __global__ void __launch_bounds__(kThreads) spmm_fixup_kernel(SpmmArgs a) {
     }
 }
 
-template <int W, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
+template <class L, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
 int launch_spmm(SpmmArgs a, cudaStream_t st) {
     static std::atomic<int> occ[kMaxDevices];            // per device, per instantiation
     const int dev = current_device();
     int blocks_per_sm = occ[dev].load(std::memory_order_relaxed);
     if (blocks_per_sm == 0) {
         int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spmm_kernel<W, G, NV, MAP, CSCALE, GUARD>, kThreads, 0) !=
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spmm_kernel<L, G, NV, MAP, CSCALE, GUARD>, kThreads, 0) !=
                 cudaSuccess || n < 1)
             n = 2;
         blocks_per_sm = n;
         occ[dev].store(n, std::memory_order_relaxed);
     }
-    constexpr int SLAB = G * W * NV;
+    constexpr int SLAB = G * L::kN * NV;
     a.n_tiles = (a.F + SLAB - 1) / SLAB;
     const int64_t items = a.n_chunks * a.n_tiles;
     int64_t want = (items + kWarps - 1) / kWarps;
     int64_t cap = (int64_t)sm_count() * blocks_per_sm;
     unsigned gx = (unsigned)(want < cap ? (want > 0 ? want : 1) : cap);
-    spmm_kernel<W, G, NV, MAP, CSCALE, GUARD><<<gx, kThreads, 0, st>>>(a);
+    spmm_kernel<L, G, NV, MAP, CSCALE, GUARD><<<gx, kThreads, 0, st>>>(a);
     g_launches += a.n_split > 0 ? 2 : 1;
-    if (a.n_split > 0) {
+    if (a.n_split > 0) {    // the partial sums are f32 rows for every lane type
         unsigned fx = (unsigned)((a.n_split + kWarps - 1) / kWarps);
-        if (W == 4) {
-            const int tiles = (a.F + 255) / 256;
-            spmm_fixup_kernel<4, 2, true><<<dim3(fx, tiles), kThreads, 0, st>>>(a);
-        } else {
-            const int tiles = (a.F + 255) / 256;
-            spmm_fixup_kernel<1, 8, true><<<dim3(fx, tiles), kThreads, 0, st>>>(a);
-        }
+        const int tiles = (a.F + 255) / 256;
+        if (L::kN == 1) spmm_fixup_kernel<1, 8, true><<<dim3(fx, tiles), kThreads, 0, st>>>(a);
+        else spmm_fixup_kernel<4, 2, true><<<dim3(fx, tiles), kThreads, 0, st>>>(a);
     }
     return BNS_OK;
 }
 
-template <int W, int G, int NV>
+template <class L, int G, int NV>
 int dispatch_flags(const SpmmArgs &a, cudaStream_t st) {
     const bool map = a.col_map != nullptr, cs = a.col_scale != nullptr || a.edge_weight != nullptr;
-    const bool guard = (a.F % (G * W * NV)) != 0;
+    const bool guard = (a.F % (G * L::kN * NV)) != 0;
     if (guard) {
-        if (map && cs) return launch_spmm<W, G, NV, true, true, true>(a, st);
-        if (map) return launch_spmm<W, G, NV, true, false, true>(a, st);
-        if (cs) return launch_spmm<W, G, NV, false, true, true>(a, st);
-        return launch_spmm<W, G, NV, false, false, true>(a, st);
+        if (map && cs) return launch_spmm<L, G, NV, true, true, true>(a, st);
+        if (map) return launch_spmm<L, G, NV, true, false, true>(a, st);
+        if (cs) return launch_spmm<L, G, NV, false, true, true>(a, st);
+        return launch_spmm<L, G, NV, false, false, true>(a, st);
     }
-    if (map && cs) return launch_spmm<W, G, NV, true, true, false>(a, st);
-    if (map) return launch_spmm<W, G, NV, true, false, false>(a, st);
-    if (cs) return launch_spmm<W, G, NV, false, true, false>(a, st);
-    return launch_spmm<W, G, NV, false, false, false>(a, st);
+    if (map && cs) return launch_spmm<L, G, NV, true, true, false>(a, st);
+    if (map) return launch_spmm<L, G, NV, true, false, false>(a, st);
+    if (cs) return launch_spmm<L, G, NV, false, true, false>(a, st);
+    return launch_spmm<L, G, NV, false, false, false>(a, st);
 }
 
 inline int64_t ws_ld(int64_t F) { return (F + 3) / 4 * 4; }
@@ -730,24 +837,43 @@ int pick_slab(int64_t F, int64_t x_rows, int32_t forced, int elem_bytes = 4) {
     return fmax;
 }
 
-int spmm_dispatch(const SpmmArgs &a, int64_t x_rows, int32_t slab_hint, cudaStream_t st) {
+int spmm_dispatch(const SpmmArgs &a, bool bf16, int64_t x_rows, int32_t slab_hint, cudaStream_t st) {
     const int64_t F = a.F;
     const bool vec = (F % 4 == 0) && (a.ldx % 4 == 0) && (a.ldy % 4 == 0) &&
                      ((reinterpret_cast<uintptr_t>(a.X) | reinterpret_cast<uintptr_t>(a.Y)) % 16 == 0);
+    BNS_REQUIRE(vec || !bf16, "spmm: bf16 rows need the 16-byte layout (F %lld, ldx %lld, ldy %lld)", (long long)F,
+                (long long)a.ldx, (long long)a.ldy);
     if (vec) {
-        int slab = pick_slab(F, x_rows, slab_hint);
+        int slab = pick_slab(F, x_rows, slab_hint, bf16 ? 2 : 4);
         while (slab > 32 && slab / 2 >= F) slab >>= 1;       // never wider than needed (F = 64 -> 64-wide groups)
         switch (slab) {
-            case 256: dispatch_flags<4, 32, 2>(a, st); break;
-            case 128: dispatch_flags<4, 32, 1>(a, st); break;
-            case 64:  dispatch_flags<4, 16, 1>(a, st); break;
-            default:  dispatch_flags<4, 8, 1>(a, st); break;
+            case 256: bf16 ? dispatch_flags<Bf16x8, 32, 1>(a, st) : dispatch_flags<Vec<4>, 32, 2>(a, st); break;
+            case 128: bf16 ? dispatch_flags<Bf16x8, 16, 1>(a, st) : dispatch_flags<Vec<4>, 32, 1>(a, st); break;
+            case 64:  bf16 ? dispatch_flags<Bf16x8, 8, 1>(a, st) : dispatch_flags<Vec<4>, 16, 1>(a, st); break;
+            default:  bf16 ? dispatch_flags<Bf16x8, 4, 1>(a, st) : dispatch_flags<Vec<4>, 8, 1>(a, st); break;
         }
     } else {
-        dispatch_flags<1, 32, 8>(a, st);
+        dispatch_flags<Vec<1>, 32, 8>(a, st);
     }
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
+}
+
+// What every entry point passes the same way: the chunk walk of g, X, Y and the split-row workspace.  The caller sets
+// the weights, the maps and (for compacted indices) indices / chunk_cnt.
+SpmmArgs spmm_args(const bns_graph_t *g, const void *X, int64_t ldx, int64_t F, float *Y, int64_t ldy, int accumulate,
+                   void *ws) {
+    SpmmArgs a = {};
+    a.indptr = g->indptr; a.indices = g->indices;
+    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part;
+    a.split_row = g->split_row; a.split_part = g->split_part;
+    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
+    a.X = X; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
+    a.edge_ld = 1;
+    a.n_direct = (int32_t)g->n_cols; a.accumulate = accumulate ? 1 : 0;
+    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
+    a.n_tiles = 1;
+    return a;
 }
 
 }  // namespace
@@ -756,6 +882,13 @@ extern "C" size_t bns_spmm_workspace_bytes(const bns_graph_t *g, int64_t F) {
     if (!g || F <= 0) return 0;
     return (size_t)g->n_parts * (size_t)ws_ld(F) * sizeof(float);
 }
+
+// the 16-byte gathers and the 2 x 16-byte stores of the bf16 lanes
+#define BNS_BF16_LAYOUT(fn)                                                                                            \
+    BNS_REQUIRE(F % 8 == 0 && ldx % 8 == 0 && ldy % 4 == 0 &&                                                          \
+                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
+                fn ": needs F %% 8 == 0, ldx %% 8 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "   \
+                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
 
 extern "C" int bns_spmm_sum_f32(const bns_graph_t *g, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                                 const float *row_scale, const float *col_scale, const float *edge_weight,
@@ -773,18 +906,10 @@ extern "C" int bns_spmm_sum_f32(const bns_graph_t *g, const float *X, int64_t ld
     if (col_map == nullptr) n_direct = g->n_cols;
     BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_f32: n_direct out of range");
     if (x_rows <= 0) x_rows = g->n_cols;
-    SpmmArgs a;
-    a.indptr = g->indptr; a.indices = g->indices;
-    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = nullptr;
-    a.split_row = g->split_row; a.split_part = g->split_part;
-    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
-    a.X = X; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
-    a.edge_perm = nullptr; a.edge_ld = 1;
-    a.n_direct = (int32_t)n_direct; a.accumulate = accumulate ? 1 : 0;
-    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
-    a.n_tiles = 1;
-    return spmm_dispatch(a, x_rows, slab_hint, as_stream(stream));
+    a.n_direct = (int32_t)n_direct;
+    return spmm_dispatch(a, false, x_rows, slab_hint, as_stream(stream));
 }
 
 // The same kernel over the per-epoch compacted indices of bns_graph_compact_cols: `cidx` already holds rows of X, the
@@ -803,18 +928,10 @@ extern "C" int bns_spmm_compact_f32(const bns_graph_t *g, const int32_t *cidx, c
     const size_t need = bns_spmm_workspace_bytes(g, F);
     if (need > 0 && (ws == nullptr || ws_bytes < need))
         return fail(BNS_E_WORKSPACE, "bns_spmm_compact_f32: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a;
-    a.indptr = g->indptr; a.indices = cidx;
-    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = chunk_cnt;
-    a.split_row = g->split_row; a.split_part = g->split_part;
-    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
-    a.X = X; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
-    a.row_scale = row_scale; a.col_scale = nullptr; a.edge_weight = cw; a.row_map = nullptr; a.col_map = nullptr;
-    a.edge_perm = nullptr; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    a.n_direct = (int32_t)g->n_cols; a.accumulate = accumulate ? 1 : 0;
-    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
-    a.n_tiles = 1;
-    return spmm_dispatch(a, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.indices = cidx; a.chunk_cnt = chunk_cnt;
+    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
+    return spmm_dispatch(a, false, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
 }
 
 // Y[orow(r)] (+)= sum_k w_k X[c_k] with w_k = weights[(perm ? perm[k] : k) * ldw]: the weighted aggregation of GATConv
@@ -831,260 +948,14 @@ extern "C" int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64
     const size_t need = bns_spmm_workspace_bytes(g, F);
     if (need > 0 && (ws == nullptr || ws_bytes < need))
         return fail(BNS_E_WORKSPACE, "bns_spmm_weighted_f32: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a;
-    a.indptr = g->indptr; a.indices = g->indices;
-    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = nullptr;
-    a.split_row = g->split_row; a.split_part = g->split_part;
-    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
-    a.X = X; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
-    a.row_scale = nullptr; a.col_scale = nullptr; a.edge_weight = weights; a.row_map = row_map; a.col_map = nullptr;
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.edge_weight = weights; a.row_map = row_map;
     a.edge_perm = perm_from_transpose ? g->perm : nullptr; a.edge_ld = ldw;
-    a.n_direct = (int32_t)g->n_cols; a.accumulate = accumulate ? 1 : 0;
-    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
-    a.n_tiles = 1;
-    return spmm_dispatch(a, x_rows > 0 ? x_rows : g->n_cols, 0, as_stream(stream));
+    return spmm_dispatch(a, false, x_rows > 0 ? x_rows : g->n_cols, 0, as_stream(stream));
 }
 
-// =================================================================================================
-// SpMM with a BF16 gather table (--agg-dtype bf16): X rows are bf16, everything else as spmm_kernel
-// =================================================================================================
-namespace {
-
-// Eight bf16 values of one 16-byte load, summed into eight f32 accumulators (bf16 -> f32 is exact: a shift).
-struct Bf16x8 {
-    uint4 u;
-    __device__ __forceinline__ void zero() { u = make_uint4(0u, 0u, 0u, 0u); }
-    __device__ __forceinline__ void load_ro(const uint16_t *p) { u = __ldg(reinterpret_cast<const uint4 *>(p)); }
-};
-__device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
-__device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-
-struct Acc8 {
-    float v[8];
-    __device__ __forceinline__ void zero() {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = 0.f;
-    }
-    __device__ __forceinline__ void add(const Bf16x8 &x) {
-        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { v[2 * i] += bf_lo(w[i]); v[2 * i + 1] += bf_hi(w[i]); }
-    }
-    __device__ __forceinline__ void fma(const Bf16x8 &x, float s) {
-        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) { v[2 * i] = fmaf(bf_lo(w[i]), s, v[2 * i]); v[2 * i + 1] = fmaf(bf_hi(w[i]), s, v[2 * i + 1]); }
-    }
-    __device__ __forceinline__ void scale(float s) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] *= s;
-    }
-    __device__ __forceinline__ void add_shfl_xor(int off) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], off);
-    }
-    __device__ __forceinline__ void add_f32(const float *p) {
-        const float4 a = *reinterpret_cast<const float4 *>(p), b = *reinterpret_cast<const float4 *>(p + 4);
-        v[0] += a.x; v[1] += a.y; v[2] += a.z; v[3] += a.w; v[4] += b.x; v[5] += b.y; v[6] += b.z; v[7] += b.w;
-    }
-    __device__ __forceinline__ void store(float *p) const {
-        *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]);
-        *reinterpret_cast<float4 *>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    }
-};
-
-// spmm_kernel with bf16 rows of X (ldx in elements): lane l of row group gi owns the 8 columns f0 + gl * 8 .. + 8, one
-// 16-byte load per gathered row, so a 256-wide slab is one 512-byte request per warp and each lane keeps 8 f32
-// accumulators (as the f32 kernel's 256-wide slab).  Work decomposition, column mapping, compaction, the partial sums
-// of split rows (f32, combined by spmm_fixup_kernel) and the epilogue are those of spmm_kernel.
-template <int G, bool MAP, bool CSCALE, bool GUARD>
-__global__ void __launch_bounds__(kThreads, 4) spmm_bf16_kernel(SpmmArgs a, const uint16_t *__restrict__ Xh) {
-    constexpr int NG = 32 / G;
-    constexpr int UNROLL = 8;
-    constexpr int SLAB = G * 8;
-    __shared__ int32_t s_col[kWarps][32];
-    __shared__ float s_sc[kWarps][32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int gi = lane / G, gl = lane % G;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    const int64_t items = a.n_chunks * a.n_tiles;
-    for (int64_t item = (int64_t)blockIdx.x * kWarps + w; item < items; item += warps_total) {
-        const int64_t c = item % a.n_chunks;
-        const int fcol = (int)(item / a.n_chunks) * SLAB + gl * 8;
-        const bool fok = !GUARD || fcol < a.F;
-        const int32_t row = a.chunk_row[c];
-        int32_t orow = row;
-        if (a.row_map) {
-            orow = a.row_map[row];
-            if (orow < 0) continue;
-        }
-        const int64_t s = a.chunk_start[c];
-        int64_t e;
-        if (a.chunk_cnt) {
-            const int32_t cnt = a.chunk_cnt[c];
-            if (cnt == 0 && a.accumulate && a.chunk_part[c] < 0) continue;
-            e = s + cnt;
-        } else {
-            e = a.indptr[row + 1];
-            if (e > s + a.chunk_nnz) e = s + a.chunk_nnz;
-        }
-        Acc8 acc;
-        acc.zero();
-        for (int64_t k0 = s; k0 < e; k0 += 32) {
-            const int64_t k = k0 + lane;
-            int32_t col = -1;
-            float sc = 1.f;
-            if (k < e) {
-                col = ld_stream_i32(a.indices + k);
-                if (CSCALE) {
-                    if (a.col_scale) sc = __ldg(a.col_scale + col);
-                    if (a.edge_weight) sc *= __ldg(a.edge_weight + (a.edge_perm ? (int64_t)__ldg(a.edge_perm + k) : k) * a.edge_ld);
-                }
-                if (MAP) {
-                    if (col >= a.n_direct) col = __ldg(a.col_map + (col - a.n_direct));
-                }
-            }
-            int cnt;
-            if (MAP) {
-                const unsigned m = __ballot_sync(0xffffffffu, col >= 0);
-                cnt = __popc(m);
-                if (col >= 0) {
-                    const int pos = __popc(m & ((1u << lane) - 1u));
-                    s_col[w][pos] = col;
-                    if (CSCALE) s_sc[w][pos] = sc;
-                }
-            } else {
-                const int64_t rem = e - k0;
-                cnt = rem < 32 ? (int)rem : 32;
-                s_col[w][lane] = col;
-                if (CSCALE) s_sc[w][lane] = sc;
-            }
-            __syncwarp();
-            int j = 0;
-            for (; j + NG * UNROLL <= cnt; j += NG * UNROLL) {
-                Bf16x8 v[UNROLL];
-#pragma unroll
-                for (int u = 0; u < UNROLL; ++u) {
-                    if (fok) v[u].load_ro(Xh + (int64_t)s_col[w][j + u * NG + gi] * a.ldx + fcol); else v[u].zero();
-                }
-#pragma unroll
-                for (int u = 0; u < UNROLL; ++u) {
-                    if (CSCALE) acc.fma(v[u], s_sc[w][j + u * NG + gi]); else acc.add(v[u]);
-                }
-            }
-            for (; j < cnt; j += NG) {
-                const int jj = j + gi;
-                if (jj < cnt && fok) {
-                    Bf16x8 v;
-                    v.load_ro(Xh + (int64_t)s_col[w][jj] * a.ldx + fcol);
-                    if (CSCALE) acc.fma(v, s_sc[w][jj]); else acc.add(v);
-                }
-            }
-            __syncwarp();
-        }
-        if (NG > 1) {
-#pragma unroll
-            for (int off = 16; off >= G; off >>= 1) acc.add_shfl_xor(off);
-            if (gi != 0) continue;
-        }
-        if (!fok) continue;
-        const int32_t part = a.chunk_part[c];
-        if (part >= 0) {
-            acc.store(a.ws + (int64_t)part * a.ldws + fcol);
-        } else {
-            float *yr = a.Y + (int64_t)orow * a.ldy + fcol;
-            if (a.row_scale) acc.scale(a.row_scale[row]);
-            if (a.accumulate) acc.add_f32(yr);
-            acc.store(yr);
-        }
-    }
-}
-
-template <int G, bool MAP, bool CSCALE, bool GUARD>
-int launch_spmm_bf16(SpmmArgs a, const uint16_t *Xh, cudaStream_t st) {
-    static std::atomic<int> occ[kMaxDevices];
-    const int dev = current_device();
-    int blocks_per_sm = occ[dev].load(std::memory_order_relaxed);
-    if (blocks_per_sm == 0) {
-        int n = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spmm_bf16_kernel<G, MAP, CSCALE, GUARD>, kThreads, 0) !=
-                cudaSuccess || n < 1)
-            n = 2;
-        blocks_per_sm = n;
-        occ[dev].store(n, std::memory_order_relaxed);
-    }
-    constexpr int SLAB = G * 8;
-    a.n_tiles = (a.F + SLAB - 1) / SLAB;
-    const int64_t items = a.n_chunks * a.n_tiles;
-    int64_t want = (items + kWarps - 1) / kWarps;
-    int64_t cap = (int64_t)sm_count() * blocks_per_sm;
-    unsigned gx = (unsigned)(want < cap ? (want > 0 ? want : 1) : cap);
-    spmm_bf16_kernel<G, MAP, CSCALE, GUARD><<<gx, kThreads, 0, st>>>(a, Xh);
-    g_launches += a.n_split > 0 ? 2 : 1;
-    if (a.n_split > 0) {    // the partial sums are f32 rows: the f32 kernel's fix-up pass combines them
-        unsigned fx = (unsigned)((a.n_split + kWarps - 1) / kWarps);
-        spmm_fixup_kernel<4, 2, true><<<dim3(fx, (a.F + 255) / 256), kThreads, 0, st>>>(a);
-    }
-    return BNS_OK;
-}
-
-template <int G>
-int dispatch_bf16_flags(const SpmmArgs &a, const uint16_t *Xh, cudaStream_t st) {
-    const bool map = a.col_map != nullptr, cs = a.col_scale != nullptr || a.edge_weight != nullptr;
-    if ((a.F % (G * 8)) != 0) {
-        if (map && cs) return launch_spmm_bf16<G, true, true, true>(a, Xh, st);
-        if (map) return launch_spmm_bf16<G, true, false, true>(a, Xh, st);
-        if (cs) return launch_spmm_bf16<G, false, true, true>(a, Xh, st);
-        return launch_spmm_bf16<G, false, false, true>(a, Xh, st);
-    }
-    if (map && cs) return launch_spmm_bf16<G, true, true, false>(a, Xh, st);
-    if (map) return launch_spmm_bf16<G, true, false, false>(a, Xh, st);
-    if (cs) return launch_spmm_bf16<G, false, true, false>(a, Xh, st);
-    return launch_spmm_bf16<G, false, false, false>(a, Xh, st);
-}
-
-int spmm_bf16_dispatch(const SpmmArgs &a, const uint16_t *Xh, int64_t x_rows, int32_t slab_hint, cudaStream_t st) {
-    int slab = pick_slab(a.F, x_rows, slab_hint, sizeof(uint16_t));
-    while (slab > 32 && slab / 2 >= a.F) slab >>= 1;
-    switch (slab) {
-        case 256: dispatch_bf16_flags<32>(a, Xh, st); break;
-        case 128: dispatch_bf16_flags<16>(a, Xh, st); break;
-        case 64:  dispatch_bf16_flags<8>(a, Xh, st); break;
-        default:  dispatch_bf16_flags<4>(a, Xh, st); break;
-    }
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
-
-// the 16-byte gathers and the 2 x 16-byte stores of the bf16 kernel
-#define BNS_BF16_LAYOUT(fn)                                                                                            \
-    BNS_REQUIRE(F % 8 == 0 && ldx % 8 == 0 && ldy % 4 == 0 &&                                                          \
-                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
-                fn ": needs F %% 8 == 0, ldx %% 8 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "   \
-                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
-
-__global__ void __launch_bounds__(kThreads) cvt_rows_bf16_kernel(const float *__restrict__ src, int64_t lds,
-                                                                 uint16_t *__restrict__ dst, int64_t ldd, int64_t n_rows,
-                                                                 int64_t F, bool vec) {
-    const int64_t per_row = vec ? F / 4 : F, total = n_rows * per_row;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t r = i / per_row, c = i - r * per_row;
-        if (vec) {
-            const float4 v = __ldg(reinterpret_cast<const float4 *>(src + r * lds) + c);
-            uint2 o;
-            o.x = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.x)) |
-                  ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.y)) << 16);
-            o.y = (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.z)) |
-                  ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v.w)) << 16);
-            reinterpret_cast<uint2 *>(dst + r * ldd)[c] = o;
-        } else {
-            dst[r * ldd + c] = __bfloat16_as_ushort(__float2bfloat16_rn(__ldg(src + r * lds + c)));
-        }
-    }
-}
-
-}  // namespace
-
+// The same sums over a bf16 gather table (--agg-dtype bf16): X rows are bf16 (ldx in bf16 elements), widened exactly
+// and summed in f32; Y, the weights and the workspace are f32 as above.
 extern "C" int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                                  const float *row_scale, const float *col_scale, const float *edge_weight,
                                  const int32_t *row_map, const int32_t *col_map, int64_t n_direct, int64_t x_rows,
@@ -1102,18 +973,10 @@ extern "C" int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X, int64_
     if (col_map == nullptr) n_direct = g->n_cols;
     BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_bf16: n_direct out of range");
     if (x_rows <= 0) x_rows = g->n_cols;
-    SpmmArgs a;
-    a.indptr = g->indptr; a.indices = g->indices;
-    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = nullptr;
-    a.split_row = g->split_row; a.split_part = g->split_part;
-    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
-    a.X = nullptr; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
-    a.edge_perm = nullptr; a.edge_ld = 1;
-    a.n_direct = (int32_t)n_direct; a.accumulate = accumulate ? 1 : 0;
-    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
-    a.n_tiles = 1;
-    return spmm_bf16_dispatch(a, X, x_rows, slab_hint, as_stream(stream));
+    a.n_direct = (int32_t)n_direct;
+    return spmm_dispatch(a, true, x_rows, slab_hint, as_stream(stream));
 }
 
 extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
@@ -1129,19 +992,30 @@ extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, 
     const size_t need = bns_spmm_workspace_bytes(g, F);
     if (need > 0 && (ws == nullptr || ws_bytes < need))
         return fail(BNS_E_WORKSPACE, "bns_spmm_compact_bf16: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a;
-    a.indptr = g->indptr; a.indices = cidx;
-    a.chunk_row = g->chunk_row; a.chunk_start = g->chunk_start; a.chunk_part = g->chunk_part; a.chunk_cnt = chunk_cnt;
-    a.split_row = g->split_row; a.split_part = g->split_part;
-    a.n_chunks = g->n_chunks; a.n_split = g->n_split; a.chunk_nnz = g->chunk_nnz;
-    a.X = nullptr; a.ldx = ldx; a.Y = Y; a.ldy = ldy; a.F = (int32_t)F;
-    a.row_scale = row_scale; a.col_scale = nullptr; a.edge_weight = cw; a.row_map = nullptr; a.col_map = nullptr;
-    a.edge_perm = nullptr; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    a.n_direct = (int32_t)g->n_cols; a.accumulate = accumulate ? 1 : 0;
-    a.ws = reinterpret_cast<float *>(ws); a.ldws = ws_ld(F);
-    a.n_tiles = 1;
-    return spmm_bf16_dispatch(a, X, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.indices = cidx; a.chunk_cnt = chunk_cnt;
+    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
+    return spmm_dispatch(a, true, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
 }
+
+namespace {
+
+__global__ void __launch_bounds__(kThreads) cvt_rows_bf16_kernel(const float *__restrict__ src, int64_t lds,
+                                                                 uint16_t *__restrict__ dst, int64_t ldd, int64_t n_rows,
+                                                                 int64_t F, bool vec) {
+    const int64_t per_row = vec ? F / 4 : F, total = n_rows * per_row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / per_row, c = i - r * per_row;
+        if (vec) {
+            const float4 v = __ldg(reinterpret_cast<const float4 *>(src + r * lds) + c);
+            reinterpret_cast<uint2 *>(dst + r * ldd)[c] = make_uint2(bf16x2_rn(v.x, v.y), bf16x2_rn(v.z, v.w));
+        } else {
+            dst[r * ldd + c] = bf16_rn(__ldg(src + r * lds + c));
+        }
+    }
+}
+
+}  // namespace
 
 extern "C" int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *dst, int64_t ldd, int64_t n_rows, int64_t F,
                                      void *stream) {
@@ -1288,32 +1162,31 @@ extern "C" int bns_sddmm_dot_f32(const bns_graph_t *g, const float *A, int64_t l
 // =================================================================================================
 namespace {
 
-// one warp per row, 16-byte lanes when aligned
-template <bool VEC, bool SCATTER>
-__global__ void __launch_bounds__(kThreads) rows_kernel(const float *__restrict__ src, int64_t lds, float *dst,
+// One warp per row: the pack  dst[i] = src[idx[i]] / div  or the scatter  dst[idx[i]] += src[i] / div  (the ids of one
+// call are distinct).  The wire side (dst of the pack, src of the scatter) holds the lane type's elements: f32 with
+// 16-byte or scalar lanes, or bf16 x 8 (--comm-dtype bf16); the other side is f32.
+template <class L, bool SCATTER>
+__global__ void __launch_bounds__(kThreads) rows_kernel(const std::conditional_t<SCATTER, typename L::T, float> *__restrict__ src,
+                                                        int64_t lds, std::conditional_t<SCATTER, float, typename L::T> *dst,
                                                         int64_t ldd, const int64_t *__restrict__ idx, int64_t k,
                                                         int32_t F, float div) {
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
     for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
+        // The bf16 pack's entry point requires the ids.  Without this the compiler adds a second copy of the row loop
+        // for a NULL idx and spills around the division's slow path.
+        if constexpr (L::kN == 8 && !SCATTER) __builtin_assume(idx != nullptr);
         const int64_t r = idx ? idx[i] : i;
-        const float *s = SCATTER ? src + i * lds : src + r * lds;
-        float *d = SCATTER ? dst + r * ldd : dst + i * ldd;
-        if (VEC) {
-            for (int f = lane * 4; f < F; f += 128) {
-                float4 v = *reinterpret_cast<const float4 *>(s + f);
-                v.x = __fdiv_rn(v.x, div); v.y = __fdiv_rn(v.y, div); v.z = __fdiv_rn(v.z, div); v.w = __fdiv_rn(v.w, div);
-                if (SCATTER) {
-                    float4 o = *reinterpret_cast<float4 *>(d + f);
-                    v.x += o.x; v.y += o.y; v.z += o.z; v.w += o.w;
-                }
-                *reinterpret_cast<float4 *>(d + f) = v;
-            }
-        } else {
-            for (int f = lane; f < F; f += 32) {
-                float v = __fdiv_rn(s[f], div);
-                if (SCATTER) v += d[f];
-                d[f] = v;
+        const auto *s = SCATTER ? src + i * lds : src + r * lds;
+        auto *d = SCATTER ? dst + r * ldd : dst + i * ldd;
+        for (int f = lane * L::kN; f < F; f += 32 * L::kN) {
+            if constexpr (SCATTER) {
+                L v;
+                v.load_div(s + f, div);
+                v.add_f32(d + f);
+                v.store(d + f);
+            } else {
+                *reinterpret_cast<typename L::Wire *>(d + f) = L::div_round(s + f, div);
             }
         }
     }
@@ -1341,9 +1214,9 @@ extern "C" int bns_gather_div_f32(const float *H, int64_t ldh, int64_t F, const 
     BNS_REQUIRE(div != 0.f, "bns_gather_div_f32: division by zero");
     cudaStream_t st = as_stream(stream);
     if (vec_ok(H, out, F, ldh, ldo))
-        rows_kernel<true, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
+        rows_kernel<Vec<4>, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
     else
-        rows_kernel<false, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
+        rows_kernel<Vec<1>, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -1358,9 +1231,9 @@ extern "C" int bns_scatter_add_div_f32(float *G, int64_t ldg, int64_t F, const i
     BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_f32: division by zero");
     cudaStream_t st = as_stream(stream);
     if (vec_ok(G, src, F, ldg, lds))
-        rows_kernel<true, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
+        rows_kernel<Vec<4>, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
     else
-        rows_kernel<false, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
+        rows_kernel<Vec<1>, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -1948,7 +1821,9 @@ __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long
 }
 
 // Each warp moves whole rows  H[idx[i]] / div  into the peer's slab (16-byte stores over NVLink).
-// The last CTA to finish (device-scope ticket) publishes the flag with a system-scope release.
+// The last CTA to finish (device-scope ticket) publishes the flag with a system-scope release.  This publish is not
+// fused.cuh's publish_flags on purpose: it raises one flag and re-arms the ticket with a plain store, and moving it onto
+// the shared one would change this kernel's code.
 template <bool VEC>
 __global__ void __launch_bounds__(kThreads) p2p_put_rows_kernel(const float *__restrict__ H, int64_t ldh, int32_t F,
                                                                const int64_t *__restrict__ idx, int64_t k, float div,
@@ -2043,10 +1918,10 @@ extern "C" int bns_p2p_create(bns_p2p_t **out, int32_t rank, int32_t world, size
     cudaFuncGetAttributes(&fa, p2p_put_rows_kernel<true>);
     cudaFuncGetAttributes(&fa, p2p_put_rows_kernel<false>);
     cudaFuncGetAttributes(&fa, p2p_wait_kernel);
-    cudaFuncGetAttributes(&fa, rows_kernel<true, true>);
-    cudaFuncGetAttributes(&fa, rows_kernel<false, true>);
-    cudaFuncGetAttributes(&fa, rows_kernel<true, false>);
-    cudaFuncGetAttributes(&fa, rows_kernel<false, false>);
+    cudaFuncGetAttributes(&fa, rows_kernel<Vec<4>, true>);
+    cudaFuncGetAttributes(&fa, rows_kernel<Vec<1>, true>);
+    cudaFuncGetAttributes(&fa, rows_kernel<Vec<4>, false>);
+    cudaFuncGetAttributes(&fa, rows_kernel<Vec<1>, false>);
     preload_exchange_kernels();
     *out = p;
     return BNS_OK;

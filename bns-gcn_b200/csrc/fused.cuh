@@ -363,41 +363,10 @@ extern "C" int bns_epoch_maps_update(const bns_epoch_maps *maps, void *fill_base
 // =====================================================================================================================
 namespace {
 
-struct PutAllDev {
-    int32_t n_seg;
-    int64_t row_begin[kMaxPeers + 1];
-    float *remote[kMaxPeers];
-    unsigned long long *flag[kMaxPeers];
-    int64_t src_begin[kMaxPeers];
-    float div[kMaxPeers];
-    const float *H; int64_t ldh; int32_t F;
-    const int64_t *idx;                         // concatenated in segment order, or NULL
-    int64_t ld_remote;
-    unsigned long long flag_value; const unsigned long long *flag_value_dev; unsigned int *ticket;
-};
-
-template <bool VEC>
-__global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllDev a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
-        int s = 0;
-        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
-        const int64_t local = i - a.row_begin[s];
-        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
-        const float *src = a.H + r * a.ldh;
-        float *d = a.remote[s] + local * a.ld_remote;
-        const float div = a.div[s];
-        if (VEC) {
-            for (int f = lane * 4; f < a.F; f += 128) {
-                float4 v = *reinterpret_cast<const float4 *>(src + f);
-                v.x = __fdiv_rn(v.x, div); v.y = __fdiv_rn(v.y, div); v.z = __fdiv_rn(v.z, div); v.w = __fdiv_rn(v.w, div);
-                *reinterpret_cast<float4 *>(d + f) = v;
-            }
-        } else {
-            for (int f = lane; f < a.F; f += 32) d[f] = __fdiv_rn(src[f], div);
-        }
-    }
+// The end of a put: every CTA's stores are made visible system-wide, then the last CTA to finish (device-scope ticket)
+// re-arms the ticket and publishes each segment's flag with a system-scope release.
+template <class D>
+__device__ __forceinline__ void publish_flags(const D &a) {
     __threadfence_system();
     __syncthreads();
     __shared__ bool s_last;
@@ -411,6 +380,38 @@ __global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllDev a) {
         __threadfence_system();
         st_release_sys(a.flag[threadIdx.x], a.flag_value + (a.flag_value_dev ? *a.flag_value_dev : 0ull));
     }
+}
+
+struct PutAllDev {
+    int32_t n_seg;
+    int64_t row_begin[kMaxPeers + 1];
+    float *remote[kMaxPeers];                   // rows of L::T (ld_remote in those elements)
+    unsigned long long *flag[kMaxPeers];
+    int64_t src_begin[kMaxPeers];
+    float div[kMaxPeers];
+    const float *H; int64_t ldh; int32_t F;
+    const int64_t *idx;                         // concatenated in segment order, or NULL
+    int64_t ld_remote;
+    unsigned long long flag_value; const unsigned long long *flag_value_dev; unsigned int *ticket;
+};
+
+// one warp per row: the remote row = H[r] / div in the lane type's wire format (f32, or bf16 after the f32 division)
+template <class L>
+__global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllDev a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
+        int s = 0;
+        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
+        const int64_t local = i - a.row_begin[s];
+        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
+        const float *src = a.H + r * a.ldh;
+        typename L::T *d = reinterpret_cast<typename L::T *>(a.remote[s]) + local * a.ld_remote;
+        const float div = a.div[s];
+        for (int f = lane * L::kN; f < a.F; f += 32 * L::kN)
+            *reinterpret_cast<typename L::Wire *>(d + f) = L::div_round(src + f, div);
+    }
+    publish_flags(a);
 }
 
 struct PutIdsDev {
@@ -429,19 +430,7 @@ __global__ void __launch_bounds__(256) p2p_put_ids_kernel(PutIdsDev a) {
         while (s + 1 < a.n_seg && a.begin[s + 1] <= i) ++s;
         a.remote[s][i - a.begin[s]] = a.src[i];
     }
-    __threadfence_system();
-    __syncthreads();
-    __shared__ bool s_last;
-    if (threadIdx.x == 0) {
-        const unsigned int done = atomicAdd(a.ticket, 1u);
-        s_last = (done == gridDim.x - 1);
-        if (s_last) atomicExch(a.ticket, 0u);
-    }
-    __syncthreads();
-    if (s_last && (int)threadIdx.x < a.n_seg) {
-        __threadfence_system();
-        st_release_sys(a.flag[threadIdx.x], a.flag_value + (a.flag_value_dev ? *a.flag_value_dev : 0ull));
-    }
+    publish_flags(a);
 }
 
 struct WaitAllDev {
@@ -467,15 +456,16 @@ __global__ void p2p_wait_all_kernel(WaitAllDev a, unsigned long long value, cons
 struct ScatterAllDev {
     int32_t n_seg;
     const int32_t *inv[kMaxPeers];
-    const float *recv[kMaxPeers];
+    const float *recv[kMaxPeers];               // rows of L::T (ld_recv in those elements)
     float div[kMaxPeers];
     int64_t ld_recv;
     float *G; int64_t ldg; int32_t F; int64_t n_rows;
 };
 
 // one warp per destination row: contributions of the peers are added in table order (= the reference's ring order,
-// helper/feature_buffer.py:111-129), each with a true division -- bit-identical to P-1 successive scatter-adds
-template <bool VEC>
+// helper/feature_buffer.py:111-129), each with a true division -- bit-identical to P-1 successive scatter-adds.  The
+// column loop is warp-uniform: every lane takes every shuffle, and the lanes past F load and store nothing.
+template <class L>
 __global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDev a) {
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
@@ -484,162 +474,54 @@ __global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDe
         if (lane < a.n_seg) mine = a.inv[lane][row];
         if (__ballot_sync(0xffffffffu, mine >= 0) == 0u) continue;
         float *g = a.G + row * a.ldg;
-        if (VEC) {
-            for (int f = lane * 4; f < a.F; f += 128) {
-                float4 v = *reinterpret_cast<float4 *>(g + f);
-                for (int s = 0; s < a.n_seg; ++s) {
-                    const int32_t k = __shfl_sync(0xffffffffu, mine, s);
-                    if (k < 0) continue;
-                    const float4 r = *reinterpret_cast<const float4 *>(a.recv[s] + (int64_t)k * a.ld_recv + f);
-                    const float d = a.div[s];
-                    v.x += __fdiv_rn(r.x, d); v.y += __fdiv_rn(r.y, d); v.z += __fdiv_rn(r.z, d); v.w += __fdiv_rn(r.w, d);
-                }
-                *reinterpret_cast<float4 *>(g + f) = v;
-            }
-        } else {
-            for (int f0 = 0; f0 < a.F; f0 += 32) {
-                const int f = f0 + lane;
-                float v = f < a.F ? g[f] : 0.f;
-                for (int s = 0; s < a.n_seg; ++s) {
-                    const int32_t k = __shfl_sync(0xffffffffu, mine, s);
-                    if (k < 0 || f >= a.F) continue;
-                    v += __fdiv_rn(a.recv[s][(int64_t)k * a.ld_recv + f], a.div[s]);
-                }
-                if (f < a.F) g[f] = v;
-            }
-        }
-    }
-}
-
-// ---- bf16 boundary exchange (--comm-dtype bf16): 8 elements per lane and 16-byte access, no scalar path ----
-
-__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
-    return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(lo)) |
-           ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(hi)) << 16);
-}
-__device__ __forceinline__ float bf16_lo(uint32_t w) { return __uint_as_float(w << 16); }
-__device__ __forceinline__ float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u); }
-
-// bf16(src[0:8] / div) as one 16-byte word (the division in f32, then one rounding)
-__device__ __forceinline__ uint4 div_round8(const float *src, float div) {
-    const float4 a = *reinterpret_cast<const float4 *>(src), b = *reinterpret_cast<const float4 *>(src + 4);
-    uint4 o;
-    o.x = bf16x2_rn(__fdiv_rn(a.x, div), __fdiv_rn(a.y, div));
-    o.y = bf16x2_rn(__fdiv_rn(a.z, div), __fdiv_rn(a.w, div));
-    o.z = bf16x2_rn(__fdiv_rn(b.x, div), __fdiv_rn(b.y, div));
-    o.w = bf16x2_rn(__fdiv_rn(b.z, div), __fdiv_rn(b.w, div));
-    return o;
-}
-
-// (a, b) += widen(r) / div, each element as the f32 siblings add it
-__device__ __forceinline__ void add_div8(float4 &a, float4 &b, uint4 r, float div) {
-    a.x += __fdiv_rn(bf16_lo(r.x), div); a.y += __fdiv_rn(bf16_hi(r.x), div);
-    a.z += __fdiv_rn(bf16_lo(r.y), div); a.w += __fdiv_rn(bf16_hi(r.y), div);
-    b.x += __fdiv_rn(bf16_lo(r.z), div); b.y += __fdiv_rn(bf16_hi(r.z), div);
-    b.z += __fdiv_rn(bf16_lo(r.w), div); b.w += __fdiv_rn(bf16_hi(r.w), div);
-}
-
-// p2p_put_all_kernel with the remote rows stored as bf16 (remote / ld_remote in bf16 elements)
-__global__ void __launch_bounds__(kThreads) p2p_put_all_bf16_kernel(PutAllDev a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
-        int s = 0;
-        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
-        const int64_t local = i - a.row_begin[s];
-        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
-        const float *src = a.H + r * a.ldh;
-        uint16_t *d = reinterpret_cast<uint16_t *>(a.remote[s]) + local * a.ld_remote;
-        for (int f = lane * 8; f < a.F; f += 256) *reinterpret_cast<uint4 *>(d + f) = div_round8(src + f, a.div[s]);
-    }
-    __threadfence_system();
-    __syncthreads();
-    __shared__ bool s_last;
-    if (threadIdx.x == 0) {
-        const unsigned int done = atomicAdd(a.ticket, 1u);
-        s_last = (done == gridDim.x - 1);
-        if (s_last) atomicExch(a.ticket, 0u);
-    }
-    __syncthreads();
-    if (s_last && (int)threadIdx.x < a.n_seg) {
-        __threadfence_system();
-        st_release_sys(a.flag[threadIdx.x], a.flag_value + (a.flag_value_dev ? *a.flag_value_dev : 0ull));
-    }
-}
-
-// scatter_rows_all_kernel reading bf16 recv rows (ld_recv in bf16 elements): same order, same per-element arithmetic
-__global__ void __launch_bounds__(kThreads) scatter_rows_all_bf16_kernel(ScatterAllDev a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < a.n_rows; row += warps_total) {
-        int32_t mine = -1;
-        if (lane < a.n_seg) mine = a.inv[lane][row];
-        if (__ballot_sync(0xffffffffu, mine >= 0) == 0u) continue;
-        float *g = a.G + row * a.ldg;
-        for (int f0 = 0; f0 < a.F; f0 += 256) {                 // warp-uniform: every lane takes every shuffle
-            const int f = f0 + lane * 8;
+        for (int f0 = 0; f0 < a.F; f0 += 32 * L::kN) {
+            const int f = f0 + lane * L::kN;
             const bool on = f < a.F;
-            float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
-            if (on) {
-                v0 = *reinterpret_cast<const float4 *>(g + f);
-                v1 = *reinterpret_cast<const float4 *>(g + f + 4);
-            }
+            L v;
+            v.zero();
+            if (on) v.load(g + f);
             for (int s = 0; s < a.n_seg; ++s) {
                 const int32_t k = __shfl_sync(0xffffffffu, mine, s);
                 if (k < 0 || !on) continue;
-                const uint16_t *r = reinterpret_cast<const uint16_t *>(a.recv[s]) + (int64_t)k * a.ld_recv + f;
-                add_div8(v0, v1, *reinterpret_cast<const uint4 *>(r), a.div[s]);
+                v.add_div(reinterpret_cast<const typename L::T *>(a.recv[s]) + (int64_t)k * a.ld_recv + f, a.div[s]);
             }
-            if (on) {
-                *reinterpret_cast<float4 *>(g + f) = v0;
-                *reinterpret_cast<float4 *>(g + f + 4) = v1;
-            }
+            if (on) v.store(g + f);
         }
     }
 }
 
-}  // namespace
-
-namespace {
-// see bns_p2p_create: a kernel's first launch loads its code, which synchronises the context -- never while a flag wait spins
-void preload_exchange_kernels() {
-    cudaFuncAttributes fa;
-    cudaFuncGetAttributes(&fa, p2p_put_all_bf16_kernel);
-    cudaFuncGetAttributes(&fa, scatter_rows_all_bf16_kernel);
-    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<true>);
-    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<false>);
-    cudaFuncGetAttributes(&fa, p2p_put_ids_kernel);
-    cudaFuncGetAttributes(&fa, p2p_wait_all_kernel);
-    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<true>);
-    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<false>);
-    cudaFuncGetAttributes(&fa, epoch_maps_kernel);
-}
-}  // namespace
-
-extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
-                                   int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
-                                   uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
-    BNS_REQUIRE(p && segs, "bns_p2p_put_all_f32: NULL argument");
-    BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "bns_p2p_put_all_f32: too many segments");
-    BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "bns_p2p_put_all_f32: bad flag index");
-    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "bns_p2p_put_all_f32: bad ticket index");
-    BNS_REQUIRE(F > 0 && ldh >= F && ld_remote >= F, "bns_p2p_put_all_f32: bad shape");
+// bns_p2p_put_all_f32 / _bf16 (T = float / uint16_t on the wire): one set of checks and one segment table
+template <class T>
+int put_all(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh, int64_t F,
+            const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index, uint64_t flag_value,
+            const uint64_t *flag_value_dev, void *stream) {
+    constexpr bool bf16 = sizeof(T) == 2;       // bf16 rows: 16-byte access only, no scalar path
+    const char *fn = bf16 ? "bns_p2p_put_all_bf16" : "bns_p2p_put_all_f32";
+    BNS_REQUIRE(p && segs, "%s: NULL argument", fn);
+    BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "%s: too many segments", fn);
+    BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "%s: bad flag index", fn);
+    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "%s: bad ticket index", fn);
+    BNS_REQUIRE(F > 0 && ldh >= F && ld_remote >= F, "%s: bad shape", fn);
+    BNS_REQUIRE(!bf16 || (F % 8 == 0 && ldh % 8 == 0 && ld_remote % 8 == 0),
+                "%s: F, ldh and ld_remote must be multiples of 8 (F %lld, ldh %lld, ld_remote %lld)", fn, (long long)F,
+                (long long)ldh, (long long)ld_remote);
     if (segs->n_seg == 0) return BNS_OK;
     PutAllDev a;
     a.n_seg = segs->n_seg;
-    // the 16-byte path also needs every destination 16-byte aligned; the scalar path takes rows of any width
+    // the f32 16-byte path also needs every destination 16-byte aligned; the scalar path takes rows of any width
     bool vec = F % 4 == 0 && ldh % 4 == 0 && ld_remote % 4 == 0 && (reinterpret_cast<uintptr_t>(H) & 15u) == 0;
     for (int s = 0; s <= segs->n_seg; ++s) a.row_begin[s] = segs->row_begin[s];
     for (int s = 0; s < segs->n_seg; ++s) {
         const int peer = segs->peer[s];
         const int64_t k = segs->row_begin[s + 1] - segs->row_begin[s];
-        BNS_REQUIRE(peer >= 0 && peer < p->world && peer != p->rank, "bns_p2p_put_all_f32: bad peer %d", peer);
-        BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "bns_p2p_put_all_f32: peer %d not connected", peer);
-        BNS_REQUIRE(k >= 0, "bns_p2p_put_all_f32: negative row count");
-        BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "bns_p2p_put_all_f32: division by zero");
-        BNS_REQUIRE(segs->remote_off[s] % 4 == 0 &&
-                        segs->remote_off[s] + (size_t)k * ld_remote * 4 <= p->peer_slab_bytes[peer],
-                    "bns_p2p_put_all_f32: remote range of segment %d outside peer %d's slab", s, peer);
+        BNS_REQUIRE(peer >= 0 && peer < p->world && peer != p->rank, "%s: bad peer %d", fn, peer);
+        BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "%s: peer %d not connected", fn, peer);
+        BNS_REQUIRE(k >= 0, "%s: negative row count", fn);
+        BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "%s: division by zero", fn);
+        BNS_REQUIRE(segs->remote_off[s] % (bf16 ? 16 : 4) == 0 &&
+                        segs->remote_off[s] + (size_t)k * ld_remote * sizeof(T) <= p->peer_slab_bytes[peer],
+                    bf16 ? "%s: remote range of segment %d outside peer %d's slab or not 16-byte aligned"
+                         : "%s: remote range of segment %d outside peer %d's slab", fn, s, peer);
         vec = vec && segs->remote_off[s] % 16 == 0;
         a.remote[s] = reinterpret_cast<float *>(p->peer_slab[peer] + segs->remote_off[s]);
         a.flag[s] = p->peer_flags[peer] + flag_index;
@@ -647,16 +529,73 @@ extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_
         a.div[s] = k == 0 ? 1.f : segs->div[s];
     }
     const int64_t total = segs->row_begin[segs->n_seg];
-    BNS_REQUIRE(total == 0 || H, "bns_p2p_put_all_f32: NULL source");
+    BNS_REQUIRE(total == 0 || H, "%s: NULL source", fn);
+    BNS_REQUIRE(!bf16 || (reinterpret_cast<uintptr_t>(H) & 15u) == 0, "%s: source not 16-byte aligned", fn);
     a.H = H; a.ldh = ldh; a.F = (int32_t)F; a.idx = idx_cat; a.ld_remote = ld_remote;
     a.flag_value = flag_value; a.flag_value_dev = reinterpret_cast<const unsigned long long *>(flag_value_dev);
     a.ticket = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(p->flags) + align256((size_t)p->n_flags * 8)) + ticket_index;
     const unsigned grid = rows_grid(total);
-    if (vec) p2p_put_all_kernel<true><<<grid, kThreads, 0, as_stream(stream)>>>(a);
-    else p2p_put_all_kernel<false><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    if (bf16) p2p_put_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else if (vec) p2p_put_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else p2p_put_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
+}
+
+// bns_scatter_rows_all_f32 / _bf16 (T = float / uint16_t received rows)
+template <class T>
+int scatter_rows_all(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg, const int32_t *const *inv,
+                     const T *const *recv, int64_t ld_recv, const float *div, void *stream) {
+    constexpr bool bf16 = sizeof(T) == 2;       // bf16 rows: 16-byte access only, no scalar path
+    const char *fn = bf16 ? "bns_scatter_rows_all_bf16" : "bns_scatter_rows_all_f32";
+    BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "%s: too many segments", fn);
+    if (n_seg == 0 || n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(G && inv && recv && div && F > 0 && ldg >= F && ld_recv >= F, "%s: bad argument", fn);
+    BNS_REQUIRE(!bf16 || (F % 8 == 0 && ldg % 4 == 0 && ld_recv % 8 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0),
+                "%s: needs F %% 8 == 0, ldg %% 4 == 0, ld_recv %% 8 == 0 and a 16-byte aligned G "
+                "(F %lld, ldg %lld, ld_recv %lld)", fn, (long long)F, (long long)ldg, (long long)ld_recv);
+    ScatterAllDev a;
+    a.n_seg = n_seg;
+    bool vec = F % 4 == 0 && ldg % 4 == 0 && ld_recv % 4 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0;
+    for (int s = 0; s < n_seg; ++s) {
+        const bool aligned = (reinterpret_cast<uintptr_t>(recv[s]) & 15u) == 0;
+        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f && (aligned || !bf16),
+                    bf16 ? "%s: bad segment %d (NULL, misaligned or division by zero)" : "%s: bad segment %d", fn, s);
+        a.inv[s] = inv[s]; a.recv[s] = reinterpret_cast<const float *>(recv[s]); a.div[s] = div[s];
+        vec = vec && aligned;
+    }
+    a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
+    const unsigned grid = rows_grid(n_rows);
+    if (bf16) scatter_rows_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else if (vec) scatter_rows_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else scatter_rows_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// see bns_p2p_create: a kernel's first launch loads its code, which synchronises the context -- never while a flag wait spins
+void preload_exchange_kernels() {
+    cudaFuncAttributes fa;
+    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Bf16x8>);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<Bf16x8>);
+    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<4>>);
+    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<1>>);
+    cudaFuncGetAttributes(&fa, p2p_put_ids_kernel);
+    cudaFuncGetAttributes(&fa, p2p_wait_all_kernel);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<Vec<4>>);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<Vec<1>>);
+    cudaFuncGetAttributes(&fa, epoch_maps_kernel);
+}
+
+}  // namespace
+
+extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
+                                   int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
+                                   uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
+    return put_all<float>(p, segs, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value, flag_value_dev,
+                          stream);
 }
 
 extern "C" int bns_p2p_put_ids_i64(bns_p2p_t *p, int32_t n_seg, const int64_t *begin, const int32_t *peers,
@@ -716,126 +655,24 @@ extern "C" int bns_p2p_wait_all(bns_p2p_t *p, int32_t n, const int32_t *flag_ind
 extern "C" int bns_scatter_rows_all_f32(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
                                         const int32_t *const *inv, const float *const *recv, int64_t ld_recv,
                                         const float *div, void *stream) {
-    BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "bns_scatter_rows_all_f32: too many segments");
-    if (n_seg == 0 || n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(G && inv && recv && div && F > 0 && ldg >= F && ld_recv >= F, "bns_scatter_rows_all_f32: bad argument");
-    ScatterAllDev a;
-    a.n_seg = n_seg;
-    bool vec = F % 4 == 0 && ldg % 4 == 0 && ld_recv % 4 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0;
-    for (int s = 0; s < n_seg; ++s) {
-        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f, "bns_scatter_rows_all_f32: bad segment %d", s);
-        a.inv[s] = inv[s]; a.recv[s] = recv[s]; a.div[s] = div[s];
-        vec = vec && (reinterpret_cast<uintptr_t>(recv[s]) & 15u) == 0;
-    }
-    a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
-    if (vec) scatter_rows_all_kernel<true><<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
-    else scatter_rows_all_kernel<false><<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
+    return scatter_rows_all<float>(G, ldg, n_rows, F, n_seg, inv, recv, ld_recv, div, stream);
 }
 
 extern "C" int bns_p2p_put_all_bf16(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
                                     int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
                                     uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
-    BNS_REQUIRE(p && segs, "bns_p2p_put_all_bf16: NULL argument");
-    BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "bns_p2p_put_all_bf16: too many segments");
-    BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "bns_p2p_put_all_bf16: bad flag index");
-    BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "bns_p2p_put_all_bf16: bad ticket index");
-    BNS_REQUIRE(F > 0 && ldh >= F && ld_remote >= F, "bns_p2p_put_all_bf16: bad shape");
-    BNS_REQUIRE(F % 8 == 0 && ldh % 8 == 0 && ld_remote % 8 == 0,
-                "bns_p2p_put_all_bf16: F, ldh and ld_remote must be multiples of 8 (F %lld, ldh %lld, ld_remote %lld)",
-                (long long)F, (long long)ldh, (long long)ld_remote);
-    if (segs->n_seg == 0) return BNS_OK;
-    PutAllDev a;
-    a.n_seg = segs->n_seg;
-    for (int s = 0; s <= segs->n_seg; ++s) a.row_begin[s] = segs->row_begin[s];
-    for (int s = 0; s < segs->n_seg; ++s) {
-        const int peer = segs->peer[s];
-        const int64_t k = segs->row_begin[s + 1] - segs->row_begin[s];
-        BNS_REQUIRE(peer >= 0 && peer < p->world && peer != p->rank, "bns_p2p_put_all_bf16: bad peer %d", peer);
-        BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "bns_p2p_put_all_bf16: peer %d not connected", peer);
-        BNS_REQUIRE(k >= 0, "bns_p2p_put_all_bf16: negative row count");
-        BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "bns_p2p_put_all_bf16: division by zero");
-        BNS_REQUIRE(segs->remote_off[s] % 16 == 0 &&
-                        segs->remote_off[s] + (size_t)k * ld_remote * 2 <= p->peer_slab_bytes[peer],
-                    "bns_p2p_put_all_bf16: remote range of segment %d outside peer %d's slab or not 16-byte aligned", s,
-                    peer);
-        a.remote[s] = reinterpret_cast<float *>(p->peer_slab[peer] + segs->remote_off[s]);
-        a.flag[s] = p->peer_flags[peer] + flag_index;
-        a.src_begin[s] = segs->src_begin[s];
-        a.div[s] = k == 0 ? 1.f : segs->div[s];
-    }
-    const int64_t total = segs->row_begin[segs->n_seg];
-    BNS_REQUIRE(total == 0 || H, "bns_p2p_put_all_bf16: NULL source");
-    BNS_REQUIRE((reinterpret_cast<uintptr_t>(H) & 15u) == 0, "bns_p2p_put_all_bf16: source not 16-byte aligned");
-    a.H = H; a.ldh = ldh; a.F = (int32_t)F; a.idx = idx_cat; a.ld_remote = ld_remote;
-    a.flag_value = flag_value; a.flag_value_dev = reinterpret_cast<const unsigned long long *>(flag_value_dev);
-    a.ticket = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(p->flags) + align256((size_t)p->n_flags * 8)) + ticket_index;
-    p2p_put_all_bf16_kernel<<<rows_grid(total), kThreads, 0, as_stream(stream)>>>(a);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
+    return put_all<uint16_t>(p, segs, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value,
+                             flag_value_dev, stream);
 }
 
 extern "C" int bns_scatter_rows_all_bf16(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
                                          const int32_t *const *inv, const uint16_t *const *recv, int64_t ld_recv,
                                          const float *div, void *stream) {
-    BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "bns_scatter_rows_all_bf16: too many segments");
-    if (n_seg == 0 || n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(G && inv && recv && div && F > 0 && ldg >= F && ld_recv >= F, "bns_scatter_rows_all_bf16: bad argument");
-    BNS_REQUIRE(F % 8 == 0 && ldg % 4 == 0 && ld_recv % 8 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0,
-                "bns_scatter_rows_all_bf16: needs F %% 8 == 0, ldg %% 4 == 0, ld_recv %% 8 == 0 and a 16-byte aligned G "
-                "(F %lld, ldg %lld, ld_recv %lld)", (long long)F, (long long)ldg, (long long)ld_recv);
-    ScatterAllDev a;
-    a.n_seg = n_seg;
-    for (int s = 0; s < n_seg; ++s) {
-        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f && (reinterpret_cast<uintptr_t>(recv[s]) & 15u) == 0,
-                    "bns_scatter_rows_all_bf16: bad segment %d (NULL, misaligned or division by zero)", s);
-        a.inv[s] = inv[s]; a.recv[s] = reinterpret_cast<const float *>(recv[s]); a.div[s] = div[s];
-    }
-    a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
-    scatter_rows_all_bf16_kernel<<<rows_grid(n_rows), kThreads, 0, as_stream(stream)>>>(a);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
+    return scatter_rows_all<uint16_t>(G, ldg, n_rows, F, n_seg, inv, recv, ld_recv, div, stream);
 }
 
 // ---- the staged transport's pack (K3) and scatter (K5) with a bf16 wire side, and the exact widening ----
 namespace {
-
-// out[i] = bf16(H[idx[i]] / div): one warp per row
-__global__ void __launch_bounds__(kThreads) gather_div_bf16_kernel(const float *__restrict__ H, int64_t ldh,
-                                                                   uint16_t *__restrict__ out, int64_t ldo,
-                                                                   const int64_t *__restrict__ idx, int64_t k, int32_t F,
-                                                                   float div) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
-        const float *s = H + idx[i] * ldh;
-        uint16_t *d = out + i * ldo;
-        for (int f = lane * 8; f < F; f += 256) *reinterpret_cast<uint4 *>(d + f) = div_round8(s + f, div);
-    }
-}
-
-// G[idx[i]] += widen(src[i]) / div: one warp per row (the ids of one call are distinct)
-__global__ void __launch_bounds__(kThreads) scatter_add_div_bf16_kernel(const uint16_t *__restrict__ src, int64_t lds,
-                                                                        float *G, int64_t ldg,
-                                                                        const int64_t *__restrict__ idx, int64_t k,
-                                                                        int32_t F, float div) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
-        const uint16_t *s = src + i * lds;
-        float *d = G + idx[i] * ldg;
-        for (int f = lane * 8; f < F; f += 256) {
-            float4 v0 = *reinterpret_cast<const float4 *>(d + f), v1 = *reinterpret_cast<const float4 *>(d + f + 4);
-            add_div8(v0, v1, *reinterpret_cast<const uint4 *>(s + f), div);
-            *reinterpret_cast<float4 *>(d + f) = v0;
-            *reinterpret_cast<float4 *>(d + f + 4) = v1;
-        }
-    }
-}
 
 __global__ void __launch_bounds__(kThreads) cvt_rows_bf16_f32_kernel(const uint16_t *__restrict__ src, int64_t lds,
                                                                      float *__restrict__ dst, int64_t ldd, int64_t n_rows,
@@ -847,7 +684,7 @@ __global__ void __launch_bounds__(kThreads) cvt_rows_bf16_f32_kernel(const uint1
             const uint2 w = __ldg(reinterpret_cast<const uint2 *>(src + r * lds) + c);
             reinterpret_cast<float4 *>(dst + r * ldd)[c] = make_float4(bf16_lo(w.x), bf16_hi(w.x), bf16_lo(w.y), bf16_hi(w.y));
         } else {
-            dst[r * ldd + c] = __uint_as_float((uint32_t)__ldg(src + r * lds + c) << 16);
+            dst[r * ldd + c] = bf16_lo(__ldg(src + r * lds + c));
         }
     }
 }
@@ -869,7 +706,7 @@ extern "C" int bns_gather_div_bf16(const float *H, int64_t ldh, int64_t F, const
     BNS_REQUIRE(bf16_rows_ok(H, out, F, ldh, ldo),
                 "bns_gather_div_bf16: needs F, ldh, ldo multiples of 8 and 16-byte aligned H, out (F %lld, ldh %lld, "
                 "ldo %lld)", (long long)F, (long long)ldh, (long long)ldo);
-    gather_div_bf16_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
+    rows_kernel<Bf16x8, false><<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -885,7 +722,7 @@ extern "C" int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const 
     BNS_REQUIRE(bf16_rows_ok(G, src, F, ldg, lds),
                 "bns_scatter_add_div_bf16: needs F, ldg, lds multiples of 8 and 16-byte aligned G, src (F %lld, "
                 "ldg %lld, lds %lld)", (long long)F, (long long)ldg, (long long)lds);
-    scatter_add_div_bf16_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
+    rows_kernel<Bf16x8, true><<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

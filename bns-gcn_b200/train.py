@@ -332,24 +332,11 @@ class TrainState:
     arena: Optional[object] = None               # fused.ParamArena when the fused training step is on
 
 
-def _fused_eligible(args, layer_size, dev) -> bool:
-    """The fused training step (fused.py) covers the BASELINE configuration families: GraphSAGE / GCN, --use-pp, LayerNorm +
-    ReLU between the layers, no trailing linear layers, widths the 16-byte vector / TMA paths take.  BNS_FUSED=0 turns
-    it off (the op-by-op autograd path, kept for every other configuration, then runs here too)."""
-    import os
-    from .module import dense
-    if os.environ.get("BNS_FUSED", "1") == "0" or dense.MODE != "tc" or dev.type != "cuda":
-        return False
-    if args.model not in ('graphsage', 'gcn') or not args.use_pp or args.n_linear != 0 or args.norm != 'layer':
-        return False
-    k0 = 2 * layer_size[0] if args.model == 'graphsage' else layer_size[0]       # width of the precomputed layer-0 input
-    widths_ok = k0 % 4 == 0 and all(w % 4 == 0 and w <= 1024 for w in layer_size[1:-1])
-    return widths_ok and len(layer_size) >= 3
-
-
 def _fused_step_refusals(args, layer_size, dev, width_why=None) -> list:
-    """Every reason why the fused training step does not run for this configuration (empty: it runs); the bf16 modes
-    of ``--agg-dtype`` / ``--comm-dtype`` / ``--dense-dtype`` only exist there.  ``width_why``: the mode's own width
+    """Every reason why the fused training step (fused.py) does not run for this configuration; empty: it runs.  It
+    covers the BASELINE configuration families: GraphSAGE / GCN, --use-pp, LayerNorm + ReLU between the layers, no
+    trailing linear layers, widths the 16-byte vector / TMA paths take.  BNS_FUSED=0 turns it off (the op-by-op
+    autograd path, kept for every other configuration, then runs here too).  ``width_why``: a bf16 mode's own width
     rule, when it is broken."""
     import os
     from .module import dense
@@ -366,68 +353,76 @@ def _fused_step_refusals(args, layer_size, dev, width_why=None) -> list:
         why.append(f"--norm {args.norm}")
     if dev.type != "cuda" or dense.MODE != "tc":
         why.append("no CUDA device with the wgmma GEMMs")
+    k0 = 2 * layer_size[0] if args.model == 'graphsage' else layer_size[0]       # width of the precomputed layer-0 input
+    bad = sorted(({k0} if k0 % 4 else set()) | {w for w in layer_size[1:-1] if w % 4 or w > 1024})
+    if bad:
+        why.append(f"layer widths {', '.join(map(str, bad))} do not fit the fused step (multiples of 4, hidden at most "
+                   f"1024)")
+    if len(layer_size) < 3:
+        why.append("fewer than two layers")
     if width_why:
         why.append(width_why)
-    if not why and not _fused_eligible(args, layer_size, dev):
-        why.append("the layer widths do not fit the fused step")
     return why
 
 
-def check_agg_dtype(args, layer_size, dev) -> bool:
-    """Whether ``--agg-dtype bf16`` is on.  It only exists on the fused training step: any configuration that step does
-    not take raises ``ValueError`` naming why, rather than training in f32 behind the user's back."""
-    mode = getattr(args, 'agg_dtype', 'f32')
-    if mode == 'f32':
-        return False
-    if mode != 'bf16':
-        raise ValueError(f"--agg-dtype {mode!r}: expected 'f32' or 'bf16'")
-    width_why = None
+def _fused_eligible(args, layer_size, dev) -> bool:
+    return not _fused_step_refusals(args, layer_size, dev)
+
+
+def _hidden_x8(args, layer_size):
     if any(w % 8 for w in layer_size[1:-1]):
-        width_why = f"hidden width {args.n_hidden} is not a multiple of 8 (bf16 rows are gathered 8 at a time)"
-    why = _fused_step_refusals(args, layer_size, dev, width_why)
+        return f"hidden width {args.n_hidden} is not a multiple of 8 (bf16 rows are gathered 8 at a time)"
+    return None
+
+
+def _exchanged_x8(args, layer_size):
+    bad = sorted({w for w in layer_size[1:-1] if w % 8})
+    if bad:
+        return f"exchanged width {', '.join(map(str, bad))} is not a multiple of 8 (bf16 rows move 8 at a time)"
+    return None
+
+
+# --<flag>-dtype: the width rule its bf16 mode adds to the fused step's (a function returning the broken rule's message
+# or None; None in place of the function: nothing more), and what the check
+# returns for f32 and for bf16
+_DTYPE_FLAGS = {
+    'agg': (_hidden_x8, False, True),
+    'comm': (_exchanged_x8, 'f32', 'bf16'),
+    'dense': (None, False, True),
+}
+
+
+def _check_dtype_flag(flag, args, layer_size, dev):
+    """The bf16 modes only exist on the fused training step: any configuration that step does not take raises
+    ``ValueError`` naming every reason, rather than training in f32 behind the user's back."""
+    width_rule, off, on = _DTYPE_FLAGS[flag]
+    mode = getattr(args, f'{flag}_dtype', 'f32')
+    if mode == 'f32':
+        return off
+    if mode != 'bf16':
+        raise ValueError(f"--{flag}-dtype {mode!r}: expected 'f32' or 'bf16'")
+    why = _fused_step_refusals(args, layer_size, dev, width_rule(args, layer_size) if width_rule else None)
     if why:
-        raise ValueError("--agg-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
-    return True
+        raise ValueError(f"--{flag}-dtype bf16 needs the fused training step, which this run does not take: "
+                         + "; ".join(why))
+    return on
+
+
+def check_agg_dtype(args, layer_size, dev) -> bool:
+    """Whether ``--agg-dtype bf16`` is on: the aggregation gathers from bf16 tables, with f32 sums."""
+    return _check_dtype_flag('agg', args, layer_size, dev)
 
 
 def check_comm_dtype(args, layer_size, dev) -> str:
-    """The element type of the boundary rows on the wire: ``'f32'``, or ``'bf16'`` (``--comm-dtype bf16``), which only
-    exists on the fused training step -- its layers take the halo rows as bf16 and hand their halo gradient back to the
-    exchange.  Any configuration that step does not take raises ``ValueError`` naming every reason."""
-    mode = getattr(args, 'comm_dtype', 'f32')
-    if mode == 'f32':
-        return mode
-    if mode != 'bf16':
-        raise ValueError(f"--comm-dtype {mode!r}: expected 'f32' or 'bf16'")
-    width_why = None
-    bad = sorted({w for w in layer_size[1:-1] if w % 8})
-    if bad:
-        width_why = f"exchanged width {', '.join(map(str, bad))} is not a multiple of 8 (bf16 rows move 8 at a time)"
-    why = _fused_step_refusals(args, layer_size, dev, width_why)
-    if why:
-        raise ValueError("--comm-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
-    return mode
+    """The element type of the boundary rows on the wire: ``'f32'``, or ``'bf16'`` (``--comm-dtype bf16``), where the
+    fused layers take the halo rows as bf16 and hand their halo gradient back to the exchange."""
+    return _check_dtype_flag('comm', args, layer_size, dev)
 
 
 def check_dense_dtype(args, layer_size, dev) -> bool:
     """Whether ``--dense-dtype bf16`` is on: every GEMM of the fused layers (forward, input and weight gradients) takes
-    its operands rounded to bf16 inside the kernel, with f32 sums.  It only exists on the fused training step; any
-    configuration that step does not take raises ``ValueError`` naming every reason."""
-    mode = getattr(args, 'dense_dtype', 'f32')
-    if mode == 'f32':
-        return False
-    if mode != 'bf16':
-        raise ValueError(f"--dense-dtype {mode!r}: expected 'f32' or 'bf16'")
-    k0 = 2 * layer_size[0] if args.model == 'graphsage' else layer_size[0]      # as _fused_eligible
-    bad = sorted(({k0} if k0 % 4 else set()) | {w for w in layer_size[1:-1] if w % 4 or w > 1024})
-    width_why = None
-    if bad or len(layer_size) < 3:
-        width_why = (f"layer widths {', '.join(map(str, bad))} do not fit the fused step (multiples of 4, hidden at most "
-                     f"1024)" if bad else "fewer than two layers")
-    why = _fused_step_refusals(args, layer_size, dev, width_why)
-    if why:
-        raise ValueError("--dense-dtype bf16 needs the fused training step, which this run does not take: " + "; ".join(why))
-    return True
+    its operands rounded to bf16 inside the kernel, with f32 sums."""
+    return _check_dtype_flag('dense', args, layer_size, dev)
 
 
 def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:

@@ -606,17 +606,19 @@ def test_flag_value_from_device_and_shared_tickets(lib, dev, fabric):
         assert np.array_equal(p1.words[:4000 * 64].cpu().numpy().reshape(4000, 64), want)
 
 
-@pytest.mark.parametrize("F,shift", [(41, 0), (44, 1), (44, 0), (256, 0), (256, 1)])
-def test_scatter_rows_all(lib, dev, F, shift):
+@pytest.mark.parametrize("F,shift,n_seg", [(41, 0, 5), (44, 1, 5), (44, 0, 5), (256, 0, 5), (256, 1, 5), (8, 0, 7)],
+                         ids=["41-0", "44-1", "44-0", "256-0", "256-1", "8-0-7seg"])
+def test_scatter_rows_all(lib, dev, F, shift, n_seg):
     """``bns_scatter_rows_all_f32``: G[r] += recv_s[inv_s[r]] / div_s for the segments in table order, with F = 41, a
-    receive buffer one float off alignment (both scalar) and the aligned 16-byte path."""
+    receive buffer one float off alignment (both scalar) and the aligned 16-byte path, the latter also at F = 8 with 7
+    segments, where only 2 lanes of a warp hold columns but every lane takes part in the segment shuffles."""
     g = np.random.default_rng(F + shift)
-    n_rows, n_seg = 3000, 5
+    n_rows = 3000
     ld = F + 4
     G0 = g.standard_normal((n_rows, F)).astype(np.float32)
     inv, recv, keep = [], [], []
     for s in range(n_seg):
-        k = [700, 0, 1500, 1, 2999][s]
+        k = [700, 0, 1500, 1, 2999, 40, 3000][s]
         sel = g.permutation(n_rows)[:k]
         m = np.full(n_rows, -1, np.int32)
         m[sel] = np.arange(k, dtype=np.int32)
@@ -626,7 +628,7 @@ def test_scatter_rows_all(lib, dev, F, shift):
         buf = torch.zeros(max(k, 1) * ld + 4, device=dev)
         buf[shift:shift + r.size] = torch.from_numpy(r.reshape(-1)).to(dev)
         keep.append((torch.from_numpy(m).to(dev), buf))
-    div = [0.3, 1.0, 0.26, 7.0, 0.1]
+    div = [0.3, 1.0, 0.26, 7.0, 0.1, 3.0, 0.7][:n_seg]
     want = G0.copy()
     for s in range(n_seg):
         rows = np.nonzero(inv[s] >= 0)[0]
