@@ -76,6 +76,7 @@ class ParamArena:
         self.exp_avg = torch.zeros(off, dtype=torch.float32, device=dev)
         self.exp_avg_sq = torch.zeros(off, dtype=torch.float32, device=dev)
         self.params = [p for _, p in params]
+        self.names = [n for n, _ in params]
         with torch.no_grad():
             for p in self.params:
                 o, n, _ = self.slots[id(p)]
@@ -110,6 +111,11 @@ class ParamArena:
         for s in shape:
             n *= s
         return self.flat_g[o:o + n].view(shape)
+
+    def unpadded(self, flat: torch.Tensor, p: torch.nn.Parameter) -> torch.Tensor:
+        """``p``'s slot of one of the four flat buffers, with ``p``'s own shape (the pad left out)."""
+        o, n, _ = self.slots[id(p)]
+        return flat[o:o + n].view(p.shape)
 
     # ---- derived parameters ------------------------------------------------------------------------------------------
     def _add(self, key, entry: DeriveEntry, out: torch.Tensor) -> torch.Tensor:
@@ -183,6 +189,39 @@ class FusedAdam(torch.optim.Optimizer):
                   "bns_adam_step_f32")
         a.refresh(advance=self.step_dev)
         return None
+
+    _HYPER = ("lr", "betas", "eps", "weight_decay")
+
+    def state_dict(self) -> dict:
+        """Adam's state as copies on the device: ``{"step": int64 [1], "state": {parameter name: {"exp_avg",
+        "exp_avg_sq"}} (each moment unpadded, in its parameter's shape), "param_groups": [the hyperparameters]}``."""
+        a = self.arena
+        state = {name: {"exp_avg": a.unpadded(a.exp_avg, p).clone(), "exp_avg_sq": a.unpadded(a.exp_avg_sq, p).clone()}
+                 for name, p in zip(a.names, a.params)}
+        g = self.param_groups[0]
+        return {"step": self.step_dev.clone(), "state": state,
+                "param_groups": [{k: g[k] for k in self._HYPER}]}
+
+    @torch.no_grad()
+    def load_state_dict(self, state_dict: dict) -> None:
+        """The inverse of ``state_dict``: the moments go into their arena slots (the pad stays zero), the step into
+        ``step_dev`` in place (a captured graph keeps reading the same counter).  The weights are not part of it: after
+        loading them into the model, call ``arena.refresh(advance=None)``."""
+        a = self.arena
+        got = state_dict["state"]
+        if set(got) != set(a.names):
+            raise ValueError(f"FusedAdam.load_state_dict: parameters {sorted(set(a.names) - set(got))} missing, "
+                             f"{sorted(set(got) - set(a.names))} unexpected")
+        for name, p in zip(a.names, a.params):
+            for key, flat in (("exp_avg", a.exp_avg), ("exp_avg_sq", a.exp_avg_sq)):
+                src = got[name][key]
+                if tuple(src.shape) != tuple(p.shape):
+                    raise ValueError(f"FusedAdam.load_state_dict: {name}.{key} has shape {tuple(src.shape)}, the "
+                                     f"parameter {tuple(p.shape)}")
+                a.unpadded(flat, p).copy_(src)
+        self.step_dev.copy_(torch.as_tensor(state_dict["step"]).reshape(1))
+        for k, v in state_dict["param_groups"][0].items():
+            self.param_groups[0][k] = v
 
 
 # ---- loss ------------------------------------------------------------------------------------------------------------

@@ -83,6 +83,15 @@ def build_parser():
                              "results that no longer match the reference to 1e-4.  Master weights, gradients, the "
                              "all-reduce, Adam, the loss and evaluation stay f32.  Only with the fused training step "
                              "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+    parser.add_argument(*_spellings("save-state-every"), type=int, default=0,
+                        help="NEW: after every N-th epoch, and after the last one, all ranks write the training state "
+                             "(weights, Adam moments and step, the CUDA generators, the evaluator's best model, the "
+                             "seed) to checkpoint/<graph_name>_state/, which --resume continues from.  0: never.  "
+                             "Independent of --eval")
+    parser.add_argument(*_spellings("resume"), action='store_true',
+                        help="NEW: before the first epoch, load the state saved under this run's graph name and "
+                             "continue with the next epoch up to --n-epochs (which counts all epochs).  The resumed run "
+                             "is bit-identical to an uninterrupted one")
     return parser
 
 

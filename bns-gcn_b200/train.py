@@ -662,12 +662,20 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     through ``evaluate.Evaluator`` -- on the GPU with the same kernels, synchronously, instead of a CPU thread pool;
     ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: regenerated from ``args.dataset``).
     With ``args.parallel_eval`` as well, EVERY rank evaluates its own nodes on its partition instead
-    (``evaluate.ParallelEvaluator``) and the full graph is never built; inductive runs are refused."""
+    (``evaluate.ParallelEvaluator``) and the full graph is never built; inductive runs are refused.
+    ``args.save_state_every`` / ``args.resume``: write the training state every N epochs and after the last one, or
+    continue from the saved one (``state.py``)."""
     rank, size = _rank_size()
     parallel = getattr(args, 'eval', False) and getattr(args, 'parallel_eval', False)
     if parallel and args.inductive:
         raise ValueError("--parallel-eval: inductive runs evaluate on the train | val subgraph and the full graph, "
                          "which the training partitions do not hold; drop --parallel-eval to evaluate them on rank 0")
+    from . import state
+    save_every = getattr(args, 'save_state_every', 0)
+    saved = None
+    if getattr(args, 'resume', False):
+        saved = state.load(args, rank)                  # refuses before any setup work
+        args.seed = saved["seed"]                       # a launch without --fix-seed drew a new one
     st = setup(graph, node_dict, gpb, args, device)
     dev = st.feat.device
     evaluator = None
@@ -682,16 +690,20 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
         fg = full_graph if full_graph is not None else make_graph(args.dataset, seed=getattr(args, 'graph_seed', 0),
                                                                   device=dev)
         evaluator = Evaluator(args, fg, dev)
+    start = 0
+    if saved is not None:
+        start = state.restore(st, saved, evaluator)
+        print(f'Process {rank} resumes after {start} epochs from {saved["dir"]}')
     train_dur, comm_dur, reduce_dur = [], [], []
     torch.cuda.reset_peak_memory_stats(dev)
     print(f'Process {rank} start training')
     loss = None
-    for epoch in range(args.n_epochs):
+    for epoch in range(start, args.n_epochs):
         torch.cuda.synchronize(dev)
         t0 = time.time()
         loss = train_epoch(st, epoch)
         torch.cuda.synchronize(dev)
-        if epoch >= 5:                                                      # train.py:415-418
+        if epoch - start >= 5:                                              # train.py:415-418 (epochs of this process)
             train_dur.append(time.time() - t0)
             comm_dur.append(comm_timer.tot_time())
             reduce_dur.append(ctx.reducer.last_reduce_seconds())
@@ -702,6 +714,8 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
                 np.mean(reduce_dur) if reduce_dur else float('nan'), loss.item() / max(st.part_train, 1)))
             if evaluator is not None:                                       # train.py:427-442
                 evaluator.after_epoch(st.model, epoch)
+        if save_every > 0 and ((epoch + 1) % save_every == 0 or epoch + 1 == args.n_epochs):
+            state.save(st, epoch + 1, evaluator)
     print_memory("memory stats")
     if evaluator is not None:                                               # train.py:446-456
         evaluator.finish(st.model)
