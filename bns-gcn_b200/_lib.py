@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -164,6 +164,13 @@ SIGNATURES = {
                                   c_int64, c_int64, c_int64, c_int64, c_void_p]),
     "bns_dense_nt_bf16": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_int64, c_int64,
                                   c_void_p, c_size_t, c_void_p]),
+    # ---- ABI 7 ----
+    "bns_spmm_sum_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_int64, c_void_p, c_void_p,
+                                 c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int32, c_int, c_void_p, c_size_t,
+                                 c_void_p]),
+    "bns_spmm_compact_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
+                                     c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int, c_void_p, c_size_t, c_void_p]),
+    "bns_cvt_rows_f32_fp8": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p]),
 }
 
 

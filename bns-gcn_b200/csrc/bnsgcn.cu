@@ -1,8 +1,9 @@
 // bnsgcn.cu -- sm_90a kernels + the C ABI of include/bnsgcn.h.
 //
 // Hot kernels (all HBM/L2-bound f32 gather / scatter work; no tensor-core shaped math here):
-//   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers; f32 or bf16
-//                                 (--agg-dtype bf16) gather tables, f32 sums; cvt_rows_bf16_kernel
+//   spmm_kernel        K1/K1b/K2  nnz-balanced CSR row-sum, one warp per chunk, 16 B/lane gathers; f32, bf16 or
+//                                 row-scaled e4m3 (--agg-dtype bf16 / fp8) gather tables, f32 sums;
+//                                 cvt_rows_bf16_kernel, cvt_rows_fp8_kernel
 //   spmm_fixup_kernel  deterministic combine of rows longer than one chunk
 //   gather / scatter   K3/K5      boundary pack and gradient scatter-add, f32 or bf16 (--comm-dtype bf16) wire rows
 //   philox_key / take  K6         counter-based exactly-k sampling (with cub radix sort)
@@ -12,6 +13,7 @@
 #include "bnsgcn.h"
 
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
@@ -444,7 +446,8 @@ __device__ __forceinline__ void add_div8(float *v, uint4 r, float div) {
 }
 
 // Lane types: what one lane of a row-wise kernel holds.  Vec<4> is one 16-byte f32 vector, Vec<1> the scalar path
-// for rows that are not 16-byte aligned, Bf16x8 eight bf16 values of one 16-byte load widened into eight f32 sums.
+// for rows that are not 16-byte aligned, Bf16x8 eight bf16 values of one 16-byte load widened into eight f32 sums
+// (E4m3x16, SpMM only, is below).
 // T / kN: element type and count of one lane's slice of a row in X (SpMM) or on the wire (exchange).  In: what one
 // gather loads.  The sums, the partial sums of split rows and Y are f32 for every lane type.
 // min_blocks(NV, G, MAP && !CSCALE): the second argument of spmm_kernel's __launch_bounds__.
@@ -557,6 +560,72 @@ struct Bf16x8 {
     }
 };
 
+// two e4m3 codes (low byte first) widened exactly to f32, through f16
+__device__ __forceinline__ float2 e4m3x2_f32(uint32_t w16) {
+    return __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)w16, __NV_E4M3)));
+}
+
+// E4m3x16: sixteen e4m3 codes of one 16-byte load (--agg-dtype fp8), widened exactly into sixteen f32 sums.  The row's
+// power-of-two scale (SpmmArgsFp8::x_scale) is folded into the entry's weight, so every entry takes fma().  SpMM only.
+struct E4m3x16 {
+    using T = uint8_t;
+    static constexpr int kN = 16;
+    static constexpr int min_blocks(int, int, bool) { return 3; }
+    struct In {
+        uint4 u;
+        __device__ __forceinline__ void zero() { u = make_uint4(0u, 0u, 0u, 0u); }
+        __device__ __forceinline__ void load_ro(const uint8_t *p) { u = __ldg(reinterpret_cast<const uint4 *>(p)); }
+    };
+    float v[16];
+    __device__ __forceinline__ void zero() {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] = 0.f;
+    }
+    __device__ __forceinline__ void store(float *p) const {
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) *reinterpret_cast<float4 *>(p + i) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
+    }
+    __device__ __forceinline__ void fma(const In &x, float s) {
+        const uint32_t w[4] = {x.u.x, x.u.y, x.u.z, x.u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 a = e4m3x2_f32(w[i] & 0xffffu), b = e4m3x2_f32(w[i] >> 16);
+            v[4 * i] = fmaf(a.x, s, v[4 * i]); v[4 * i + 1] = fmaf(a.y, s, v[4 * i + 1]);
+            v[4 * i + 2] = fmaf(b.x, s, v[4 * i + 2]); v[4 * i + 3] = fmaf(b.y, s, v[4 * i + 3]);
+        }
+    }
+    __device__ __forceinline__ void add(const In &x) { fma(x, 1.f); }
+    __device__ __forceinline__ void add_f32(const float *p) {
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+            const float4 a = *reinterpret_cast<const float4 *>(p + i);
+            v[i] += a.x; v[i + 1] += a.y; v[i + 2] += a.z; v[i + 3] += a.w;
+        }
+    }
+    __device__ __forceinline__ void scale(float s) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] *= s;
+    }
+    __device__ __forceinline__ void add_shfl_xor(int off) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], off);
+    }
+};
+
+// What spmm_kernel takes for a lane type: SpmmArgs, and for a row-scaled table (E4m3x16) one f32 scale per row of X as
+// well, indexed like X (after col_map).  Every entry of a row-scaled table takes the FMA path.
+struct SpmmArgsFp8 : SpmmArgs {
+    const float *x_scale;
+};
+template <class L> struct LaneArgs {
+    using type = SpmmArgs;
+    static constexpr bool kRowScaled = false;
+};
+template <> struct LaneArgs<E4m3x16> {
+    using type = SpmmArgsFp8;
+    static constexpr bool kRowScaled = true;
+};
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -571,7 +640,7 @@ __device__ __forceinline__ int32_t ld_stream_i32(const int32_t *p) {
 
 // One warp per chunk of <= chunk_nnz entries of one row.  Lane l owns columns
 //   f0 + (l + 32 t) * W .. + W   for t < NV   (W = L::kN: 4 for one 16-byte f32 vector, 1 for the scalar path,
-//                                              8 for one 16-byte load of bf16 rows)
+//                                              8 for one 16-byte load of bf16 rows, 16 of e4m3 codes)
 // so a warp reads each gathered row as NV fully coalesced 512-byte (16-byte lanes) requests.
 // Column ids of 32 entries are fetched with one coalesced load, mapped (col_map: sampled halo ->
 // slab row, -1 = skip), compacted through shared memory and then consumed UNROLL at a time so that
@@ -584,7 +653,8 @@ __device__ __forceinline__ int32_t ld_stream_i32(const int32_t *p) {
 // split into 32/G row groups of G lanes that walk different entries of the chunk concurrently (every lane
 // still issues 16-byte loads) and are summed with shuffles at the end.
 template <class L, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
-__global__ void __launch_bounds__(kThreads, L::min_blocks(NV, G, MAP && !CSCALE)) spmm_kernel(SpmmArgs a) {
+__global__ void __launch_bounds__(kThreads, L::min_blocks(NV, G, MAP && !CSCALE))
+    spmm_kernel(typename LaneArgs<L>::type a) {
     using T = typename L::T;
     constexpr int W = L::kN;
     constexpr int NG = 32 / G;                               // entries walked concurrently by one warp
@@ -638,6 +708,9 @@ __global__ void __launch_bounds__(kThreads, L::min_blocks(NV, G, MAP && !CSCALE)
                 }
                 if (MAP) {
                     if (col >= a.n_direct) col = __ldg(a.col_map + (col - a.n_direct));
+                }
+                if constexpr (LaneArgs<L>::kRowScaled) {
+                    if (col >= 0) sc *= __ldg(a.x_scale + col);
                 }
             }
             int cnt;
@@ -759,7 +832,7 @@ __global__ void __launch_bounds__(kThreads) spmm_fixup_kernel(SpmmArgs a) {
 }
 
 template <class L, int G, int NV, bool MAP, bool CSCALE, bool GUARD>
-int launch_spmm(SpmmArgs a, cudaStream_t st) {
+int launch_spmm(typename LaneArgs<L>::type a, cudaStream_t st) {
     static std::atomic<int> occ[kMaxDevices];            // per device, per instantiation
     const int dev = current_device();
     int blocks_per_sm = occ[dev].load(std::memory_order_relaxed);
@@ -789,19 +862,26 @@ int launch_spmm(SpmmArgs a, cudaStream_t st) {
 }
 
 template <class L, int G, int NV>
-int dispatch_flags(const SpmmArgs &a, cudaStream_t st) {
+int dispatch_flags(const typename LaneArgs<L>::type &a, cudaStream_t st) {
     const bool map = a.col_map != nullptr, cs = a.col_scale != nullptr || a.edge_weight != nullptr;
     const bool guard = (a.F % (G * L::kN * NV)) != 0;
-    if (guard) {
-        if (map && cs) return launch_spmm<L, G, NV, true, true, true>(a, st);
-        if (map) return launch_spmm<L, G, NV, true, false, true>(a, st);
-        if (cs) return launch_spmm<L, G, NV, false, true, true>(a, st);
-        return launch_spmm<L, G, NV, false, false, true>(a, st);
+    if constexpr (LaneArgs<L>::kRowScaled) {      // the row scale is a weight of every entry
+        if (guard && map) return launch_spmm<L, G, NV, true, true, true>(a, st);
+        if (guard) return launch_spmm<L, G, NV, false, true, true>(a, st);
+        if (map) return launch_spmm<L, G, NV, true, true, false>(a, st);
+        return launch_spmm<L, G, NV, false, true, false>(a, st);
+    } else {
+        if (guard) {
+            if (map && cs) return launch_spmm<L, G, NV, true, true, true>(a, st);
+            if (map) return launch_spmm<L, G, NV, true, false, true>(a, st);
+            if (cs) return launch_spmm<L, G, NV, false, true, true>(a, st);
+            return launch_spmm<L, G, NV, false, false, true>(a, st);
+        }
+        if (map && cs) return launch_spmm<L, G, NV, true, true, false>(a, st);
+        if (map) return launch_spmm<L, G, NV, true, false, false>(a, st);
+        if (cs) return launch_spmm<L, G, NV, false, true, false>(a, st);
+        return launch_spmm<L, G, NV, false, false, false>(a, st);
     }
-    if (map && cs) return launch_spmm<L, G, NV, true, true, false>(a, st);
-    if (map) return launch_spmm<L, G, NV, true, false, false>(a, st);
-    if (cs) return launch_spmm<L, G, NV, false, true, false>(a, st);
-    return launch_spmm<L, G, NV, false, false, false>(a, st);
 }
 
 inline int64_t ws_ld(int64_t F) { return (F + 3) / 4 * 4; }
@@ -818,7 +898,8 @@ int64_t l2_bytes() {
 }
 
 // Widest column slab (in elements: 256, 128, 64 or 32) whose source slab  x_rows * slab * elem_bytes  fits the L2
-// budget (elem_bytes: 4 for f32 tables, 2 for the bf16 tables of bns_spmm_sum_bf16).
+// budget (elem_bytes: 4 for f32 tables, 2 for the bf16 tables of bns_spmm_sum_bf16, 1 for the e4m3 codes of
+// bns_spmm_sum_fp8; their row scales are not counted).
 int pick_slab(int64_t F, int64_t x_rows, int32_t forced, int elem_bytes = 4) {
     if (forced == 256 || forced == 128 || forced == 64 || forced == 32) return forced;
     const char *env = getenv("BNS_SPMM_SLAB");
@@ -837,13 +918,33 @@ int pick_slab(int64_t F, int64_t x_rows, int32_t forced, int elem_bytes = 4) {
     return fmax;
 }
 
-int spmm_dispatch(const SpmmArgs &a, bool bf16, int64_t x_rows, int32_t slab_hint, cudaStream_t st) {
+enum class Elem { kF32, kBf16, kFp8 };
+
+// x_scale: the row scales of an fp8 table (Elem::kFp8), NULL otherwise
+int spmm_dispatch(const SpmmArgs &a, Elem elem, int64_t x_rows, int32_t slab_hint, cudaStream_t st,
+                  const float *x_scale = nullptr) {
     const int64_t F = a.F;
+    const bool bf16 = elem == Elem::kBf16;
     const bool vec = (F % 4 == 0) && (a.ldx % 4 == 0) && (a.ldy % 4 == 0) &&
                      ((reinterpret_cast<uintptr_t>(a.X) | reinterpret_cast<uintptr_t>(a.Y)) % 16 == 0);
     BNS_REQUIRE(vec || !bf16, "spmm: bf16 rows need the 16-byte layout (F %lld, ldx %lld, ldy %lld)", (long long)F,
                 (long long)a.ldx, (long long)a.ldy);
-    if (vec) {
+    if (elem == Elem::kFp8) {
+        BNS_REQUIRE(vec && F % 16 == 0 && a.ldx % 16 == 0 && (x_scale || a.X == nullptr),
+                    "spmm: fp8 rows need the 16-byte layout and their scales (F %lld, ldx %lld, ldy %lld)", (long long)F,
+                    (long long)a.ldx, (long long)a.ldy);
+        SpmmArgsFp8 f;
+        static_cast<SpmmArgs &>(f) = a;
+        f.x_scale = x_scale;
+        int slab = pick_slab(F, x_rows, slab_hint, 1);
+        while (slab > 32 && slab / 2 >= F) slab >>= 1;
+        switch (slab) {
+            case 256: dispatch_flags<E4m3x16, 16, 1>(f, st); break;
+            case 128: dispatch_flags<E4m3x16, 8, 1>(f, st); break;
+            case 64:  dispatch_flags<E4m3x16, 4, 1>(f, st); break;
+            default:  dispatch_flags<E4m3x16, 2, 1>(f, st); break;
+        }
+    } else if (vec) {
         int slab = pick_slab(F, x_rows, slab_hint, bf16 ? 2 : 4);
         while (slab > 32 && slab / 2 >= F) slab >>= 1;       // never wider than needed (F = 64 -> 64-wide groups)
         switch (slab) {
@@ -909,7 +1010,7 @@ extern "C" int bns_spmm_sum_f32(const bns_graph_t *g, const float *X, int64_t ld
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
     a.n_direct = (int32_t)n_direct;
-    return spmm_dispatch(a, false, x_rows, slab_hint, as_stream(stream));
+    return spmm_dispatch(a, Elem::kF32, x_rows, slab_hint, as_stream(stream));
 }
 
 // The same kernel over the per-epoch compacted indices of bns_graph_compact_cols: `cidx` already holds rows of X, the
@@ -931,7 +1032,7 @@ extern "C" int bns_spmm_compact_f32(const bns_graph_t *g, const int32_t *cidx, c
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.indices = cidx; a.chunk_cnt = chunk_cnt;
     a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    return spmm_dispatch(a, false, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    return spmm_dispatch(a, Elem::kF32, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
 }
 
 // Y[orow(r)] (+)= sum_k w_k X[c_k] with w_k = weights[(perm ? perm[k] : k) * ldw]: the weighted aggregation of GATConv
@@ -951,7 +1052,7 @@ extern "C" int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.edge_weight = weights; a.row_map = row_map;
     a.edge_perm = perm_from_transpose ? g->perm : nullptr; a.edge_ld = ldw;
-    return spmm_dispatch(a, false, x_rows > 0 ? x_rows : g->n_cols, 0, as_stream(stream));
+    return spmm_dispatch(a, Elem::kF32, x_rows > 0 ? x_rows : g->n_cols, 0, as_stream(stream));
 }
 
 // The same sums over a bf16 gather table (--agg-dtype bf16): X rows are bf16 (ldx in bf16 elements), widened exactly
@@ -976,7 +1077,7 @@ extern "C" int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X, int64_
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
     a.n_direct = (int32_t)n_direct;
-    return spmm_dispatch(a, true, x_rows, slab_hint, as_stream(stream));
+    return spmm_dispatch(a, Elem::kBf16, x_rows, slab_hint, as_stream(stream));
 }
 
 extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
@@ -995,7 +1096,60 @@ extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, 
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.indices = cidx; a.chunk_cnt = chunk_cnt;
     a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    return spmm_dispatch(a, true, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    return spmm_dispatch(a, Elem::kBf16, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+}
+
+// the 16-byte gathers of the fp8 lanes (16 codes each) and their 16-byte f32 stores
+#define BNS_FP8_LAYOUT(fn)                                                                                             \
+    BNS_REQUIRE(F % 16 == 0 && ldx % 16 == 0 && ldy % 4 == 0 &&                                                        \
+                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
+                fn ": needs F %% 16 == 0, ldx %% 16 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "  \
+                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
+
+// The same sums over an fp8 gather table (--agg-dtype fp8): X rows are e4m3 codes (ldx in bytes) and x_scale holds one
+// f32 scale per row of X.  Entry k adds  w_k * x_scale[xrow(c_k)] * widen(X[xrow(c_k)])  in f32, w_k = col_scale[c_k]
+// (times the per-entry weight) or 1; Y, the weights and the workspace are f32 as above.
+extern "C" int bns_spmm_sum_fp8(const bns_graph_t *g, const uint8_t *X, const float *x_scale, int64_t ldx, int64_t F,
+                                float *Y, int64_t ldy, const float *row_scale, const float *col_scale,
+                                const float *edge_weight, const int32_t *row_map, const int32_t *col_map, int64_t n_direct,
+                                int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes,
+                                void *stream) {
+    BNS_REQUIRE(g, "bns_spmm_sum_fp8: NULL graph");
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_sum_fp8: bad feature width %lld", (long long)F);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(Y, "bns_spmm_sum_fp8: NULL output matrix");
+    BNS_REQUIRE((X && x_scale) || g->nnz == 0, "bns_spmm_sum_fp8: NULL input matrix or scales");
+    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_sum_fp8: leading dimension smaller than F");
+    BNS_FP8_LAYOUT("bns_spmm_sum_fp8");
+    const size_t need = bns_spmm_workspace_bytes(g, F);
+    if (need > 0 && (ws == nullptr || ws_bytes < need))
+        return fail(BNS_E_WORKSPACE, "bns_spmm_sum_fp8: workspace %zu bytes < %zu needed", ws_bytes, need);
+    if (col_map == nullptr) n_direct = g->n_cols;
+    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_fp8: n_direct out of range");
+    if (x_rows <= 0) x_rows = g->n_cols;
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
+    a.n_direct = (int32_t)n_direct;
+    return spmm_dispatch(a, Elem::kFp8, x_rows, slab_hint, as_stream(stream), x_scale);
+}
+
+extern "C" int bns_spmm_compact_fp8(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
+                                    const int32_t *chunk_cnt, const uint8_t *X, const float *x_scale, int64_t ldx, int64_t F,
+                                    float *Y, int64_t ldy, const float *row_scale, int64_t x_rows, int32_t slab_hint,
+                                    int accumulate, void *ws, size_t ws_bytes, void *stream) {
+    BNS_REQUIRE(g && cidx && chunk_cnt, "bns_spmm_compact_fp8: NULL argument");
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_compact_fp8: bad feature width %lld", (long long)F);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(Y && ((X && x_scale) || g->nnz == 0), "bns_spmm_compact_fp8: NULL matrix");
+    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_compact_fp8: leading dimension smaller than F");
+    BNS_FP8_LAYOUT("bns_spmm_compact_fp8");
+    const size_t need = bns_spmm_workspace_bytes(g, F);
+    if (need > 0 && (ws == nullptr || ws_bytes < need))
+        return fail(BNS_E_WORKSPACE, "bns_spmm_compact_fp8: workspace %zu bytes < %zu needed", ws_bytes, need);
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.indices = cidx; a.chunk_cnt = chunk_cnt;
+    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
+    return spmm_dispatch(a, Elem::kFp8, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream), x_scale);
 }
 
 namespace {
@@ -1029,6 +1183,73 @@ extern "C" int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *ds
     const int64_t want = (work + kThreads - 1) / kThreads;
     cvt_rows_bf16_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, dst, ldd,
                                                                                                    n_rows, F, vec);
+    g_launches += 1;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+namespace {
+
+// One warp per row, 8 columns per lane and step.  m = max |x| of the row; the scale is 2^e with e the smallest integer
+// such that m * 2^-e <= 448 (the largest finite e4m3), e >= -126; 1 for a row of zeros; NaN for a row holding NaN or
+// +-Inf, whose codes are 0.  Codes: x * 2^-e (exact: a power of two, never above 448) rounded to nearest even e4m3.
+__global__ void __launch_bounds__(kThreads) cvt_rows_fp8_kernel(const float *__restrict__ src, int64_t lds,
+                                                                uint8_t *__restrict__ codes, int64_t ldc,
+                                                                float *__restrict__ scale, int64_t n_rows, int F) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * kWarps;
+    for (int64_t r = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); r < n_rows; r += warps) {
+        const float *x = src + r * lds;
+        uint32_t m = 0;                         // bits of max |x|: NaN > Inf > every finite value
+        for (int c = lane * 8; c < F; c += 256) {
+            const float4 a = __ldg(reinterpret_cast<const float4 *>(x + c)), b = __ldg(reinterpret_cast<const float4 *>(x + c + 4));
+            const float e[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int i = 0; i < 8; ++i) m = max(m, __float_as_uint(e[i]) & 0x7fffffffu);
+        }
+        m = __reduce_max_sync(0xffffffffu, m);
+        const bool bad = m >= 0x7f800000u;
+        int ex = 0;
+        if (m >= 0x00800000u) {                 // normal: m = 1.M * 2^(E-127); 1.M <= 1.75 leaves one more doubling
+            const int E = (int)(m >> 23);
+            ex = E - 135 + ((m & 0x7fffffu) > 0x600000u ? 1 : 0);
+            if (ex < -126) ex = -126;
+        } else if (m != 0) {
+            ex = -126;
+        }
+        const float inv = __uint_as_float((uint32_t)(127 - ex) << 23);
+        if (lane == 0) scale[r] = bad ? __uint_as_float(0x7fc00000u) : __uint_as_float((uint32_t)(127 + ex) << 23);
+        uint8_t *q = codes + r * ldc;
+        for (int c = lane * 8; c < F; c += 256) {
+            uint2 o = make_uint2(0u, 0u);
+            if (!bad) {
+                const float4 a = __ldg(reinterpret_cast<const float4 *>(x + c)), b = __ldg(reinterpret_cast<const float4 *>(x + c + 4));
+                const uint32_t q0 = __nv_cvt_float2_to_fp8x2(make_float2(a.x * inv, a.y * inv), __NV_SATFINITE, __NV_E4M3);
+                const uint32_t q1 = __nv_cvt_float2_to_fp8x2(make_float2(a.z * inv, a.w * inv), __NV_SATFINITE, __NV_E4M3);
+                const uint32_t q2 = __nv_cvt_float2_to_fp8x2(make_float2(b.x * inv, b.y * inv), __NV_SATFINITE, __NV_E4M3);
+                const uint32_t q3 = __nv_cvt_float2_to_fp8x2(make_float2(b.z * inv, b.w * inv), __NV_SATFINITE, __NV_E4M3);
+                o = make_uint2(q0 | (q1 << 16), q2 | (q3 << 16));
+            }
+            *reinterpret_cast<uint2 *>(q + c) = o;
+        }
+    }
+}
+
+}  // namespace
+
+extern "C" int bns_cvt_rows_f32_fp8(const float *src, int64_t lds, uint8_t *codes, int64_t ldc, float *scale,
+                                    int64_t n_rows, int64_t F, void *stream) {
+    BNS_REQUIRE(n_rows >= 0 && F >= 0 && F < (1 << 24) && lds >= F && ldc >= F, "bns_cvt_rows_f32_fp8: bad shape");
+    if (n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(src && codes && scale, "bns_cvt_rows_f32_fp8: NULL matrix");
+    BNS_REQUIRE(F % 16 == 0 && ldc % 16 == 0 && lds % 4 == 0 &&
+                    ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(codes)) % 16) == 0,
+                "bns_cvt_rows_f32_fp8: needs F %% 16 == 0, ldc %% 16 == 0, lds %% 4 == 0 and 16-byte aligned src, codes "
+                "(F %lld, lds %lld, ldc %lld)", (long long)F, (long long)lds, (long long)ldc);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const int64_t want = (n_rows + kWarps - 1) / kWarps;
+    cvt_rows_fp8_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, codes, ldc,
+                                                                                                  scale, n_rows, (int)F);
     g_launches += 1;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

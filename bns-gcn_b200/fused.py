@@ -353,17 +353,25 @@ class PPLinearFn(torch.autograd.Function):
         return dx, None, None, None, None, None
 
 
-def _gather_table(x: torch.Tensor, bf16: bool) -> torch.Tensor:
-    """What an aggregation pass gathers: ``x`` itself, or (``--agg-dtype bf16``) its rows rounded to bf16."""
-    return ops.cvt_rows_bf16(x) if bf16 else x
+def _agg_mode(g: PartitionGraph):
+    """The table mode ``_gather_table`` takes for ``g``'s wide passes: ``False`` (f32), ``True`` (bf16) or ``'fp8'``."""
+    return 'fp8' if g.agg_fp8 else g.agg_bf16
+
+
+def _gather_table(x: torch.Tensor, mode):
+    """What an aggregation pass gathers: ``x`` itself (``mode`` false), its rows rounded to bf16 (``True``,
+    ``--agg-dtype bf16``) or an fp8 table of them (``'fp8'``, ``--agg-dtype fp8``: e4m3 codes, a scale per row)."""
+    if mode == 'fp8':
+        return ops.cvt_rows_fp8(x)
+    return ops.cvt_rows_bf16(x) if mode else x
 
 
 def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf16: bool = False,
                halo: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``rs * (A_in x_u[:n_in] + A_out[:, sampled] x_u[n_in:])`` -- the inner pass first (it needs local rows only), the
-    halo pass after the exchange's event.  ``bf16``: both passes gather bf16 copies of the rows (f32 sums).  ``halo``:
+    halo pass after the exchange's event.  ``bf16``: the ``_gather_table`` mode of both passes (f32 sums).  ``halo``:
     the halo rows as they arrived in bf16 (``--comm-dtype bf16``; ``x_u`` is then the inner rows alone), gathered as
-    they are."""
+    they are, whatever the mode."""
     y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16), row_scale=rs)
     if ready is not None:
         torch.cuda.current_stream(x_u.device).wait_event(ready)
@@ -400,8 +408,8 @@ def _aggregate_t(g: PartitionGraph, dys: torch.Tensor, n_u: int, cs_in=None, cs_
                  bf16: bool = False) -> torch.Tensor:
     """``cs * (A^T dys)`` over the epoch's graph: ``[n_u, F]`` (inner rows, then the sampled halo rows); ``cs``: GCN's
     per-source scale (1/sqrt(out_deg)), applied as the row scale of the transposed products.  The halo rows come first;
-    ``after_halo(du)`` is called as soon as they are final (the gradient return trip starts there).  ``bf16``: both
-    passes gather one bf16 copy of ``dys``."""
+    ``after_halo(du)`` is called as soon as they are final (the gradient return trip starts there).  ``bf16``: the
+    ``_gather_table`` mode; both passes gather one table of ``dys``."""
     du = torch.empty(n_u, dys.shape[1], dtype=torch.float32, device=dys.device)
     dys = _gather_table(dys, bf16)
     if n_u > g.n_in:
@@ -453,7 +461,7 @@ class SageConvFn(torch.autograd.Function):
                 halo_aggregate(g, t[n_in:], out, rs, None)                      # ... + (A_out t_halo) / deg
             ctx.save_for_backward(*((h_u,) if halo is None else (h_in, h_halo)))
         else:
-            ah = _aggregate(g, h_u, rs, ready, g.agg_bf16, halo)                # [n_in, in]
+            ah = _aggregate(g, h_u, rs, ready, _agg_mode(g), halo)              # [n_in, in]
             t = dense.tc_mm_tn(ah, W2, arena.padded(b2), bf16=bf)
             out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t, bf16=bf)
             ctx.save_for_backward(h_u, ah)
@@ -490,7 +498,7 @@ class SageConvFn(torch.autograd.Function):
         else:
             h_u, ah = ctx.saved_tensors
             dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs, bf16=bf)  # (dout W2) / deg
-            du = _aggregate_t(g, dys, ctx.n_u, after_halo=begin, bf16=g.agg_bf16)
+            du = _aggregate_t(g, dys, ctx.n_u, after_halo=begin, bf16=_agg_mode(g))
             dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1), bf16=bf)
             dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2), bf16=bf)
         inner = du[:n_in]
@@ -533,7 +541,7 @@ class GcnConvFn(torch.autograd.Function):
             out = scale_rows(s, rs, bias=bp)                                                          # / in_norm + b
             ctx.save_for_backward(*((h_u,) if halo is None else (h_u[:n_in], h_halo)))
         else:
-            bf16 = g.agg_bf16
+            bf16 = _agg_mode(g)
             y = ops.spmm_auto(g.a_in, _gather_table(scale_rows(h_u[:n_in], cs_in), bf16), row_scale=rs)
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
@@ -568,7 +576,7 @@ class GcnConvFn(torch.autograd.Function):
             (y,) = ctx.saved_tensors
             dense.tc_mm_nt(dout, y, out=a.grad_padded(w), bf16=bf)
             dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs, bf16=bf)  # (dout W) / in_norm
-            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, after_halo=begin, bf16=g.agg_bf16)
+            du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, after_halo=begin, bf16=_agg_mode(g))
         return du[:g.n_in] if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None
 
 

@@ -31,8 +31,10 @@ class PartitionGraph:
         self.compact: Optional[ops.CompactedCols] = None
         self.halo_col_scale: Optional[torch.Tensor] = None      # GCN: 1/sqrt(out_deg) of the halo nodes (static)
         self.want_positions = False                             # GAT: the compaction also records CSR positions
-        # --agg-dtype bf16: the fused layers' wide aggregation passes gather bf16 copies of their source rows
+        # --agg-dtype bf16 / fp8: the fused layers' wide aggregation passes gather bf16 copies, or fp8 tables
+        # (ops.Fp8Rows), of their source rows (fused._gather_table); at most one of the two is set
         self.agg_bf16 = False
+        self.agg_fp8 = False
 
     def refresh_compaction(self) -> None:
         """Call after every change of ``slot`` (train.construct_graph does)."""

@@ -65,12 +65,14 @@ def build_parser():
                         help="NEW: with --eval, every rank evaluates its own nodes on its partition (the whole halo "
                              "exchanged layer by layer) instead of rank 0 evaluating the full graph alone; the full "
                              "graph is never built.  Transductive runs only")
-    parser.add_argument(*_spellings("agg-dtype"), default="f32", choices=["f32", "bf16"],
+    parser.add_argument(*_spellings("agg-dtype"), default="f32", choices=["f32", "bf16", "fp8"],
                         help="NEW: element type of the rows the wide (hidden-width) aggregation passes gather.  bf16 "
                              "rounds them to bf16 (nearest even) before each pass -- h_u forward, the transposed "
                              "passes' input gradient backward -- and sums in f32: half the gathered bytes, and results "
-                             "that no longer match the reference to 1e-4.  Only with the fused training step "
-                             "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+                             "that no longer match the reference to 1e-4.  fp8 stores the same rows as e4m3 (nearest "
+                             "even) with one power-of-two scale per row: a quarter of the f32 bytes; hidden widths "
+                             "must be multiples of 16.  Only with the fused training step (GraphSAGE / GCN, --use-pp, "
+                             "--norm layer, no --n-linear)")
     parser.add_argument(*_spellings("comm-dtype"), default="f32", choices=["f32", "bf16"],
                         help="NEW: element type of the boundary rows the training exchange moves.  bf16 rounds each "
                              "sampled row H[selected]/ratio, and each returned halo gradient row, to bf16 (nearest even) "

@@ -121,19 +121,69 @@ class DeviceGraph:
                 pass
 
 
+class Fp8Rows:
+    """An fp8 gather table (``--agg-dtype fp8``, ``cvt_rows_fp8``): e4m3 ``codes`` ``[rows, F]`` (``float8_e4m3fn``, row
+    stride a multiple of 16 bytes) and one power-of-two f32 ``scale`` per row; row ``r`` stands for
+    ``codes[r].float() * scale[r]``.  Slicing takes rows."""
+
+    __slots__ = ("codes", "scale")
+
+    def __init__(self, codes: torch.Tensor, scale: torch.Tensor):
+        self.codes, self.scale = codes, scale
+
+    @property
+    def shape(self):
+        return self.codes.shape
+
+    @property
+    def device(self):
+        return self.codes.device
+
+    def element_size(self) -> int:
+        return 1
+
+    def __getitem__(self, rows: slice) -> "Fp8Rows":
+        return Fp8Rows(self.codes[rows], self.scale[rows])
+
+    def dequantize(self) -> torch.Tensor:
+        """The f32 rows the SpMM sums (for tests and diagnostics)."""
+        return self.codes.float() * self.scale.unsqueeze(1)
+
+
+def _table(x, name: str = "x"):
+    """``(kind, data pointer, row stride, scale pointer)`` of a gather table: f32, bf16 or ``Fp8Rows``."""
+    if isinstance(x, Fp8Rows):
+        c = x.codes
+        _req(c, torch.float8_e4m3fn, name + ".codes")
+        _req(x.scale, torch.float32, name + ".scale")
+        if c.dim() != 2 or c.stride(1) != 1 or x.scale.dim() != 1 or x.scale.shape[0] != c.shape[0] or \
+                x.scale.stride(0) != 1:
+            raise _lib.BnsError(f"{name}: codes must be a row-major 2-D tensor with one contiguous scale per row")
+        return "fp8", c.data_ptr(), c.stride(0), x.scale.data_ptr()
+    if x.dtype == torch.bfloat16:
+        if not x.is_cuda:
+            raise _lib.BnsError(f"{name} must be a CUDA tensor (there is no CPU path)")
+        kind = "bf16"
+    else:
+        _req(x, torch.float32, name)
+        kind = "f32"
+    if x.dim() != 2 or x.stride(1) != 1:
+        raise _lib.BnsError(f"{name} must be a row-major 2-D tensor")
+    return kind, x.data_ptr(), x.stride(0), None
+
+
+def _table_bytes(x, F: int) -> int:
+    return x.element_size() * F * x.shape[0] + (4 * x.shape[0] if isinstance(x, Fp8Rows) else 0)
+
+
 def spmm(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *, n_out_rows: Optional[int] = None,
          row_scale: Optional[torch.Tensor] = None, col_scale: Optional[torch.Tensor] = None,
          row_map: Optional[torch.Tensor] = None, col_map: Optional[torch.Tensor] = None, n_direct: int = 0,
          accumulate: bool = False, slab: int = 0, edge_weight: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``bns_spmm_sum_f32``: ``out[orow(r)] (+)= row_scale[r] * sum_k col_scale[c_k] * x[xrow(c_k)]``.  A bf16 ``x``
-    (``cvt_rows_bf16``) takes ``bns_spmm_sum_bf16``: the same sum, accumulated and written in f32."""
-    bf16 = x.dtype == torch.bfloat16
-    if not bf16:
-        _req(x, torch.float32, "x")
-    elif not x.is_cuda:
-        raise _lib.BnsError("x must be a CUDA tensor (there is no CPU path)")
-    if x.dim() != 2 or x.stride(1) != 1:
-        raise _lib.BnsError("x must be a row-major 2-D tensor")
+    (``cvt_rows_bf16``) takes ``bns_spmm_sum_bf16``, an ``Fp8Rows`` ``x`` (``cvt_rows_fp8``) ``bns_spmm_sum_fp8``: the
+    same sum, accumulated and written in f32."""
+    kind, xp, ldx, xs = _table(x)
     F = x.shape[1]
     if out is None:
         if accumulate:
@@ -152,16 +202,17 @@ def spmm(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = None, *,
     if prof is not None:
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(torch.cuda.current_stream(x.device))
-    fn, name = (lib.bns_spmm_sum_bf16, "bns_spmm_sum_bf16") if bf16 else (lib.bns_spmm_sum_f32, "bns_spmm_sum_f32")
+    name = "bns_spmm_sum_" + kind
+    xargs = (xp, xs, ldx) if kind == "fp8" else (xp, ldx)
     with torch.cuda.device(x.device):
-        check(fn(g._h, x.data_ptr(), x.stride(0), F, out.data_ptr(), out.stride(0),
-                 _ptr(row_scale), _ptr(col_scale), _ptr(edge_weight), _ptr(row_map), _ptr(col_map),
-                 n_direct, x.shape[0], slab, 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()),
-              name)
+        check(getattr(lib, name)(g._h, *xargs, F, out.data_ptr(), out.stride(0),
+                                 _ptr(row_scale), _ptr(col_scale), _ptr(edge_weight), _ptr(row_map), _ptr(col_map),
+                                 n_direct, x.shape[0], slab, 1 if accumulate else 0, _ptr(ws),
+                                 0 if ws is None else ws.numel(), _stream_ptr()), name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(x.device))
         # SURVEY.md §8(d): every distinct operand byte once -- row offsets, column ids, source rows, output rows
-        alg = 8 * (g.n_rows + 1) + 4 * g.nnz + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
+        alg = 8 * (g.n_rows + 1) + 4 * g.nnz + _table_bytes(x, F) + 4 * F * out.shape[0]
         # entries whose source row is really gathered: all of them, or (sampled halo) the mapped fraction
         live = g.nnz
         if col_map is not None and g.n_cols > n_direct:
@@ -183,7 +234,8 @@ BLOCK_MAX = 4
 
 
 def plan_col_blocks(g: DeviceGraph, F: int, elem_bytes: int = 4) -> int:
-    """Number of source-row blocks for width ``F`` (1 = no blocking); ``elem_bytes``: 4 for an f32 table, 2 for bf16."""
+    """Number of source-row blocks for width ``F`` (1 = no blocking); ``elem_bytes``: 4 for an f32 table, 2 for bf16,
+    1 for fp8 (its row scales are not counted)."""
     import os
     forced = os.environ.get("BNS_SPMM_COLBLOCKS")
     if forced:
@@ -233,7 +285,7 @@ def spmm_auto(g: DeviceGraph, x: torch.Tensor, out: Optional[torch.Tensor] = Non
                  col_scale=None if col_scale is None else col_scale[c0:c1])
         if prof is not None:
             ev1.record(torch.cuda.current_stream(x.device))
-            alg = 8 * (g.n_rows + 1) + 4 * g.nnz + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
+            alg = 8 * (g.n_rows + 1) + 4 * g.nnz + _table_bytes(x, F) + 4 * F * out.shape[0]
             prof.append((ev0, ev1, alg, g.nnz, F, g.nnz))
     finally:
         PROFILE = prof
@@ -268,13 +320,11 @@ def spmm_compact(c: CompactedCols, x: torch.Tensor, out: torch.Tensor, *, row_sc
                  weights: Optional[torch.Tensor] = None, head: int = 0) -> torch.Tensor:
     """``bns_spmm_compact_f32``: the SpMM over the compacted (sampled) entries only.  ``weights`` ``[nnz, heads]`` at
     the COMPACTED positions (GAT's dropped attention, column ``head``) replaces the compaction's own per-entry weights.
-    A bf16 ``x`` takes ``bns_spmm_compact_bf16``."""
+    A bf16 ``x`` takes ``bns_spmm_compact_bf16``, an ``Fp8Rows`` ``x`` ``bns_spmm_compact_fp8``."""
     g = c.g
-    bf16 = x.dtype == torch.bfloat16
-    if not bf16:
-        _req(x, torch.float32, "x")
+    kind, xp, ldx, xs = _table(x)
     _req(out, torch.float32, "out")
-    if x.dim() != 2 or x.stride(1) != 1 or out.stride(1) != 1 or out.shape[1] != x.shape[1]:
+    if out.stride(1) != 1 or out.shape[1] != x.shape[1]:
         raise _lib.BnsError("x / out must be row-major [*, F]")
     F = x.shape[1]
     ws = g.workspace(F)
@@ -284,16 +334,16 @@ def spmm_compact(c: CompactedCols, x: torch.Tensor, out: torch.Tensor, *, row_sc
         ev0.record(torch.cuda.current_stream(x.device))
     with torch.cuda.device(x.device):
         cw_ptr, cw_ld = (_ptr(c.cw), 1) if weights is None else (weights.data_ptr() + 4 * head, weights.stride(0))
-        fn, name = ((lib.bns_spmm_compact_bf16, "bns_spmm_compact_bf16") if bf16 else
-                    (lib.bns_spmm_compact_f32, "bns_spmm_compact_f32"))
-        check(fn(g._h, c.cidx.data_ptr(), cw_ptr, cw_ld, c.chunk_cnt.data_ptr(), x.data_ptr(), x.stride(0),
-                 F, out.data_ptr(), out.stride(0), _ptr(row_scale), x.shape[0], slab,
-                 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()), name)
+        name = "bns_spmm_compact_" + kind
+        xargs = (xp, xs, ldx) if kind == "fp8" else (xp, ldx)
+        check(getattr(lib, name)(g._h, c.cidx.data_ptr(), cw_ptr, cw_ld, c.chunk_cnt.data_ptr(), *xargs,
+                                 F, out.data_ptr(), out.stride(0), _ptr(row_scale), x.shape[0], slab,
+                                 1 if accumulate else 0, _ptr(ws), 0 if ws is None else ws.numel(), _stream_ptr()), name)
     if prof is not None:
         ev1.record(torch.cuda.current_stream(x.device))
         live = int(g.nnz * min(1.0, x.shape[0] / max(g.n_cols, 1))) if live_nnz is None else live_nnz
         # algorithmic bytes of the SAMPLED product: its live entries, the rows of X it can reference, the output rows
-        alg = 8 * (g.n_rows + 1) + 4 * live + x.element_size() * F * x.shape[0] + 4 * F * out.shape[0]
+        alg = 8 * (g.n_rows + 1) + 4 * live + _table_bytes(x, F) + 4 * F * out.shape[0]
         prof.append((ev0, ev1, alg, live, F, live))
     return out
 
@@ -406,6 +456,27 @@ def cvt_rows_bf16(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torc
     with torch.cuda.device(src.device):
         check(lib.bns_cvt_rows_f32_bf16(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0), n, F, _stream_ptr()),
               "bns_cvt_rows_f32_bf16")
+    return out
+
+
+def cvt_rows_fp8(src: torch.Tensor, out: Optional[Fp8Rows] = None) -> Fp8Rows:
+    """``bns_cvt_rows_f32_fp8``: ``src`` as an fp8 table, into ``out`` or a new ``Fp8Rows`` whose code rows are 16-byte
+    aligned.  Per row: scale ``2^e`` with ``e`` the smallest integer >= -126 such that ``max|x| * 2^-e <= 448`` (1 for
+    a row of zeros), codes ``x * 2^-e`` rounded to nearest even e4m3; a row holding NaN or +-Inf gets scale NaN and
+    zero codes.  ``F`` must be a multiple of 16."""
+    _req(src, torch.float32, "src")
+    if src.dim() != 2 or src.stride(1) != 1:
+        raise _lib.BnsError("src must be a row-major 2-D tensor")
+    n, F = src.shape
+    if out is None:
+        out = Fp8Rows(torch.empty(n, (F + 15) // 16 * 16, dtype=torch.float8_e4m3fn, device=src.device)[:, :F],
+                      torch.empty(n, dtype=torch.float32, device=src.device))
+    _table(out, "out")
+    if out.shape != src.shape:
+        raise _lib.BnsError("out must have the shape of src")
+    with torch.cuda.device(src.device):
+        check(lib.bns_cvt_rows_f32_fp8(src.data_ptr(), src.stride(0), out.codes.data_ptr(), out.codes.stride(0),
+                                       out.scale.data_ptr(), n, F, _stream_ptr()), "bns_cvt_rows_f32_fp8")
     return out
 
 

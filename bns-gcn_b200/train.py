@@ -375,6 +375,12 @@ def _hidden_x8(args, layer_size):
     return None
 
 
+def _hidden_x16(args, layer_size):
+    if any(w % 16 for w in layer_size[1:-1]):
+        return f"hidden width {args.n_hidden} is not a multiple of 16 (fp8 rows are gathered 16 at a time)"
+    return None
+
+
 def _exchanged_x8(args, layer_size):
     bad = sorted({w for w in layer_size[1:-1] if w % 8})
     if bad:
@@ -382,34 +388,36 @@ def _exchanged_x8(args, layer_size):
     return None
 
 
-# --<flag>-dtype: the width rule its bf16 mode adds to the fused step's (a function returning the broken rule's message
-# or None; None in place of the function: nothing more), and what the check
-# returns for f32 and for bf16
+# --<flag>-dtype: what the check returns for f32, and for each narrower mode the width rule it adds to the fused step's
+# (a function returning the broken rule's message or None; None in place of the function: nothing more) and what the
+# check returns for it
 _DTYPE_FLAGS = {
-    'agg': (_hidden_x8, False, True),
-    'comm': (_exchanged_x8, 'f32', 'bf16'),
-    'dense': (None, False, True),
+    'agg': (False, {'bf16': (_hidden_x8, True), 'fp8': (_hidden_x16, 'fp8')}),
+    'comm': ('f32', {'bf16': (_exchanged_x8, 'bf16')}),
+    'dense': (False, {'bf16': (None, True)}),
 }
 
 
 def _check_dtype_flag(flag, args, layer_size, dev):
-    """The bf16 modes only exist on the fused training step: any configuration that step does not take raises
+    """The bf16 / fp8 modes only exist on the fused training step: any configuration that step does not take raises
     ``ValueError`` naming every reason, rather than training in f32 behind the user's back."""
-    width_rule, off, on = _DTYPE_FLAGS[flag]
+    off, modes = _DTYPE_FLAGS[flag]
     mode = getattr(args, f'{flag}_dtype', 'f32')
     if mode == 'f32':
         return off
-    if mode != 'bf16':
-        raise ValueError(f"--{flag}-dtype {mode!r}: expected 'f32' or 'bf16'")
+    if mode not in modes:
+        raise ValueError(f"--{flag}-dtype {mode!r}: expected " + " or ".join(repr(m) for m in ['f32', *modes]))
+    width_rule, on = modes[mode]
     why = _fused_step_refusals(args, layer_size, dev, width_rule(args, layer_size) if width_rule else None)
     if why:
-        raise ValueError(f"--{flag}-dtype bf16 needs the fused training step, which this run does not take: "
+        raise ValueError(f"--{flag}-dtype {mode} needs the fused training step, which this run does not take: "
                          + "; ".join(why))
     return on
 
 
-def check_agg_dtype(args, layer_size, dev) -> bool:
-    """Whether ``--agg-dtype bf16`` is on: the aggregation gathers from bf16 tables, with f32 sums."""
+def check_agg_dtype(args, layer_size, dev):
+    """``False`` for f32, ``True`` for ``--agg-dtype bf16`` (the aggregation gathers from bf16 tables) and ``'fp8'``
+    for ``--agg-dtype fp8`` (e4m3 tables with a power-of-two scale per row); the sums are f32 in every mode."""
     return _check_dtype_flag('agg', args, layer_size, dev)
 
 
@@ -435,7 +443,8 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     part.want_positions = args.model == 'gat'          # the fused attention keeps per-entry values at CSR positions
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
-    part.agg_bf16 = check_agg_dtype(args, layer_size, dev)
+    agg = check_agg_dtype(args, layer_size, dev)
+    part.agg_bf16, part.agg_fp8 = agg is True, agg == 'fp8'
     comm_dtype = check_comm_dtype(args, layer_size, dev)
     dense_bf16 = check_dense_dtype(args, layer_size, dev)
     _, _, _, node_dict, boundary = move_to_cuda(graph, in_graph, out_graph, node_dict, boundary, dev)

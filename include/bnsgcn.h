@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 6
+#define BNS_ABI_VERSION 7
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -328,6 +328,30 @@ int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float
                           int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes, void *stream);
 int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *dst /*bf16*/, int64_t ldd, int64_t n_rows, int64_t F,
                           void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 7: FP8 gather tables (--agg-dtype fp8).  A table is e4m3 codes X [rows, F] (ldx in bytes) plus one f32 power-of-two
+ * scale per row, x_scale [rows]; row r stands for x_scale[r] * e4m3(X[r, :]).  bns_spmm_sum_fp8 / bns_spmm_compact_fp8
+ * are bns_spmm_sum_f32 / bns_spmm_compact_f32 over such a table: entry k adds w_k * x_scale[xrow(c_k)] * X[xrow(c_k)]
+ * (codes widened exactly, f32 FMA, same entry order), where w_k is the f32 column scale / per-entry weight (or 1) and the
+ * scale is indexed by the row of X the entry gathers (after col_map / compaction).  X is read as 16-byte vectors of 16
+ * codes: F % 16 == 0, ldx % 16 == 0, ldy % 4 == 0 and 16-byte aligned X, Y, else BNS_E_INVALID.  The column slab is
+ * sized from x_rows * slab * 1 byte; the workspace is the f32 one (bns_spmm_workspace_bytes).
+ * bns_cvt_rows_f32_fp8: with m = max |src[r, :F]|, scale[r] = 2^e for the smallest integer e >= -126 with
+ * m * 2^-e <= 448 (1 when m == 0), codes[r, c] = e4m3(src[r, c] * 2^-e) rounded to nearest even (the product is exact
+ * and never saturates; subnormal codes are kept).  A row holding NaN or +-Inf gets scale NaN and all-zero codes, so
+ * every sum that gathers it is NaN.  Needs F % 16 == 0, ldc % 16 == 0, lds % 4 == 0 and 16-byte aligned src, codes.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_spmm_sum_fp8(const bns_graph_t *g, const uint8_t *X /*e4m3*/, const float *x_scale, int64_t ldx, int64_t F,
+                     float *Y, int64_t ldy, const float *row_scale, const float *col_scale, const float *edge_weight,
+                     const int32_t *row_map, const int32_t *col_map, int64_t n_direct, int64_t x_rows, int32_t slab_hint,
+                     int accumulate, void *ws, size_t ws_bytes, void *stream);
+int bns_spmm_compact_fp8(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld, const int32_t *chunk_cnt,
+                         const uint8_t *X /*e4m3*/, const float *x_scale, int64_t ldx, int64_t F, float *Y, int64_t ldy,
+                         const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws,
+                         size_t ws_bytes, void *stream);
+int bns_cvt_rows_f32_fp8(const float *src, int64_t lds, uint8_t *codes /*e4m3*/, int64_t ldc, float *scale, int64_t n_rows,
+                         int64_t F, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * K10 fused: the attention of dgl.nn.GATConv (module/model.py:96-132; DGL 0.9 python/dgl/nn/pytorch/conv/gatconv.py):
