@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -171,6 +171,16 @@ SIGNATURES = {
     "bns_spmm_compact_fp8": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int64,
                                      c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int, c_void_p, c_size_t, c_void_p]),
     "bns_cvt_rows_f32_fp8": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p]),
+    # ---- ABI 8 ----
+    "bns_p2p_put_all_fp8": (c_int, [c_void_p, POINTER(PutAll), POINTER(c_uint64), c_int64, c_void_p, c_int64, c_int64,
+                                    c_void_p, c_int32, c_int32, c_uint64, c_void_p, c_void_p]),
+    "bns_scatter_rows_all_fp8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int32, POINTER(c_void_p),
+                                         POINTER(c_void_p), POINTER(c_void_p), c_int64, POINTER(c_float), c_void_p]),
+    "bns_gather_div_fp8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float, c_void_p, c_int64, c_void_p,
+                                   c_void_p]),
+    "bns_scatter_add_div_fp8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float, c_void_p, c_int64,
+                                        c_void_p, c_void_p]),
+    "bns_cvt_rows_fp8_f32": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
 }
 
 

@@ -610,6 +610,25 @@ struct E4m3x16 {
 #pragma unroll
         for (int i = 0; i < 16; ++i) v[i] += __shfl_xor_sync(0xffffffffu, v[i], off);
     }
+    // the exchange's scatters (--comm-dtype fp8): load f32 sums, then v += (code * scale) / div per element.  The
+    // product is exact in f32 (subnormals included), so this adds what the f32 lanes' add_div adds for the widened row.
+    __device__ __forceinline__ void load(const float *p) {
+#pragma unroll
+        for (int i = 0; i < 16; i += 4) {
+            const float4 a = *reinterpret_cast<const float4 *>(p + i);
+            v[i] = a.x; v[i + 1] = a.y; v[i + 2] = a.z; v[i + 3] = a.w;
+        }
+    }
+    __device__ __forceinline__ void add_div(const uint8_t *r, float scale, float div) {
+        const uint4 u = *reinterpret_cast<const uint4 *>(r);
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float2 a = e4m3x2_f32(w[i] & 0xffffu), b = e4m3x2_f32(w[i] >> 16);
+            v[4 * i] += __fdiv_rn(a.x * scale, div); v[4 * i + 1] += __fdiv_rn(a.y * scale, div);
+            v[4 * i + 2] += __fdiv_rn(b.x * scale, div); v[4 * i + 3] += __fdiv_rn(b.y * scale, div);
+        }
+    }
 };
 
 // What spmm_kernel takes for a lane type: SpmmArgs, and for a row-scaled table (E4m3x16) one f32 scale per row of X as
@@ -1190,25 +1209,17 @@ extern "C" int bns_cvt_rows_f32_bf16(const float *src, int64_t lds, uint16_t *ds
 
 namespace {
 
-// One warp per row, 8 columns per lane and step.  m = max |x| of the row; the scale is 2^e with e the smallest integer
-// such that m * 2^-e <= 448 (the largest finite e4m3), e >= -126; 1 for a row of zeros; NaN for a row holding NaN or
-// +-Inf, whose codes are 0.  Codes: x * 2^-e (exact: a power of two, never above 448) rounded to nearest even e4m3.
-__global__ void __launch_bounds__(kThreads) cvt_rows_fp8_kernel(const float *__restrict__ src, int64_t lds,
-                                                                uint8_t *__restrict__ codes, int64_t ldc,
-                                                                float *__restrict__ scale, int64_t n_rows, int F) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps = (int64_t)gridDim.x * kWarps;
-    for (int64_t r = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); r < n_rows; r += warps) {
-        const float *x = src + r * lds;
-        uint32_t m = 0;                         // bits of max |x|: NaN > Inf > every finite value
-        for (int c = lane * 8; c < F; c += 256) {
-            const float4 a = __ldg(reinterpret_cast<const float4 *>(x + c)), b = __ldg(reinterpret_cast<const float4 *>(x + c + 4));
-            const float e[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-#pragma unroll
-            for (int i = 0; i < 8; ++i) m = max(m, __float_as_uint(e[i]) & 0x7fffffffu);
-        }
-        m = __reduce_max_sync(0xffffffffu, m);
-        const bool bad = m >= 0x7f800000u;
+// The fp8 row rule (ABI 7), the one place it is stated: every fp8 table and every fp8 row on the exchange's wire is made
+// here.  m = max |x| of the row, given as the bits of |x| reduced over the row (abs_bits: NaN > Inf > every finite
+// value); the scale is 2^e with e the smallest integer such that m * 2^-e <= 448 (the largest finite e4m3), e >= -126;
+// 1 for a row of zeros; NaN for a row holding NaN or +-Inf, whose codes are 0.  Codes: x * 2^-e (exact: a power of two,
+// never above 448) rounded to nearest even e4m3.
+struct Fp8Row {
+    float scale, inv;                           // 2^e (NaN for a row that is not finite) and 2^-e
+    bool bad;
+    __device__ __forceinline__ static uint32_t abs_bits(float x) { return __float_as_uint(x) & 0x7fffffffu; }
+    __device__ __forceinline__ explicit Fp8Row(uint32_t m) {
+        bad = m >= 0x7f800000u;
         int ex = 0;
         if (m >= 0x00800000u) {                 // normal: m = 1.M * 2^(E-127); 1.M <= 1.75 leaves one more doubling
             const int E = (int)(m >> 23);
@@ -1217,22 +1228,77 @@ __global__ void __launch_bounds__(kThreads) cvt_rows_fp8_kernel(const float *__r
         } else if (m != 0) {
             ex = -126;
         }
-        const float inv = __uint_as_float((uint32_t)(127 - ex) << 23);
-        if (lane == 0) scale[r] = bad ? __uint_as_float(0x7fc00000u) : __uint_as_float((uint32_t)(127 + ex) << 23);
+        inv = __uint_as_float((uint32_t)(127 - ex) << 23);
+        scale = bad ? __uint_as_float(0x7fc00000u) : __uint_as_float((uint32_t)(127 + ex) << 23);
+    }
+    // the codes of x[0:4], low byte first
+    __device__ __forceinline__ uint32_t codes4(float4 x) const {
+        if (bad) return 0u;
+        const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(x.x * inv, x.y * inv), __NV_SATFINITE, __NV_E4M3);
+        const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(x.z * inv, x.w * inv), __NV_SATFINITE, __NV_E4M3);
+        return lo | (hi << 16);
+    }
+};
+
+// One warp per row, 8 columns per lane and step (rows of any width: the row is read twice).
+__global__ void __launch_bounds__(kThreads) cvt_rows_fp8_kernel(const float *__restrict__ src, int64_t lds,
+                                                                uint8_t *__restrict__ codes, int64_t ldc,
+                                                                float *__restrict__ scale, int64_t n_rows, int F) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps = (int64_t)gridDim.x * kWarps;
+    for (int64_t r = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); r < n_rows; r += warps) {
+        const float *x = src + r * lds;
+        uint32_t m = 0;
+        for (int c = lane * 8; c < F; c += 256) {
+            const float4 a = __ldg(reinterpret_cast<const float4 *>(x + c)), b = __ldg(reinterpret_cast<const float4 *>(x + c + 4));
+            const float e[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int i = 0; i < 8; ++i) m = max(m, Fp8Row::abs_bits(e[i]));
+        }
+        const Fp8Row row(__reduce_max_sync(0xffffffffu, m));
+        if (lane == 0) scale[r] = row.scale;
         uint8_t *q = codes + r * ldc;
         for (int c = lane * 8; c < F; c += 256) {
             uint2 o = make_uint2(0u, 0u);
-            if (!bad) {
+            if (!row.bad) {
                 const float4 a = __ldg(reinterpret_cast<const float4 *>(x + c)), b = __ldg(reinterpret_cast<const float4 *>(x + c + 4));
-                const uint32_t q0 = __nv_cvt_float2_to_fp8x2(make_float2(a.x * inv, a.y * inv), __NV_SATFINITE, __NV_E4M3);
-                const uint32_t q1 = __nv_cvt_float2_to_fp8x2(make_float2(a.z * inv, a.w * inv), __NV_SATFINITE, __NV_E4M3);
-                const uint32_t q2 = __nv_cvt_float2_to_fp8x2(make_float2(b.x * inv, b.y * inv), __NV_SATFINITE, __NV_E4M3);
-                const uint32_t q3 = __nv_cvt_float2_to_fp8x2(make_float2(b.z * inv, b.w * inv), __NV_SATFINITE, __NV_E4M3);
-                o = make_uint2(q0 | (q1 << 16), q2 | (q3 << 16));
+                o = make_uint2(row.codes4(a), row.codes4(b));
             }
             *reinterpret_cast<uint2 *>(q + c) = o;
         }
     }
+}
+
+// By one warp: codes[0:F] and *scale, the fp8 row (Fp8Row) of the f32 quotients src[0:F] / div.  F <= 1024 and
+// F % 16 == 0, so each lane keeps its quotients of at most two 16-column groups in registers and stores each group's
+// codes as one 16-byte word.  The divisions are the f32 put's (Vec<4>::load_div).
+__device__ __forceinline__ void quantize_row_fp8(const float *src, float div, int F, uint8_t *codes, float *scale,
+                                                 int lane) {
+    float4 q[2][4];
+    uint32_t m = 0;
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+        const int f = (lane + 32 * t) * 16;
+        if (f < F) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                Vec<4> v;
+                v.load_div(src + f + 4 * j, div);
+                q[t][j] = v.v;
+                m = max(max(m, max(Fp8Row::abs_bits(v.v.x), Fp8Row::abs_bits(v.v.y))),
+                        max(Fp8Row::abs_bits(v.v.z), Fp8Row::abs_bits(v.v.w)));
+            }
+        }
+    }
+    const Fp8Row row(__reduce_max_sync(0xffffffffu, m));
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+        const int f = (lane + 32 * t) * 16;
+        if (f < F)
+            *reinterpret_cast<uint4 *>(codes + f) =
+                make_uint4(row.codes4(q[t][0]), row.codes4(q[t][1]), row.codes4(q[t][2]), row.codes4(q[t][3]));
+    }
+    if (lane == 0) *scale = row.scale;
 }
 
 }  // namespace

@@ -414,6 +414,25 @@ __global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllDev a) {
     publish_flags(a);
 }
 
+struct PutAllFp8Dev : PutAllDev {               // remote: the code rows (ld_remote bytes apart)
+    float *scale[kMaxPeers];                    // the rows' scales in the peer's slab
+};
+
+// one warp per row: the remote row = the fp8 row of H[r] / div (quantize_row_fp8: codes and scale), F <= 1024
+__global__ void __launch_bounds__(kThreads) p2p_put_all_fp8_kernel(PutAllFp8Dev a) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
+        int s = 0;
+        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
+        const int64_t local = i - a.row_begin[s];
+        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
+        quantize_row_fp8(a.H + r * a.ldh, a.div[s], a.F, reinterpret_cast<uint8_t *>(a.remote[s]) + local * a.ld_remote,
+                         a.scale[s] + local, lane);
+    }
+    publish_flags(a);
+}
+
 struct PutIdsDev {
     int32_t n_seg;
     int64_t begin[kMaxPeers + 1];
@@ -462,11 +481,16 @@ struct ScatterAllDev {
     float *G; int64_t ldg; int32_t F; int64_t n_rows;
 };
 
+struct ScatterAllFp8Dev : ScatterAllDev {      // recv: the code rows (ld_recv bytes apart)
+    const float *scale[kMaxPeers];              // their scales
+};
+
 // one warp per destination row: contributions of the peers are added in table order (= the reference's ring order,
 // helper/feature_buffer.py:111-129), each with a true division -- bit-identical to P-1 successive scatter-adds.  The
 // column loop is warp-uniform: every lane takes every shuffle, and the lanes past F load and store nothing.
-template <class L>
-__global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDev a) {
+// D: ScatterAllDev, or ScatterAllFp8Dev for fp8 rows (E4m3x16), whose received row k of segment s is scaled by scale[s][k].
+template <class L, class D>
+__device__ __forceinline__ void scatter_rows_all_body(const D &a) {
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
     for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < a.n_rows; row += warps_total) {
@@ -483,21 +507,32 @@ __global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDe
             for (int s = 0; s < a.n_seg; ++s) {
                 const int32_t k = __shfl_sync(0xffffffffu, mine, s);
                 if (k < 0 || !on) continue;
-                v.add_div(reinterpret_cast<const typename L::T *>(a.recv[s]) + (int64_t)k * a.ld_recv + f, a.div[s]);
+                const auto *r = reinterpret_cast<const typename L::T *>(a.recv[s]) + (int64_t)k * a.ld_recv + f;
+                if constexpr (std::is_same_v<D, ScatterAllFp8Dev>) v.add_div(r, a.scale[s][k], a.div[s]);
+                else v.add_div(r, a.div[s]);
             }
             if (on) v.store(g + f);
         }
     }
 }
 
-// bns_p2p_put_all_f32 / _bf16 (T = float / uint16_t on the wire): one set of checks and one segment table
+template <class L>
+__global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDev a) { scatter_rows_all_body<L>(a); }
+
+__global__ void __launch_bounds__(kThreads) scatter_rows_all_fp8_kernel(ScatterAllFp8Dev a) {
+    scatter_rows_all_body<E4m3x16>(a);
+}
+
+// bns_p2p_put_all_f32 / _bf16 / _fp8 (T = float / uint16_t / uint8_t on the wire): one set of checks and one segment
+// table; scale_off: the fp8 rows' scale offsets (NULL otherwise)
 template <class T>
-int put_all(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh, int64_t F,
-            const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index, uint64_t flag_value,
-            const uint64_t *flag_value_dev, void *stream) {
+int put_all(bns_p2p_t *p, const bns_put_all *segs, const uint64_t *scale_off, int64_t ld_remote, const float *H,
+            int64_t ldh, int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
+            uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
     constexpr bool bf16 = sizeof(T) == 2;       // bf16 rows: 16-byte access only, no scalar path
-    const char *fn = bf16 ? "bns_p2p_put_all_bf16" : "bns_p2p_put_all_f32";
-    BNS_REQUIRE(p && segs, "%s: NULL argument", fn);
+    constexpr bool fp8 = sizeof(T) == 1;        // fp8 rows: 16-byte code words, a warp's row in registers
+    const char *fn = fp8 ? "bns_p2p_put_all_fp8" : bf16 ? "bns_p2p_put_all_bf16" : "bns_p2p_put_all_f32";
+    BNS_REQUIRE(p && segs && (!fp8 || scale_off), "%s: NULL argument", fn);
     BNS_REQUIRE(segs->n_seg >= 0 && segs->n_seg <= kMaxPeers, "%s: too many segments", fn);
     BNS_REQUIRE(flag_index >= 0 && flag_index < p->n_flags, "%s: bad flag index", fn);
     BNS_REQUIRE(ticket_index >= 0 && ticket_index < p->n_tickets, "%s: bad ticket index", fn);
@@ -505,8 +540,11 @@ int put_all(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const floa
     BNS_REQUIRE(!bf16 || (F % 8 == 0 && ldh % 8 == 0 && ld_remote % 8 == 0),
                 "%s: F, ldh and ld_remote must be multiples of 8 (F %lld, ldh %lld, ld_remote %lld)", fn, (long long)F,
                 (long long)ldh, (long long)ld_remote);
+    BNS_REQUIRE(!fp8 || (F % 16 == 0 && ldh % 16 == 0 && ld_remote % 16 == 0 && F <= 1024),
+                "%s: F, ldh and ld_remote must be multiples of 16 and F at most 1024 (F %lld, ldh %lld, ld_remote %lld)",
+                fn, (long long)F, (long long)ldh, (long long)ld_remote);
     if (segs->n_seg == 0) return BNS_OK;
-    PutAllDev a;
+    PutAllFp8Dev a;
     a.n_seg = segs->n_seg;
     // the f32 16-byte path also needs every destination 16-byte aligned; the scalar path takes rows of any width
     bool vec = F % 4 == 0 && ldh % 4 == 0 && ld_remote % 4 == 0 && (reinterpret_cast<uintptr_t>(H) & 15u) == 0;
@@ -518,10 +556,15 @@ int put_all(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const floa
         BNS_REQUIRE(p->peer_slab[peer] && p->peer_flags[peer], "%s: peer %d not connected", fn, peer);
         BNS_REQUIRE(k >= 0, "%s: negative row count", fn);
         BNS_REQUIRE(k == 0 || segs->div[s] != 0.f, "%s: division by zero", fn);
-        BNS_REQUIRE(segs->remote_off[s] % (bf16 ? 16 : 4) == 0 &&
+        BNS_REQUIRE(segs->remote_off[s] % (bf16 || fp8 ? 16 : 4) == 0 &&
                         segs->remote_off[s] + (size_t)k * ld_remote * sizeof(T) <= p->peer_slab_bytes[peer],
-                    bf16 ? "%s: remote range of segment %d outside peer %d's slab or not 16-byte aligned"
-                         : "%s: remote range of segment %d outside peer %d's slab", fn, s, peer);
+                    bf16 || fp8 ? "%s: remote range of segment %d outside peer %d's slab or not 16-byte aligned"
+                                : "%s: remote range of segment %d outside peer %d's slab", fn, s, peer);
+        if (fp8) {
+            BNS_REQUIRE(scale_off[s] % 4 == 0 && scale_off[s] + (size_t)k * sizeof(float) <= p->peer_slab_bytes[peer],
+                        "%s: scale range of segment %d outside peer %d's slab or not 4-byte aligned", fn, s, peer);
+            a.scale[s] = reinterpret_cast<float *>(p->peer_slab[peer] + scale_off[s]);
+        }
         vec = vec && segs->remote_off[s] % 16 == 0;
         a.remote[s] = reinterpret_cast<float *>(p->peer_slab[peer] + segs->remote_off[s]);
         a.flag[s] = p->peer_flags[peer] + flag_index;
@@ -530,46 +573,60 @@ int put_all(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const floa
     }
     const int64_t total = segs->row_begin[segs->n_seg];
     BNS_REQUIRE(total == 0 || H, "%s: NULL source", fn);
-    BNS_REQUIRE(!bf16 || (reinterpret_cast<uintptr_t>(H) & 15u) == 0, "%s: source not 16-byte aligned", fn);
+    BNS_REQUIRE(!(bf16 || fp8) || (reinterpret_cast<uintptr_t>(H) & 15u) == 0, "%s: source not 16-byte aligned", fn);
     a.H = H; a.ldh = ldh; a.F = (int32_t)F; a.idx = idx_cat; a.ld_remote = ld_remote;
     a.flag_value = flag_value; a.flag_value_dev = reinterpret_cast<const unsigned long long *>(flag_value_dev);
     a.ticket = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(p->flags) + align256((size_t)p->n_flags * 8)) + ticket_index;
     const unsigned grid = rows_grid(total);
-    if (bf16) p2p_put_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(a);
-    else if (vec) p2p_put_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
-    else p2p_put_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    const PutAllDev &b = a;
+    if (fp8) p2p_put_all_fp8_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else if (bf16) p2p_put_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(b);
+    else if (vec) p2p_put_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
+    else p2p_put_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
 }
 
-// bns_scatter_rows_all_f32 / _bf16 (T = float / uint16_t received rows)
+// bns_scatter_rows_all_f32 / _bf16 / _fp8 (T = float / uint16_t / uint8_t received rows); scale: the fp8 rows' scales
+// per segment (NULL otherwise)
 template <class T>
 int scatter_rows_all(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg, const int32_t *const *inv,
-                     const T *const *recv, int64_t ld_recv, const float *div, void *stream) {
+                     const T *const *recv, const float *const *scale, int64_t ld_recv, const float *div, void *stream) {
     constexpr bool bf16 = sizeof(T) == 2;       // bf16 rows: 16-byte access only, no scalar path
-    const char *fn = bf16 ? "bns_scatter_rows_all_bf16" : "bns_scatter_rows_all_f32";
+    constexpr bool fp8 = sizeof(T) == 1;        // fp8 rows: 16-byte code words only
+    const char *fn = fp8 ? "bns_scatter_rows_all_fp8" : bf16 ? "bns_scatter_rows_all_bf16" : "bns_scatter_rows_all_f32";
     BNS_REQUIRE(n_seg >= 0 && n_seg <= kMaxPeers, "%s: too many segments", fn);
     if (n_seg == 0 || n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(G && inv && recv && div && F > 0 && ldg >= F && ld_recv >= F, "%s: bad argument", fn);
+    BNS_REQUIRE(G && inv && recv && div && (!fp8 || scale) && F > 0 && ldg >= F && ld_recv >= F, "%s: bad argument", fn);
     BNS_REQUIRE(!bf16 || (F % 8 == 0 && ldg % 4 == 0 && ld_recv % 8 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0),
                 "%s: needs F %% 8 == 0, ldg %% 4 == 0, ld_recv %% 8 == 0 and a 16-byte aligned G "
                 "(F %lld, ldg %lld, ld_recv %lld)", fn, (long long)F, (long long)ldg, (long long)ld_recv);
-    ScatterAllDev a;
+    BNS_REQUIRE(!fp8 || (F % 16 == 0 && ldg % 4 == 0 && ld_recv % 16 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0),
+                "%s: needs F %% 16 == 0, ldg %% 4 == 0, ld_recv %% 16 == 0 and a 16-byte aligned G "
+                "(F %lld, ldg %lld, ld_recv %lld)", fn, (long long)F, (long long)ldg, (long long)ld_recv);
+    ScatterAllFp8Dev a;
     a.n_seg = n_seg;
     bool vec = F % 4 == 0 && ldg % 4 == 0 && ld_recv % 4 == 0 && (reinterpret_cast<uintptr_t>(G) & 15u) == 0;
     for (int s = 0; s < n_seg; ++s) {
         const bool aligned = (reinterpret_cast<uintptr_t>(recv[s]) & 15u) == 0;
-        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f && (aligned || !bf16),
-                    bf16 ? "%s: bad segment %d (NULL, misaligned or division by zero)" : "%s: bad segment %d", fn, s);
+        BNS_REQUIRE(inv[s] && recv[s] && div[s] != 0.f && (aligned || !(bf16 || fp8)),
+                    bf16 || fp8 ? "%s: bad segment %d (NULL, misaligned or division by zero)" : "%s: bad segment %d", fn, s);
+        if (fp8) {
+            BNS_REQUIRE(scale[s] && (reinterpret_cast<uintptr_t>(scale[s]) & 3u) == 0,
+                        "%s: scales of segment %d NULL or not 4-byte aligned", fn, s);
+            a.scale[s] = scale[s];
+        }
         a.inv[s] = inv[s]; a.recv[s] = reinterpret_cast<const float *>(recv[s]); a.div[s] = div[s];
         vec = vec && aligned;
     }
     a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
     const unsigned grid = rows_grid(n_rows);
-    if (bf16) scatter_rows_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(a);
-    else if (vec) scatter_rows_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
-    else scatter_rows_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    const ScatterAllDev &b = a;
+    if (fp8) scatter_rows_all_fp8_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    else if (bf16) scatter_rows_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(b);
+    else if (vec) scatter_rows_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
+    else scatter_rows_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -580,6 +637,8 @@ void preload_exchange_kernels() {
     cudaFuncAttributes fa;
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Bf16x8>);
     cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<Bf16x8>);
+    cudaFuncGetAttributes(&fa, p2p_put_all_fp8_kernel);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_fp8_kernel);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<4>>);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<1>>);
     cudaFuncGetAttributes(&fa, p2p_put_ids_kernel);
@@ -594,8 +653,8 @@ void preload_exchange_kernels() {
 extern "C" int bns_p2p_put_all_f32(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
                                    int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
                                    uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
-    return put_all<float>(p, segs, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value, flag_value_dev,
-                          stream);
+    return put_all<float>(p, segs, nullptr, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value,
+                          flag_value_dev, stream);
 }
 
 extern "C" int bns_p2p_put_ids_i64(bns_p2p_t *p, int32_t n_seg, const int64_t *begin, const int32_t *peers,
@@ -655,20 +714,35 @@ extern "C" int bns_p2p_wait_all(bns_p2p_t *p, int32_t n, const int32_t *flag_ind
 extern "C" int bns_scatter_rows_all_f32(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
                                         const int32_t *const *inv, const float *const *recv, int64_t ld_recv,
                                         const float *div, void *stream) {
-    return scatter_rows_all<float>(G, ldg, n_rows, F, n_seg, inv, recv, ld_recv, div, stream);
+    return scatter_rows_all<float>(G, ldg, n_rows, F, n_seg, inv, recv, nullptr, ld_recv, div, stream);
 }
 
 extern "C" int bns_p2p_put_all_bf16(bns_p2p_t *p, const bns_put_all *segs, int64_t ld_remote, const float *H, int64_t ldh,
                                     int64_t F, const int64_t *idx_cat, int32_t flag_index, int32_t ticket_index,
                                     uint64_t flag_value, const uint64_t *flag_value_dev, void *stream) {
-    return put_all<uint16_t>(p, segs, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value,
+    return put_all<uint16_t>(p, segs, nullptr, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value,
                              flag_value_dev, stream);
 }
 
 extern "C" int bns_scatter_rows_all_bf16(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
                                          const int32_t *const *inv, const uint16_t *const *recv, int64_t ld_recv,
                                          const float *div, void *stream) {
-    return scatter_rows_all<uint16_t>(G, ldg, n_rows, F, n_seg, inv, recv, ld_recv, div, stream);
+    return scatter_rows_all<uint16_t>(G, ldg, n_rows, F, n_seg, inv, recv, nullptr, ld_recv, div, stream);
+}
+
+extern "C" int bns_p2p_put_all_fp8(bns_p2p_t *p, const bns_put_all *segs, const uint64_t *scale_off, int64_t ld_remote,
+                                   const float *H, int64_t ldh, int64_t F, const int64_t *idx_cat, int32_t flag_index,
+                                   int32_t ticket_index, uint64_t flag_value, const uint64_t *flag_value_dev,
+                                   void *stream) {
+    return put_all<uint8_t>(p, segs, scale_off, ld_remote, H, ldh, F, idx_cat, flag_index, ticket_index, flag_value,
+                            flag_value_dev, stream);
+}
+
+extern "C" int bns_scatter_rows_all_fp8(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
+                                        const int32_t *const *inv, const uint8_t *const *recv,
+                                        const float *const *recv_scale, int64_t ld_recv, const float *div,
+                                        void *stream) {
+    return scatter_rows_all<uint8_t>(G, ldg, n_rows, F, n_seg, inv, recv, recv_scale, ld_recv, div, stream);
 }
 
 // ---- the staged transport's pack (K3) and scatter (K5) with a bf16 wire side, and the exact widening ----
@@ -740,6 +814,121 @@ extern "C" int bns_cvt_rows_bf16_f32(const uint16_t *src, int64_t lds, float *ds
     const int64_t want = (work + kThreads - 1) / kThreads;
     cvt_rows_bf16_f32_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, dst, ldd,
                                                                                                        n_rows, F, vec);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// ---- the staged transport's pack and scatter with an fp8 wire side, and the exact widening ----
+namespace {
+
+// one warp per row: out[i] / out_scale[i] = the fp8 row of H[idx[i]] / div (quantize_row_fp8)
+__global__ void __launch_bounds__(kThreads) gather_div_fp8_kernel(const float *__restrict__ H, int64_t ldh,
+                                                                  const int64_t *__restrict__ idx, int64_t k, int32_t F,
+                                                                  float div, uint8_t *__restrict__ out, int64_t ldo,
+                                                                  float *__restrict__ out_scale) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total)
+        quantize_row_fp8(H + idx[i] * ldh, div, F, out + i * ldo, out_scale + i, lane);
+}
+
+// one warp per row: G[idx[i]] += (src[i] * src_scale[i]) / div, the f32 scatter's arithmetic (E4m3x16::add_div)
+__global__ void __launch_bounds__(kThreads) scatter_add_div_fp8_kernel(const uint8_t *__restrict__ src, int64_t lds,
+                                                                       const float *__restrict__ src_scale,
+                                                                       const int64_t *__restrict__ idx, int64_t k,
+                                                                       int32_t F, float div, float *__restrict__ G,
+                                                                       int64_t ldg) {
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
+        float *g = G + idx[i] * ldg;
+        const float s = src_scale[i];
+        for (int f = lane * 16; f < F; f += 512) {
+            E4m3x16 v;
+            v.load(g + f);
+            v.add_div(src + i * lds + f, s, div);
+            v.store(g + f);
+        }
+    }
+}
+
+// one thread per 16 codes: dst = codes * scale, exact
+__global__ void __launch_bounds__(kThreads) cvt_rows_fp8_f32_kernel(const uint8_t *__restrict__ codes, int64_t ldc,
+                                                                    const float *__restrict__ scale,
+                                                                    float *__restrict__ dst, int64_t ldd,
+                                                                    int64_t n_rows, int64_t F) {
+    const int64_t per_row = F / 16, total = n_rows * per_row;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t r = i / per_row, c = (i - r * per_row) * 16;
+        const uint4 u = __ldg(reinterpret_cast<const uint4 *>(codes + r * ldc + c));
+        const float s = __ldg(scale + r);
+        const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+        float4 *d = reinterpret_cast<float4 *>(dst + r * ldd + c);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 a = e4m3x2_f32(w[j] & 0xffffu), b = e4m3x2_f32(w[j] >> 16);
+            d[j] = make_float4(a.x * s, a.y * s, b.x * s, b.y * s);
+        }
+    }
+}
+
+// fp8 rows with an f32 side: F, both leading dimensions multiples of 16 (f32 side: of 4), 16-byte aligned matrices
+inline bool fp8_rows_ok(const void *f32, const void *codes, const void *scale, int64_t F, int64_t ld32, int64_t ld8) {
+    return F % 16 == 0 && ld32 % 4 == 0 && ld8 % 16 == 0 &&
+           ((reinterpret_cast<uintptr_t>(f32) | reinterpret_cast<uintptr_t>(codes)) % 16) == 0 &&
+           reinterpret_cast<uintptr_t>(scale) % 4 == 0;
+}
+
+}  // namespace
+
+extern "C" int bns_gather_div_fp8(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
+                                  uint8_t *out, int64_t ldo, float *out_scale, void *stream) {
+    BNS_REQUIRE(k >= 0 && F > 0, "bns_gather_div_fp8: bad size");
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(H && out && out_scale && idx, "bns_gather_div_fp8: NULL pointer");
+    BNS_REQUIRE(ldh >= F && ldo >= F, "bns_gather_div_fp8: leading dimension smaller than F");
+    BNS_REQUIRE(div != 0.f, "bns_gather_div_fp8: division by zero");
+    BNS_REQUIRE(F <= 1024 && ldh % 16 == 0 && fp8_rows_ok(H, out, out_scale, F, ldh, ldo),
+                "bns_gather_div_fp8: needs F <= 1024, F, ldh, ldo multiples of 16, 16-byte aligned H, out and 4-byte "
+                "aligned scales (F %lld, ldh %lld, ldo %lld)", (long long)F, (long long)ldh, (long long)ldo);
+    gather_div_fp8_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, idx, k, (int32_t)F, div, out, ldo,
+                                                                             out_scale);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_scatter_add_div_fp8(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
+                                       const uint8_t *src, int64_t lds, const float *src_scale, void *stream) {
+    BNS_REQUIRE(k >= 0 && F > 0, "bns_scatter_add_div_fp8: bad size");
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(G && src && src_scale && idx, "bns_scatter_add_div_fp8: NULL pointer");
+    BNS_REQUIRE(ldg >= F && lds >= F, "bns_scatter_add_div_fp8: leading dimension smaller than F");
+    BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_fp8: division by zero");
+    BNS_REQUIRE(fp8_rows_ok(G, src, src_scale, F, ldg, lds),
+                "bns_scatter_add_div_fp8: needs F, lds multiples of 16, ldg of 4, 16-byte aligned G, src and 4-byte "
+                "aligned scales (F %lld, ldg %lld, lds %lld)", (long long)F, (long long)ldg, (long long)lds);
+    scatter_add_div_fp8_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, src_scale, idx, k, (int32_t)F,
+                                                                                  div, G, ldg);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_cvt_rows_fp8_f32(const uint8_t *codes, int64_t ldc, const float *scale, float *dst, int64_t ldd,
+                                    int64_t n_rows, int64_t F, void *stream) {
+    BNS_REQUIRE(n_rows >= 0 && F >= 0 && ldc >= F && ldd >= F, "bns_cvt_rows_fp8_f32: bad shape");
+    if (n_rows == 0 || F == 0) return BNS_OK;
+    BNS_REQUIRE(codes && scale && dst, "bns_cvt_rows_fp8_f32: NULL matrix");
+    BNS_REQUIRE(fp8_rows_ok(dst, codes, scale, F, ldd, ldc),
+                "bns_cvt_rows_fp8_f32: needs F, ldc multiples of 16, ldd of 4, 16-byte aligned codes, dst and 4-byte "
+                "aligned scales (F %lld, ldc %lld, ldd %lld)", (long long)F, (long long)ldc, (long long)ldd);
+    const int64_t work = n_rows * (F / 16);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const int64_t want = (work + kThreads - 1) / kThreads;
+    cvt_rows_fp8_f32_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(codes, ldc, scale, dst,
+                                                                                                      ldd, n_rows, F);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

@@ -370,8 +370,8 @@ def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf
                halo: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``rs * (A_in x_u[:n_in] + A_out[:, sampled] x_u[n_in:])`` -- the inner pass first (it needs local rows only), the
     halo pass after the exchange's event.  ``bf16``: the ``_gather_table`` mode of both passes (f32 sums).  ``halo``:
-    the halo rows as they arrived in bf16 (``--comm-dtype bf16``; ``x_u`` is then the inner rows alone), gathered as
-    they are, whatever the mode."""
+    the halo rows as they arrived, bf16 or an ``ops.Fp8Rows`` table (``--comm-dtype bf16`` / ``fp8``; ``x_u`` is then
+    the inner rows alone), gathered as they are, whatever the mode."""
     y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16), row_scale=rs)
     if ready is not None:
         torch.cuda.current_stream(x_u.device).wait_event(ready)
@@ -384,8 +384,8 @@ def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf
 
 
 def _halo_rows(h_u: torch.Tensor, n_in: int, halo: Optional[torch.Tensor]) -> torch.Tensor:
-    """The f32 halo rows a narrow layer transforms: ``h_u[n_in:]``, or (``--comm-dtype bf16``) the received bf16 rows
-    widened into a matrix of their own -- the inner rows stay where they are."""
+    """The f32 halo rows a narrow layer transforms: ``h_u[n_in:]``, or (``--comm-dtype bf16`` / ``fp8``) the received
+    bf16 / fp8 rows widened exactly into a matrix of their own -- the inner rows stay where they are."""
     return h_u[n_in:] if halo is None else ops.cvt_rows_f32(halo)
 
 
@@ -438,7 +438,8 @@ class SageConvFn(torch.autograd.Function):
                 exchange=None, halo=None):
         """``exchange = (Buffer, layer)`` when ``h_u`` came out of ``Buffer.update``: the backward then hands the halo
         rows of its gradient to ``Buffer.begin_backward`` as soon as they are final.  ``halo``: the received halo rows in
-        bf16 (``--comm-dtype bf16``); ``h_u`` is then the inner rows alone, and so is the returned gradient."""
+        bf16 (``--comm-dtype bf16``) or as an ``ops.Fp8Rows`` table (``--comm-dtype fp8``); ``h_u`` is then the inner
+        rows alone, and so is the returned gradient."""
         ctx.exchange, ctx.inner_only = exchange, halo is not None
         n_in = g.n_in
         h_u = h_u.contiguous()
@@ -518,7 +519,7 @@ class GcnConvFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h_u, w, b, g: PartitionGraph, rs, cs_u, ready, arena: ParamArena, narrow_first: bool,
                 exchange=None, halo=None):
-        """``exchange`` / ``halo``: as for ``SageConvFn`` (``--comm-dtype bf16``)."""
+        """``exchange`` / ``halo``: as for ``SageConvFn`` (``--comm-dtype bf16`` / ``fp8``)."""
         ctx.exchange, ctx.inner_only = exchange, halo is not None
         n_in = g.n_in
         h_u = h_u.contiguous()

@@ -15,6 +15,9 @@ Same surface -- ``init_buffer(num_in, ratio, f_send_shape, f_recv_shape, layer_s
 ``H[selected]/ratio`` -- and each returned gradient row -- to bf16 once, so the wire and the receiving slab carry half
 the bytes.  ``update`` then returns the inner rows ``[n_in, F]`` (f32, as given) with the received halo rows attached
 as ``_bns_halo`` (bf16 ``[recv_total, F]``), and the halo gradient travels only through ``begin_backward``.
+``comm_dtype='fp8'`` (``--comm-dtype fp8``) does the same with fp8 rows (``ops.Fp8Rows``: e4m3 codes plus a power-of-two
+scale per row, ``ops.cvt_rows_fp8``'s rule over the f32 quotients): ``F + 4`` bytes a row, and ``_bns_halo`` is an
+``Fp8Rows`` view of the received codes and scales -- the gather table of the wide layers' halo pass as it arrived.
 
 The exchange runs on ``self._comm_stream``; with ``update(..., overlap=True)`` the caller's stream does not wait
 for it -- the aggregation op waits on ``h_u._bns_ready`` right before it touches the halo rows, so the transfer
@@ -50,7 +53,24 @@ def slab_layout(n_in, recv_total, send_total, width, n_comm_layers, comm_dtype='
     """Byte layout of one rank's peer-mapped slab.  Per communicating layer: a forward region -- the ``n_in`` inner f32
     rows, then the ``recv_total`` received halo rows -- and a backward region of the ``send_total`` gradient rows this
     rank gets back; the received id lists close the slab.  With bf16 the halo and backward rows are bf16 and every
-    sub-region starts on 256 bytes.  ``*_bytes``: the size of each region (one layer)."""
+    sub-region starts on 256 bytes.  With fp8 the halo and backward rows are e4m3 codes, each followed by its region of
+    f32 scales (``halo_scale_off`` / ``bwd_scale_off``), every sub-region on 256 bytes.  ``*_bytes``: the size of each
+    region (one layer)."""
+    if comm_dtype == 'fp8':
+        n_h, n_b = max(recv_total, 1), max(send_total, 1)
+        inner, halo, halo_s = _a256(n_in * width * 4), _a256(n_h * width), _a256(n_h * 4)
+        bwd, bwd_s = _a256(n_b * width), _a256(n_b * 4)
+        stride = inner + halo + halo_s + bwd + bwd_s
+        fwd_off = [l * stride for l in range(n_comm_layers)]
+        halo_off = [o + inner for o in fwd_off]
+        halo_scale_off = [o + halo for o in halo_off]
+        bwd_off = [o + halo_s for o in halo_scale_off]
+        bwd_scale_off = [o + bwd for o in bwd_off]
+        ids_off = n_comm_layers * stride
+        return {"fwd_off": fwd_off, "halo_off": halo_off, "halo_scale_off": halo_scale_off, "bwd_off": bwd_off,
+                "bwd_scale_off": bwd_scale_off, "ids_off": ids_off, "slab_bytes": ids_off + max(recv_total, 1) * 8,
+                "inner_bytes": inner, "halo_bytes": halo, "halo_scale_bytes": halo_s, "bwd_bytes": bwd,
+                "bwd_scale_bytes": bwd_s}
     if comm_dtype == 'bf16':
         inner, halo, bwd = _a256(n_in * width * 4), _a256(max(recv_total, 1) * width * 2), _a256(max(send_total, 1) * width * 2)
         stride = inner + halo + bwd
@@ -71,10 +91,10 @@ def slab_layout(n_in, recv_total, send_total, width, n_comm_layers, comm_dtype='
 
 def wire_bytes(send_total, recv_total, F, comm_dtype='f32') -> dict:
     """Feature bytes one rank moves per communicating layer and epoch: forward it sends its ``send_total`` sampled rows
-    and receives ``recv_total`` halo rows; backward the reverse."""
-    e = 2 if comm_dtype == 'bf16' else 4
-    return {"fwd_send": send_total * F * e, "fwd_recv": recv_total * F * e,
-            "bwd_send": recv_total * F * e, "bwd_recv": send_total * F * e}
+    and receives ``recv_total`` halo rows; backward the reverse.  An fp8 row is ``F`` codes and one f32 scale."""
+    row = F + 4 if comm_dtype == 'fp8' else F * (2 if comm_dtype == 'bf16' else 4)
+    return {"fwd_send": send_total * row, "fwd_recv": recv_total * row,
+            "bwd_send": recv_total * row, "bwd_recv": send_total * row}
 
 
 class Buffer(object):
@@ -98,7 +118,9 @@ class Buffer(object):
         self.seq_dev = None
         self.seq_base = 0
         self._maps = None
-        self._bf16 = False
+        self._comm_dtype = 'f32'
+        self._bf16 = self._fp8 = False
+        self._apart = False                     # bf16 / fp8: the halo rows travel and are returned apart from feat
 
     # helper/feature_buffer.py:23-33
     def __init_pl_pr(self):
@@ -118,8 +140,8 @@ class Buffer(object):
                     device=None, comm_dtype='f32'):
         if use_pp is False:
             raise NotImplementedError            # helper/feature_buffer.py:36-37
-        if comm_dtype not in ('f32', 'bf16'):
-            raise ValueError(f"comm_dtype {comm_dtype!r}: expected 'f32' or 'bf16'")
+        if comm_dtype not in ('f32', 'bf16', 'fp8'):
+            raise ValueError(f"comm_dtype {comm_dtype!r}: expected 'f32', 'bf16' or 'fp8'")
         c = ctx.comm()
         # captured now: backward runs on autograd's device thread, where thread-local lookups would miss
         self._comm, self._timer = c, comm_timer._get()
@@ -144,9 +166,13 @@ class Buffer(object):
             raise RuntimeError("Buffer needs a CUDA device: there is no CPU exchange path")
         width = self._layer_size[1]              # the reference sizes every slab with layer_size[1] (:54-55)
         self._width = width
-        self._bf16 = comm_dtype == 'bf16'
+        self._comm_dtype = comm_dtype
+        self._bf16, self._fp8 = comm_dtype == 'bf16', comm_dtype == 'fp8'
+        self._apart = self._bf16 or self._fp8
         if self._bf16 and width % 8:
             raise ValueError(f"comm_dtype bf16: exchanged width {width} is not a multiple of 8")
+        if self._fp8 and width % 16:
+            raise ValueError(f"comm_dtype fp8: exchanged width {width} is not a multiple of 16")
         wire = torch.bfloat16 if self._bf16 else torch.float32
         self._comm_stream = torch.cuda.Stream(self._device)
         self._send_begin, tot = [], 0
@@ -155,15 +181,13 @@ class Buffer(object):
             tot += 0 if j == self._rank else self._send_shape[j]
         self._send_total = tot
         if backend == 'nccl':
-            self._send_buf = [None if j == self._rank else
-                              torch.zeros(self._send_shape[j], width, dtype=wire, device=self._device)
-                              for j in range(self._size)]
-            self._b_recv = [None if j == self._rank else
-                            torch.zeros(self._send_shape[j], width, dtype=wire, device=self._device)
-                            for j in range(self._size)]
-            # bf16: the halo gradient rows are rounded into this buffer before they are sent (f32 sends them in place)
-            self._b_send = (torch.zeros(max(self._n_u - num_in, 1), width, dtype=wire, device=self._device)
-                            if self._bf16 else None)
+            def rows(n):
+                return self._fp8_rows(n) if self._fp8 else torch.zeros(n, width, dtype=wire, device=self._device)
+            self._send_buf = [None if j == self._rank else rows(self._send_shape[j]) for j in range(self._size)]
+            self._b_recv = [None if j == self._rank else rows(self._send_shape[j]) for j in range(self._size)]
+            # bf16 / fp8: the halo gradient rows are rounded into this buffer before they are sent (f32 sends them in
+            # place)
+            self._b_send = rows(max(self._n_u - num_in, 1)) if self._apart else None
         else:
             self.__init_p2p(c, width)
 
@@ -178,9 +202,10 @@ class Buffer(object):
             tot += 0 if j == self._rank else self._recv_shape[j]
         self._recv_total = tot
         # after the feature regions: the received id lists of the epoch (data_transfer NODE), int64 [sum of recv sizes]
-        lay = slab_layout(self._num_in, tot, self._send_total, width, n_comm_layers, 'bf16' if self._bf16 else 'f32')
+        lay = slab_layout(self._num_in, tot, self._send_total, width, n_comm_layers, self._comm_dtype)
         self._fwd_off, self._halo_off, self._bwd_off, self._ids_off = (lay["fwd_off"], lay["halo_off"], lay["bwd_off"],
                                                                        lay["ids_off"])
+        self._halo_scale_off, self._bwd_scale_off = lay.get("halo_scale_off"), lay.get("bwd_scale_off")
         slab_bytes = lay["slab_bytes"]
         self._n_comm_layers = n_comm_layers
         n_flags = (n_comm_layers * 2 + 1) * self._size          # (layer, direction, source) + (ids, source)
@@ -195,7 +220,7 @@ class Buffer(object):
         self._slab_ptr = slab.value
         # publish: where peers must write inside MY slab (row offsets of their segment) + how to map my memory
         my = {"fwd_off": self._fwd_off, "halo_off": self._halo_off, "bwd_off": self._bwd_off, "pl": self._pl,
-              "send_begin": self._send_begin,
+              "send_begin": self._send_begin, "halo_scale_off": self._halo_scale_off, "bwd_scale_off": self._bwd_scale_off,
               "ids_off": self._ids_off, "hop_begin": self._hop_begin, "slab_bytes": nbytes.value}
         if c.kind == "thread":
             my["ptrs"] = (slab.value, flags.value)
@@ -330,8 +355,31 @@ class Buffer(object):
         self._seq[key] = self._seq.get(key, 0) + 1
         return self._seq[key], None
 
+    def _esz(self):
+        """Bytes per element of a row on the wire (an fp8 row's scale lives apart)."""
+        return 1 if self._fp8 else 2 if self._bf16 else 4
+
     def _flag(self, layer, backward, src):
         return ((layer - 1) * 2 + (1 if backward else 0)) * self._size + src
+
+    def _fp8_rows(self, rows, alloc=torch.zeros):
+        """An ``ops.Fp8Rows`` of ``rows`` rows of the slab width (the staged transport's buffers)."""
+        return ops.Fp8Rows(alloc(rows, self._width, dtype=torch.float8_e4m3fn, device=self._device),
+                           alloc(rows, dtype=torch.float32, device=self._device))
+
+    def _slab_fp8(self, codes_off, scale_off, rows):
+        """``ops.Fp8Rows`` view of ``rows`` code rows of the slab width and their scales in this rank's slab."""
+        codes = torch.as_tensor(_DevArray(self._slab_ptr + codes_off, (rows, self._width), "|u1"), device=self._device)
+        scale = torch.as_tensor(_DevArray(self._slab_ptr + scale_off, (rows,)), device=self._device)
+        return ops.Fp8Rows(codes.view(torch.float8_e4m3fn), scale)
+
+    def _alltoall(self, send, recv, tag):
+        """``comm.alltoall``; fp8 rows go as two messages per peer, their codes (as bytes), then their scales."""
+        if not self._fp8:
+            return self._comm.alltoall(send, recv, tag=tag)
+        for part in (lambda r: r.codes.view(torch.uint8), lambda r: r.scale):
+            self._comm.alltoall([None if r is None else part(r) for r in send],
+                                [None if r is None else part(r) for r in recv], tag=tag)
 
     def _slab_view(self, byte_off, rows, bf16=False):
         if bf16:
@@ -367,8 +415,8 @@ class Buffer(object):
         if overlap:
             res._bns_ready = self._last_ready
         res._bns_exchange = (self, layer)          # lets a fused consumer start the gradient return trip early
-        if self._bf16:
-            res._bns_halo = self._last_halo        # the received rows, bf16: the layer gathers / widens them itself
+        if self._apart:
+            res._bns_halo = self._last_halo        # the received rows, bf16 / fp8: the layer gathers / widens them itself
         return res
 
     def _forward(self, layer, feat, overlap):
@@ -378,14 +426,18 @@ class Buffer(object):
         feat = feat.contiguous()
         main, cs = torch.cuda.current_stream(self._device), self._comm_stream
         ready = torch.cuda.Event()
-        bf16, halo = self._bf16, None
-        if self._p2p is not None and F != self._width:
-            raise RuntimeError("p2p transport needs equal hidden widths")
-        if bf16:
-            # the inner rows go on as they are (no concat); the halo rows land in a bf16 table of their own
+        bf16, fp8, apart, halo = self._bf16, self._fp8, self._apart, None
+        if (self._p2p is not None or fp8) and F != self._width:
+            raise RuntimeError(f"{'p2p transport' if self._p2p is not None else 'comm_dtype fp8'} needs equal hidden "
+                               "widths")
+        if apart:
+            # the inner rows go on as they are (no concat); the halo rows land in a bf16 / fp8 table of their own
             h_u, n_halo = feat, self._n_u - self._num_in
             if self._backend == 'nccl':
-                halo = torch.empty(n_halo, F, dtype=torch.bfloat16, device=self._device)
+                halo = (self._fp8_rows(n_halo, torch.empty) if fp8 else
+                        torch.empty(n_halo, F, dtype=torch.bfloat16, device=self._device))
+            elif fp8:
+                halo = self._slab_fp8(self._halo_off[layer - 1], self._halo_scale_off[layer - 1], max(n_halo, 1))[:n_halo]
             else:
                 halo = self._slab_view(self._halo_off[layer - 1], max(n_halo, 1), bf16=True)[:n_halo]
         elif self._backend == 'nccl':
@@ -405,32 +457,36 @@ class Buffer(object):
                     for j in range(self._size):
                         if j == self._rank:
                             continue
-                        send[j] = self._send_buf[j][:, :F] if F == self._width else \
+                        send[j] = self._send_buf[j] if fp8 else self._send_buf[j][:, :F] if F == self._width else \
                             torch.empty(self._send_shape[j], F, dtype=self._send_buf[j].dtype, device=self._device)
                         ops.gather_div(feat, self._selected[j], self._ratio[j], out=send[j])      # K3
-                        recv[j] = (halo[self._pl[j] - self._num_in:self._pr[j] - self._num_in] if bf16 else
+                        recv[j] = (halo[self._pl[j] - self._num_in:self._pr[j] - self._num_in] if apart else
                                    h_u[self._pl[j]:self._pr[j]])
-                    self._comm.alltoall(send, recv, tag=16 + layer)                               # C1/C2
+                    self._alltoall(send, recv, 16 + layer)                                        # C1/C2
                 else:
                     seq, seq_dev = self._seq_args(layer, False)
                     segs = PutAll()
                     segs.n_seg = len(self._peers)
+                    scale_off = (ctypes.c_uint64 * max(len(self._peers), 1))()
                     tot = 0
                     for s_, j in enumerate(self._peers):
                         lay = self._peer_layout[j]
                         segs.row_begin[s_] = tot
                         tot += self._send_shape[j]
                         segs.peer[s_] = j
-                        if bf16:
+                        if fp8:
+                            segs.remote_off[s_] = lay["halo_off"][layer - 1] + lay["hop_begin"][self._rank] * self._width
+                            scale_off[s_] = lay["halo_scale_off"][layer - 1] + lay["hop_begin"][self._rank] * 4
+                        elif bf16:
                             segs.remote_off[s_] = lay["halo_off"][layer - 1] + lay["hop_begin"][self._rank] * self._width * 2
                         else:
                             segs.remote_off[s_] = lay["fwd_off"][layer - 1] + lay["pl"][self._rank] * self._width * 4
                         segs.div[s_] = float(self._ratio[j]) if self._send_shape[j] else 1.0
                     segs.row_begin[segs.n_seg] = tot
                     sel_cat = self._selected_cat
-                    put = "bns_p2p_put_all_bf16" if bf16 else "bns_p2p_put_all_f32"
-                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), self._width, feat.data_ptr(), feat.stride(0),
-                                            F, sel_cat.data_ptr() if tot else None,
+                    put = f"bns_p2p_put_all_{self._comm_dtype}"
+                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), *((scale_off,) if fp8 else ()), self._width,
+                                            feat.data_ptr(), feat.stride(0), F, sel_cat.data_ptr() if tot else None,
                                             self._flag(layer, False, self._rank), self._size + (layer - 1) * 2, seq,
                                             seq_dev, cs.cuda_stream), put)
                     for j in self._peers:
@@ -443,7 +499,9 @@ class Buffer(object):
             ready.record(cs)
         if not self.graph_mode:
             feat.record_stream(cs)
-            (halo if bf16 else h_u).record_stream(cs)
+            (halo.codes if fp8 else halo if bf16 else h_u).record_stream(cs)
+            if fp8:
+                halo.scale.record_stream(cs)
         if not overlap:
             main.wait_event(ready)
         self._last_ready, self._last_halo = ready, halo
@@ -469,23 +527,27 @@ class Buffer(object):
         with torch.cuda.stream(cs):
             with self._timer_ctx(f'backward_{layer}', cs):
                 if self._backend == 'nccl':
-                    # bf16: the sender rounds its halo gradient rows once, then sends them per peer
+                    # bf16 / fp8: the sender rounds its halo gradient rows once, then sends them per peer
                     rows = grad
-                    if self._bf16:
+                    if self._fp8:
+                        halo = grad[self._num_in:]
+                        rows = ops.cvt_rows_fp8(halo, out=self._b_send[:halo.shape[0]])
+                    elif self._bf16:
                         halo = grad[self._num_in:]
                         rows = (ops.cvt_rows_bf16(halo, out=self._b_send[:halo.shape[0]]) if F == self._width else
                                 ops.cvt_rows_bf16(halo))
-                    b0 = self._num_in if self._bf16 else 0
+                    b0 = self._num_in if self._apart else 0
                     send = [None if j == self._rank else rows[self._pl[j] - b0:self._pr[j] - b0] for j in range(self._size)]
                     recv = [None if j == self._rank else
-                            (self._b_recv[j][:, :F] if F == self._width else
+                            (self._b_recv[j] if self._fp8 else self._b_recv[j][:, :F] if F == self._width else
                              torch.empty(self._send_shape[j], F, dtype=self._b_recv[j].dtype, device=self._device))
                             for j in range(self._size)]
-                    self._comm.alltoall(send, recv, tag=64 + layer)
+                    self._alltoall(send, recv, 64 + layer)
                 else:
                     seq, seq_dev = self._seq_args(layer, True)
                     segs = PutAll()
                     segs.n_seg = len(self._peers)
+                    scale_off = (ctypes.c_uint64 * max(len(self._peers), 1))()
                     tot = 0
                     for s_, j in enumerate(self._peers):
                         lay = self._peer_layout[j]
@@ -493,14 +555,17 @@ class Buffer(object):
                         tot += self._recv_shape[j]
                         segs.peer[s_] = j
                         segs.remote_off[s_] = (lay["bwd_off"][layer - 1] +
-                                               lay["send_begin"][self._rank] * self._width * (2 if self._bf16 else 4))
+                                               lay["send_begin"][self._rank] * self._width * self._esz())
+                        if self._fp8:
+                            scale_off[s_] = lay["bwd_scale_off"][layer - 1] + lay["send_begin"][self._rank] * 4
                         segs.src_begin[s_] = self._pl[j]
                         segs.div[s_] = 1.0
                     segs.row_begin[segs.n_seg] = tot
-                    put = "bns_p2p_put_all_bf16" if self._bf16 else "bns_p2p_put_all_f32"
-                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), self._width, grad.data_ptr(), grad.stride(0),
-                                            F, None, self._flag(layer, True, self._rank),
-                                            self._size + (layer - 1) * 2 + 1, seq, seq_dev, cs.cuda_stream), put)
+                    put = f"bns_p2p_put_all_{self._comm_dtype}"
+                    check(getattr(lib, put)(self._p2p, ctypes.byref(segs), *((scale_off,) if self._fp8 else ()),
+                                            self._width, grad.data_ptr(), grad.stride(0), F, None,
+                                            self._flag(layer, True, self._rank), self._size + (layer - 1) * 2 + 1, seq,
+                                            seq_dev, cs.cuda_stream), put)
                     for j in self._peers:
                         self._post_put_event(j, 2001 + 2 * layer, cs)
                     for j in self._peers:
@@ -509,9 +574,11 @@ class Buffer(object):
                     check(lib.bns_p2p_wait_all(self._p2p, len(self._peers), idx, seq, seq_dev, cs.cuda_stream),
                           "bns_p2p_wait_all")
                     recv = [None] * self._size
-                    bwd = self._slab_view(self._bwd_off[layer - 1], max(self._send_total, 1), bf16=self._bf16)
+                    n_b = max(self._send_total, 1)
+                    bwd = (self._slab_fp8(self._bwd_off[layer - 1], self._bwd_scale_off[layer - 1], n_b) if self._fp8 else
+                           self._slab_view(self._bwd_off[layer - 1], n_b, bf16=self._bf16)[:, :F])
                     for j in self._peers:
-                        recv[j] = bwd[self._send_begin[j]:self._send_begin[j] + self._send_shape[j], :F]
+                        recv[j] = bwd[self._send_begin[j]:self._send_begin[j] + self._send_shape[j]]
             done.record(cs)
         if not self.graph_mode:
             grad.record_stream(cs)
@@ -528,9 +595,9 @@ class Buffer(object):
         begun, self._begun = getattr(self, "_begun", None), None
         if begun is not None and begun[0] == layer and begun[1] == grad.data_ptr():
             done, recv = begun[2]                     # the producer already sent the halo rows (begin_backward)
-        elif self._bf16:
-            raise RuntimeError("comm_dtype bf16: the layer that consumed the exchange must hand its halo gradient to "
-                               "Buffer.begin_backward (the fused GraphSAGE / GCN layers do)")
+        elif self._apart:
+            raise RuntimeError(f"comm_dtype {self._comm_dtype}: the layer that consumed the exchange must hand its halo "
+                               "gradient to Buffer.begin_backward (the fused GraphSAGE / GCN layers do)")
         else:
             done, recv = self._exchange_backward(layer, grad)
         main.wait_event(done)
@@ -546,12 +613,15 @@ class Buffer(object):
                 n = len(order)
                 inv = (ctypes.c_void_p * n)(*[self._inv[j].data_ptr() for j in order])
                 base = self._slab_ptr + self._bwd_off[layer - 1]
-                esz = 2 if self._bf16 else 4
-                rcv = (ctypes.c_void_p * n)(*[base + self._send_begin[j] * self._width * esz for j in order])
+                rcv = (ctypes.c_void_p * n)(*[base + self._send_begin[j] * self._width * self._esz() for j in order])
+                scl = ()
+                if self._fp8:
+                    sb = self._slab_ptr + self._bwd_scale_off[layer - 1]
+                    scl = ((ctypes.c_void_p * n)(*[sb + self._send_begin[j] * 4 for j in order]),)
                 div = (ctypes.c_float * n)(*[float(self._ratio[j]) for j in order])
-                fn = "bns_scatter_rows_all_bf16" if self._bf16 else "bns_scatter_rows_all_f32"
+                fn = f"bns_scatter_rows_all_{self._comm_dtype}"
                 with torch.cuda.device(self._device):
-                    check(getattr(lib, fn)(inner.data_ptr(), inner.stride(0), self._num_in, F, n, inv, rcv,
+                    check(getattr(lib, fn)(inner.data_ptr(), inner.stride(0), self._num_in, F, n, inv, rcv, *scl,
                                            self._width, div, main.cuda_stream), fn)
         if trace is not None:
             trace[f"grad_h{layer}"] = inner.detach().clone()

@@ -73,11 +73,13 @@ def build_parser():
                              "even) with one power-of-two scale per row: a quarter of the f32 bytes; hidden widths "
                              "must be multiples of 16.  Only with the fused training step (GraphSAGE / GCN, --use-pp, "
                              "--norm layer, no --n-linear)")
-    parser.add_argument(*_spellings("comm-dtype"), default="f32", choices=["f32", "bf16"],
+    parser.add_argument(*_spellings("comm-dtype"), default="f32", choices=["f32", "bf16", "fp8"],
                         help="NEW: element type of the boundary rows the training exchange moves.  bf16 rounds each "
                              "sampled row H[selected]/ratio, and each returned halo gradient row, to bf16 (nearest even) "
-                             "at the sender: half the wire and slab bytes; the receiver widens and sums in f32.  Only "
-                             "with the fused training step (GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+                             "at the sender: half the wire and slab bytes; the receiver widens and sums in f32.  fp8 "
+                             "sends each such row as e4m3 codes plus one power-of-two scale (the --agg-dtype fp8 row "
+                             "format): F + 4 bytes a row; the hidden width must be a multiple of 16.  Only with the "
+                             "fused training step (GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
     parser.add_argument(*_spellings("dense-dtype"), default="f32", choices=["f32", "bf16"],
                         help="NEW: operand precision of the training step's dense layers.  f32 runs the f32-accurate "
                              "3xTF32 tensor-core scheme; bf16 rounds every GEMM operand to bf16 (nearest even) inside "

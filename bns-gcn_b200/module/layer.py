@@ -84,7 +84,7 @@ class GCNLayer(nn.Module):
                 return _f.PPLinearFn.apply(feat, self.linear.weight, self.linear.bias, arena, p, seed)
             out_f, in_f = self.linear.out_features, self.linear.in_features
             narrow = AGGREGATE_AFTER_TRANSFORM and out_f < in_f
-            # --comm-dtype bf16: the halo rows arrive apart from feat, and their gradient returns through the exchange
+            # --comm-dtype bf16 / fp8: the halo rows arrive apart from feat, and their gradient returns through the exchange
             halo = getattr(feat, '_bns_halo', None)
             out = _f.GcnConvFn.apply(feat, self.linear.weight, self.linear.bias, graph, graph.recip(in_norm),
                                      graph.recip(out_norm), getattr(feat, '_bns_ready', None), arena, narrow,

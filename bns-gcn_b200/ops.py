@@ -406,12 +406,19 @@ class AggregateSum(torch.autograd.Function):
 
 def gather_div(h: torch.Tensor, idx: torch.Tensor, div: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``out[i] = h[idx[i]] / div`` (helper/feature_buffer.py:117).  A bf16 ``out`` (``--comm-dtype bf16``) receives the
-    f32 quotient rounded to nearest even (``bns_gather_div_bf16``)."""
+    f32 quotient rounded to nearest even (``bns_gather_div_bf16``); an ``Fp8Rows`` ``out`` (``--comm-dtype fp8``) the
+    fp8 rows of the f32 quotients (``bns_gather_div_fp8``, ``cvt_rows_fp8``'s rule)."""
     _req(h, torch.float32, "h")
     _req(idx, torch.int64, "idx")
     k, F = idx.numel(), h.shape[1]
     if out is None:
         out = torch.empty(k, F, dtype=torch.float32, device=h.device)
+    if isinstance(out, Fp8Rows):
+        _table(out, "out")
+        with torch.cuda.device(h.device):
+            check(lib.bns_gather_div_fp8(h.data_ptr(), h.stride(0), F, idx.data_ptr(), k, float(div), out.codes.data_ptr(),
+                                         out.codes.stride(0), out.scale.data_ptr(), _stream_ptr()), "bns_gather_div_fp8")
+        return out
     fn = "bns_gather_div_bf16" if out.dtype == torch.bfloat16 else "bns_gather_div_f32"
     if fn == "bns_gather_div_f32":
         _req(out, torch.float32, "out")
@@ -423,8 +430,17 @@ def gather_div(h: torch.Tensor, idx: torch.Tensor, div: float, out: Optional[tor
 
 def scatter_add_div(g: torch.Tensor, idx: torch.Tensor, src: torch.Tensor, div: float) -> torch.Tensor:
     """``g[idx[i]] += src[i] / div`` in place (helper/feature_buffer.py:129).  A bf16 ``src`` (``--comm-dtype bf16``)
-    is widened exactly before the f32 division and sum (``bns_scatter_add_div_bf16``)."""
+    is widened exactly before the f32 division and sum (``bns_scatter_add_div_bf16``), an ``Fp8Rows`` ``src``
+    (``--comm-dtype fp8``) dequantized exactly (``bns_scatter_add_div_fp8``)."""
     _req(g, torch.float32, "g")
+    if isinstance(src, Fp8Rows):
+        _table(src, "src")
+        _req(idx, torch.int64, "idx")
+        with torch.cuda.device(g.device):
+            check(lib.bns_scatter_add_div_fp8(g.data_ptr(), g.stride(0), g.shape[1], idx.data_ptr(), idx.numel(),
+                                              float(div), src.codes.data_ptr(), src.codes.stride(0), src.scale.data_ptr(),
+                                              _stream_ptr()), "bns_scatter_add_div_fp8")
+        return g
     fn = "bns_scatter_add_div_bf16" if src.dtype == torch.bfloat16 else "bns_scatter_add_div_f32"
     if fn == "bns_scatter_add_div_f32":
         _req(src, torch.float32, "src")
@@ -481,16 +497,26 @@ def cvt_rows_fp8(src: torch.Tensor, out: Optional[Fp8Rows] = None) -> Fp8Rows:
 
 
 def cvt_rows_f32(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """``bns_cvt_rows_bf16_f32``: bf16 rows widened to f32 (exact), into ``out`` or a new ``[rows, F]`` matrix."""
-    _req(src, torch.bfloat16, "src")
-    if src.dim() != 2 or src.stride(1) != 1:
-        raise _lib.BnsError("src must be a row-major 2-D tensor")
+    """``bns_cvt_rows_bf16_f32``: bf16 rows widened to f32 (exact), into ``out`` or a new ``[rows, F]`` matrix.  An
+    ``Fp8Rows`` ``src`` (``bns_cvt_rows_fp8_f32``) gives its codes times their scales (exact)."""
+    fp8 = isinstance(src, Fp8Rows)
+    if fp8:
+        _table(src, "src")
+    else:
+        _req(src, torch.bfloat16, "src")
+        if src.dim() != 2 or src.stride(1) != 1:
+            raise _lib.BnsError("src must be a row-major 2-D tensor")
     n, F = src.shape
     if out is None:
         out = torch.empty(n, F, dtype=torch.float32, device=src.device)
     _req(out, torch.float32, "out")
     if out.shape != src.shape or out.stride(1) != 1:
         raise _lib.BnsError("out must be row-major with the shape of src")
+    if fp8:
+        with torch.cuda.device(src.device):
+            check(lib.bns_cvt_rows_fp8_f32(src.codes.data_ptr(), src.codes.stride(0), src.scale.data_ptr(), out.data_ptr(),
+                                           out.stride(0), n, F, _stream_ptr()), "bns_cvt_rows_fp8_f32")
+        return out
     with torch.cuda.device(src.device):
         check(lib.bns_cvt_rows_bf16_f32(src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0), n, F, _stream_ptr()),
               "bns_cvt_rows_bf16_f32")

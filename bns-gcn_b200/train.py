@@ -388,12 +388,19 @@ def _exchanged_x8(args, layer_size):
     return None
 
 
+def _exchanged_x16(args, layer_size):
+    bad = sorted({w for w in layer_size[1:-1] if w % 16})
+    if bad:
+        return f"exchanged width {', '.join(map(str, bad))} is not a multiple of 16 (fp8 rows move 16 at a time)"
+    return None
+
+
 # --<flag>-dtype: what the check returns for f32, and for each narrower mode the width rule it adds to the fused step's
 # (a function returning the broken rule's message or None; None in place of the function: nothing more) and what the
 # check returns for it
 _DTYPE_FLAGS = {
     'agg': (False, {'bf16': (_hidden_x8, True), 'fp8': (_hidden_x16, 'fp8')}),
-    'comm': ('f32', {'bf16': (_exchanged_x8, 'bf16')}),
+    'comm': ('f32', {'bf16': (_exchanged_x8, 'bf16'), 'fp8': (_exchanged_x16, 'fp8')}),
     'dense': (False, {'bf16': (None, True)}),
 }
 
@@ -422,8 +429,9 @@ def check_agg_dtype(args, layer_size, dev):
 
 
 def check_comm_dtype(args, layer_size, dev) -> str:
-    """The element type of the boundary rows on the wire: ``'f32'``, or ``'bf16'`` (``--comm-dtype bf16``), where the
-    fused layers take the halo rows as bf16 and hand their halo gradient back to the exchange."""
+    """The element type of the boundary rows on the wire: ``'f32'``, ``'bf16'`` (``--comm-dtype bf16``) or ``'fp8'``
+    (``--comm-dtype fp8``: e4m3 codes plus a power-of-two scale per row), where the fused layers take the halo rows as
+    they arrived and hand their halo gradient back to the exchange."""
     return _check_dtype_flag('comm', args, layer_size, dev)
 
 

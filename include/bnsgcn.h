@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 7
+#define BNS_ABI_VERSION 8
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -476,6 +476,41 @@ int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *id
                              const uint16_t *src /*bf16*/, int64_t lds, void *stream);
 int bns_cvt_rows_bf16_f32(const uint16_t *src /*bf16*/, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
                           void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 8: the boundary exchange with an fp8 wire side (--comm-dtype fp8).  Every row that crosses the wire is an ABI 7
+ * fp8 row -- e4m3 codes plus one f32 power-of-two scale, by bns_cvt_rows_f32_fp8's rule -- made by the sender from the
+ * f32 quotients H / div (m is the max of |H / div|, not of |H|).  The receiver's scatters add (code * scale) / div in
+ * f32: the product is exact, so they are the f32 scatters over the dequantized rows, bit for bit.
+ * bns_p2p_put_all_fp8: bns_p2p_put_all_f32 with the remote rows stored as fp8 rows, one warp per row: the codes at
+ *     remote_off[s] (ld_remote bytes apart, as in bns_put_all) and the scales at scale_off[s] (host [n_seg], one float
+ *     per row); same segments, idx_cat / src_begin modes, flags and tickets.  F <= 1024; F, ldh and ld_remote multiples
+ *     of 16, H 16-byte aligned, every remote_off a multiple of 16 and every scale_off of 4, both ranges inside the
+ *     peer's slab, else BNS_E_INVALID before anything launches.
+ * bns_scatter_rows_all_fp8: bns_scatter_rows_all_f32 reading fp8 recv rows (ld_recv in bytes) with their scales
+ *     recv_scale[s] (row k of segment s is scaled by recv_scale[s][k]); same order, same division.  F % 16 == 0,
+ *     ldg % 4 == 0, ld_recv % 16 == 0, 16-byte aligned G and recv rows, 4-byte aligned scales.
+ * bns_gather_div_fp8 / bns_scatter_add_div_fp8: bns_gather_div_f32 / bns_scatter_add_div_f32 (the staged transport's
+ *     pack and scatter) with an fp8 out / src and its scales.  The pack: F <= 1024, F, ldh, ldo multiples of 16; the
+ *     scatter: F, lds multiples of 16, ldg of 4; 16-byte aligned matrices and 4-byte aligned scales.
+ * bns_cvt_rows_fp8_f32: dst[r, :F] = codes[r, :F] * scale[r], exact.  F, ldc multiples of 16, ldd of 4, 16-byte aligned
+ *     codes and dst.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_p2p_put_all_fp8(bns_p2p_t *p, const bns_put_all *segs /*host*/, const uint64_t *scale_off /*host [n_seg]*/,
+                        int64_t ld_remote, const float *H, int64_t ldh, int64_t F, const int64_t *idx_cat,
+                        int32_t flag_index, int32_t ticket_index, uint64_t flag_value, const uint64_t *flag_value_dev,
+                        void *stream);
+int bns_scatter_rows_all_fp8(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n_seg,
+                             const int32_t *const *inv /*host array of device pointers*/,
+                             const uint8_t *const *recv /*host array of device pointers, e4m3*/,
+                             const float *const *recv_scale /*host array of device pointers*/, int64_t ld_recv,
+                             const float *div /*host*/, void *stream);
+int bns_gather_div_fp8(const float *H, int64_t ldh, int64_t F, const int64_t *idx /*device [k]*/, int64_t k, float div,
+                       uint8_t *out /*e4m3*/, int64_t ldo, float *out_scale, void *stream);
+int bns_scatter_add_div_fp8(float *G, int64_t ldg, int64_t F, const int64_t *idx /*device [k]*/, int64_t k, float div,
+                            const uint8_t *src /*e4m3*/, int64_t lds, const float *src_scale, void *stream);
+int bns_cvt_rows_fp8_f32(const uint8_t *codes /*e4m3*/, int64_t ldc, const float *scale, float *dst, int64_t ldd,
+                         int64_t n_rows, int64_t F, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * ABI 6: the dense layers with bf16 tensor-core products (--dense-dtype bf16).  Same operands (f32 in HBM), shapes,

@@ -1,11 +1,11 @@
-"""``--comm-dtype f32`` against ``--comm-dtype bf16``: what the boundary exchange moves and what it costs.
+"""``--comm-dtype f32`` against ``bf16`` and ``fp8``: what the boundary exchange moves and what it costs.
 
 * ``bytes``: exact counts from shapes (no GPU): per epoch and rank, the feature bytes sent and received forward and
   backward per communicating layer, and the peer-mapped slab (``feature_buffer.slab_layout``), for the Reddit shape at
   P = 2 / 4 / 8 and the papers100M per-rank shape, at the benchmark's sampling rate 0.1 and hidden width 256.  Reddit:
   232,965 nodes in random partitions, where every inner node is on every peer's boundary, so each rank sends
   int(0.1 n_in) rows to each peer; papers100M: 13.9 M inner nodes and 9.7 M sampled halo rows per rank (sent as many).
-* ``kernels`` (one GPU): CUDA-event time per launch of the all-peer put and the gradient scatter, f32 against bf16, at
+* ``kernels`` (one GPU): CUDA-event time per launch of the all-peer put and the gradient scatter in each mode, at
   the Reddit shape's per-rank sizes at P = 4.  The peers are slabs of this process on the same GPU, so a put's stores
   go to this GPU's HBM: these times say nothing about NVLink.
 * ``epochs``: eager epochs/s of the benchmark's model on the Reddit shape with 4 in-process ranks (threads of this
@@ -30,6 +30,7 @@ sys.path.insert(0, ROOT)
 
 REDDIT_NODES = 232_965
 RATE, WIDTH, N_COMM = 0.1, 256, 2          # the benchmark's model: 3 layers, the inputs of layers 1 and 2 exchanged
+MODES = ("f32", "bf16", "fp8")
 
 
 def byte_counts() -> dict:
@@ -43,14 +44,16 @@ def byte_counts() -> dict:
     out = {}
     for name, (n_in, send, recv) in shapes.items():
         row = {"n_in": n_in, "send_rows": send, "recv_rows": recv}
-        for m in ("f32", "bf16"):
+        for m in MODES:
             w = wire_bytes(send, recv, WIDTH, m)
             lay = slab_layout(n_in, recv, send, WIDTH, N_COMM, m)
             row[m] = {"per_layer": w, "per_epoch_sent": N_COMM * (w["fwd_send"] + w["bwd_send"]),
                       "per_epoch_received": N_COMM * (w["fwd_recv"] + w["bwd_recv"]),
-                      "slab_bytes": lay["slab_bytes"], "slab_halo_region": lay["halo_bytes"],
-                      "slab_backward_region": lay["bwd_bytes"]}
+                      "slab_bytes": lay["slab_bytes"],
+                      "slab_halo_region": lay["halo_bytes"] + lay.get("halo_scale_bytes", 0),
+                      "slab_backward_region": lay["bwd_bytes"] + lay.get("bwd_scale_bytes", 0)}
         row["sent_ratio_bf16_over_f32"] = row["bf16"]["per_epoch_sent"] / row["f32"]["per_epoch_sent"]
+        row["sent_ratio_fp8_over_bf16"] = row["fp8"]["per_epoch_sent"] / row["bf16"]["per_epoch_sent"]
         out[name] = row
     return out
 
@@ -68,6 +71,7 @@ def card() -> dict:
 def kernel_times(iters: int = 200) -> dict:
     """Rank 0 of P = 4 on the Reddit shape: 3 peers, int(0.1 n_in) rows each, F = 256."""
     import torch
+    from bns_gcn_b200 import ops
     from bns_gcn_b200._lib import PutAll, check, lib
     dev = torch.device("cuda", 0)
     P, n_in = 4, -(-REDDIT_NODES // 4)
@@ -109,11 +113,14 @@ def kernel_times(iters: int = 200) -> dict:
         b.record()
         b.synchronize()
         return a.elapsed_time(b) / iters
-    s32, s16 = segs(4), segs(2)
+    s32, s16, s8 = segs(4), segs(2), segs(1)
+    scale_off = (ctypes.c_uint64 * (P - 1))(*[k * WIDTH] * (P - 1))          # the codes at 0, their scales after them
     put = {"f32": lambda: check(lib.bns_p2p_put_all_f32(hs[0], ctypes.byref(s32), WIDTH, H.data_ptr(), WIDTH, WIDTH,
                                                         idx.data_ptr(), 1, P, 1, None, st), "put f32"),
            "bf16": lambda: check(lib.bns_p2p_put_all_bf16(hs[0], ctypes.byref(s16), WIDTH, H.data_ptr(), WIDTH, WIDTH,
-                                                          idx.data_ptr(), 1, P, 1, None, st), "put bf16")}
+                                                          idx.data_ptr(), 1, P, 1, None, st), "put bf16"),
+           "fp8": lambda: check(lib.bns_p2p_put_all_fp8(hs[0], ctypes.byref(s8), scale_off, WIDTH, H.data_ptr(), WIDTH,
+                                                        WIDTH, idx.data_ptr(), 1, P, 1, None, st), "put fp8")}
     invs = []
     for i in range(P - 1):
         m = torch.full((n_in,), -1, dtype=torch.int32, device=dev)
@@ -121,17 +128,22 @@ def kernel_times(iters: int = 200) -> dict:
         invs.append(m)
     recv32 = [torch.randn(k, WIDTH, device=dev, generator=g) for _ in range(P - 1)]
     recv16 = [r.to(torch.bfloat16) for r in recv32]
+    recv8 = [ops.cvt_rows_fp8(r) for r in recv32]
     G = torch.zeros(n_in, WIDTH, device=dev)
     inv = (ctypes.c_void_p * (P - 1))(*[m.data_ptr() for m in invs])
     div = (ctypes.c_float * (P - 1))(*[0.1] * (P - 1))
     r32 = (ctypes.c_void_p * (P - 1))(*[r.data_ptr() for r in recv32])
     r16 = (ctypes.c_void_p * (P - 1))(*[r.data_ptr() for r in recv16])
+    r8 = (ctypes.c_void_p * (P - 1))(*[r.codes.data_ptr() for r in recv8])
+    sc8 = (ctypes.c_void_p * (P - 1))(*[r.scale.data_ptr() for r in recv8])
     scat = {"f32": lambda: check(lib.bns_scatter_rows_all_f32(G.data_ptr(), WIDTH, n_in, WIDTH, P - 1, inv, r32, WIDTH,
                                                               div, st), "scatter f32"),
             "bf16": lambda: check(lib.bns_scatter_rows_all_bf16(G.data_ptr(), WIDTH, n_in, WIDTH, P - 1, inv, r16, WIDTH,
-                                                                div, st), "scatter bf16")}
+                                                                div, st), "scatter bf16"),
+            "fp8": lambda: check(lib.bns_scatter_rows_all_fp8(G.data_ptr(), WIDTH, n_in, WIDTH, P - 1, inv, r8, sc8, WIDTH,
+                                                              div, st), "scatter fp8")}
     for rnd in range(3):                        # alternate the modes: other work on the host shares the GPU
-        for m in ("f32", "bf16"):
+        for m in MODES:
             res.setdefault(f"put_ms_{m}", []).append(round(timed(put[m]), 5))
             res.setdefault(f"scatter_ms_{m}", []).append(round(timed(scat[m]), 5))
     torch.cuda.synchronize()
@@ -201,11 +213,11 @@ def main():
         out["kernels"] = kernel_times()
         out["kernels"]["note"] = ("in-process peers share one GPU's HBM: these times say nothing about NVLink")
     if a.only in (None, "epochs"):
-        out["epochs_reddit_P4_inprocess_eager"] = {m: _train("reddit", 4, m, a.epochs, 2, False) for m in ("f32", "bf16")}
+        out["epochs_reddit_P4_inprocess_eager"] = {m: _train("reddit", 4, m, a.epochs, 2, False) for m in MODES}
         out["epochs_reddit_P4_inprocess_eager"]["note"] = (
             "4 ranks as threads of one process on one GPU (shared HBM, eager: in-process ranks cannot be graph-captured)")
     if a.only in (None, "convergence"):
-        out["convergence_small_P4_200_epochs"] = {m: _train("small", 4, m, 198, 2, True) for m in ("f32", "bf16")}
+        out["convergence_small_P4_200_epochs"] = {m: _train("small", 4, m, 198, 2, True) for m in MODES}
     print(json.dumps(out))
 
 

@@ -1,7 +1,7 @@
 """Multi-process / multi-GPU check of the exchange transports (run under torchrun, one rank per GPU):
 
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 \
-      tools/dist_check.py [--shape small] [--rate 0.3] [--graph] [--dropout 0.5] [--comm-dtype bf16]
+      tools/dist_check.py [--shape small] [--rate 0.3] [--graph] [--dropout 0.5] [--comm-dtype bf16|fp8]
 
 Every rank trains a few epochs of the same seeded configuration with backend=nccl and backend=p2p (real NCCL
 send/recv, real cudaIpc peer mappings over NVLink) and rank 0 compares the result -- loss, all-reduced weight
@@ -62,7 +62,7 @@ def main():
                     help="dropout rate of the model (the replayed masks must equal the eager ones)")
     ap.add_argument("--comm", default="torch", choices=["torch", "abi"],
                     help="abi: all-reduce / all-to-all through libbnsgcn.so's own communicator (bns_ctx_create ...)")
-    ap.add_argument("--comm-dtype", default="f32", choices=["f32", "bf16"],
+    ap.add_argument("--comm-dtype", default="f32", choices=["f32", "bf16", "fp8"],
                     help="element type of the exchanged boundary rows, on both sides of the comparison")
     a = ap.parse_args()
     os.environ["BNS_COMM"] = a.comm
@@ -90,8 +90,8 @@ def main():
         ctx.reset()
         ref = run_threads(world, lambda c, r: train_rank(parts[r], mk_args(a.shape, a.rate, "nccl", a.hidden, world, a.dropout,
                                                                            a.comm_dtype), dev, a.epochs), device=str(dev))
-        # bf16 rows: a last-bit difference of an f32 quotient (the all-reduce sums in NCCL's order, not the in-process
-        # one) can move a row element across a bf16 rounding boundary, a 2^-8 step of that element
+        # bf16 / fp8 rows: a last-bit difference of an f32 quotient (the all-reduce sums in NCCL's order, not the
+        # in-process one) can move a row element across a rounding boundary, a 2^-8 (bf16) or 2^-4 (fp8) step of it
         tol = 1e-5 if a.comm_dtype == "f32" else 1e-4
         ref_loss = [sum(ref[r]["loss"][e] for r in range(world)) for e in range(a.epochs)]
         for backend in backends:
