@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -181,6 +181,12 @@ SIGNATURES = {
     "bns_scatter_add_div_fp8": (c_int, [c_void_p, c_int64, c_int64, c_void_p, c_int64, c_float, c_void_p, c_int64,
                                         c_void_p, c_void_p]),
     "bns_cvt_rows_fp8_f32": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p]),
+    # ---- ABI 9 ----
+    "bns_dense_tn_fp8": (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64,
+                                 c_void_p, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p]),
+    "bns_cvt_rows_f32_fp8_any": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p]),
+    "bns_dropout_fp8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_float, c_uint64, c_uint64, c_void_p, c_void_p,
+                                c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
 }
 
 

@@ -1301,7 +1301,52 @@ __device__ __forceinline__ void quantize_row_fp8(const float *src, float div, in
     if (lane == 0) *scale = row.scale;
 }
 
+// By one warp: codes[0:F] and *scale, the fp8 row (Fp8Row) of x[0], x[step], ..., x[(F - 1) step] for any F % 4 == 0
+// (codes 4-byte aligned; step == 1 reads 16-byte vectors, so x must then be 16-byte aligned).  The row is read twice.
+__device__ __forceinline__ void fp8_row_any(const float *x, int64_t step, int F, uint8_t *codes, float *scale, int lane) {
+    auto load4 = [&](int c) {
+        return step == 1 ? *reinterpret_cast<const float4 *>(x + c)
+                         : make_float4(x[c * step], x[(c + 1) * step], x[(c + 2) * step], x[(c + 3) * step]);
+    };
+    uint32_t m = 0;
+    for (int c = 4 * lane; c < F; c += 128) {
+        const float4 v = load4(c);
+        m = max(max(m, max(Fp8Row::abs_bits(v.x), Fp8Row::abs_bits(v.y))),
+                max(Fp8Row::abs_bits(v.z), Fp8Row::abs_bits(v.w)));
+    }
+    const Fp8Row row(__reduce_max_sync(0xffffffffu, m));
+    for (int c = 4 * lane; c < F; c += 128) *reinterpret_cast<uint32_t *>(codes + c) = row.codes4(load4(c));
+    if (lane == 0) *scale = row.scale;
+}
+
+// bns_cvt_rows_f32_fp8 for rows of any width F % 4 == 0 (the dense layers' operands: K = 1204, 44), one warp per row.
+__global__ void __launch_bounds__(kThreads) cvt_rows_fp8_any_kernel(const float *__restrict__ src, int64_t lds,
+                                                                    uint8_t *__restrict__ codes, int64_t ldc,
+                                                                    float *__restrict__ scale, int64_t n_rows, int F) {
+    const int64_t warps = (int64_t)gridDim.x * kWarps;
+    for (int64_t r = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); r < n_rows; r += warps)
+        fp8_row_any(src + r * lds, 1, F, codes + r * ldc, scale + r, threadIdx.x & 31);
+}
+
 }  // namespace
+
+extern "C" int bns_cvt_rows_f32_fp8_any(const float *src, int64_t lds, uint8_t *codes, int64_t ldc, float *scale,
+                                        int64_t n_rows, int64_t F, void *stream) {
+    BNS_REQUIRE(n_rows >= 0 && F >= 0 && F < (1 << 24) && lds >= F && ldc >= F, "bns_cvt_rows_f32_fp8_any: bad shape");
+    if (n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(src && codes && scale, "bns_cvt_rows_f32_fp8_any: NULL matrix");
+    BNS_REQUIRE(F % 4 == 0 && ldc % 16 == 0 && lds % 4 == 0 && (reinterpret_cast<uintptr_t>(scale) & 3u) == 0 &&
+                    ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(codes)) % 16) == 0,
+                "bns_cvt_rows_f32_fp8_any: needs F %% 4 == 0, ldc %% 16 == 0, lds %% 4 == 0, 16-byte aligned src and "
+                "codes and a 4-byte aligned scale (F %lld, lds %lld, ldc %lld)", (long long)F, (long long)lds, (long long)ldc);
+    const int64_t cap = (int64_t)sm_count() * 8;
+    const int64_t want = (n_rows + kWarps - 1) / kWarps;
+    cvt_rows_fp8_any_kernel<<<(unsigned)(want < cap ? want : cap), kThreads, 0, as_stream(stream)>>>(src, lds, codes, ldc,
+                                                                                                      scale, n_rows, (int)F);
+    g_launches += 1;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
 
 extern "C" int bns_cvt_rows_f32_fp8(const float *src, int64_t lds, uint8_t *codes, int64_t ldc, float *scale,
                                     int64_t n_rows, int64_t F, void *stream) {

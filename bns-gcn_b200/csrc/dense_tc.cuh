@@ -60,6 +60,17 @@ constexpr int OP_BF_BYTES = A_BF_BYTES + BN * BK * 2;
 constexpr int SMEM_BF_BYTES = kStagesBf * RAW_BYTES + kOpBufs * OP_BF_BYTES + BAR_BYTES + 1024;
 static_assert(SMEM_BF_BYTES <= 227 * 1024, "exceeds the shared memory of one block");
 static_assert(2 * kStagesBf * 8 <= BAR_BYTES, "barrier region too small");
+// fp8 pipeline (bns_dense_tn_fp8): the operands arrive as e4m3 codes, so one 128-byte swizzle row holds 128 contraction
+// elements and the A / B tiles keep the 16 KB geometry.  The raw stages ARE the wgmma operands (no operand buffer, no
+// conversion): all the shared memory goes into ring depth.
+constexpr int BK_FP8 = 128;                     // e4m3 codes per k-block (one swizzle row)
+constexpr int WG_K_FP8 = 32;                    // wgmma .e4m3: 32 elements (32 bytes) of contraction per instruction
+constexpr int kStagesFp8 = 7;
+constexpr int SMEM_FP8_BYTES = kStagesFp8 * RAW_BYTES + BAR_BYTES + 1024;
+static_assert(SMEM_FP8_BYTES <= 227 * 1024, "exceeds the shared memory of one block");
+static_assert(2 * kStagesFp8 * 8 <= BAR_BYTES, "barrier region too small");
+// operand precision of gemm_body
+enum Prec : int { kPrec3xTf32 = 0, kPrecBf16 = 1, kPrecFp8 = 2 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -271,17 +282,54 @@ __device__ __forceinline__ void cvt_stage(const uint8_t *raw, uint8_t *op, int w
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// The whole pipeline, shared by the 3xTF32 and the bf16 kernels (kBf16 picks the ring depth, the operand buffer and
-// its conversion, and the wgmma form).
+// ---- fp8 operands ----
+// d[64 x 128] (+)= A[64 x 32] * B[128 x 32]^T, e4m3 operands, f32 accumulators; scale_d == 0 starts from zero
+__device__ __forceinline__ void wgmma_e4m3(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, "
+        "%47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d)
+        : "memory");
+}
+
+// The 4 wgmmas of one 128-code k-block for consumer warpgroup wg, straight from raw stage `stage` (TMA's 128-byte
+// swizzle is the K-major layout smem_desc describes).  The chain starts from zero: d holds this k-block's products only.
+__device__ __forceinline__ void mma_kblock_fp8(float (&d)[64], uint32_t stage, uint32_t wg) {
+    const uint32_t a = stage + wg * (64 * 128), b = stage + A_BYTES;
+#pragma unroll
+    for (int k = 0; k < BK_FP8 / WG_K_FP8; ++k) wgmma_e4m3(d, smem_desc(a + 32 * k), smem_desc(b + 32 * k), k);
+}
+
+// The whole pipeline, shared by the 3xTF32, the bf16 and the fp8 kernels (kPrec picks the ring depth, the operand
+// buffer and its conversion -- none for fp8 --, the wgmma form and, for fp8, the per-k-block promotion and the row
+// scales of the epilogue).
 // Persistent: gridDim.x = min(work items, SMs); a work item = (output tile, contraction slice).  All roles walk the same
 // item sequence; the raw ring and its phases run on across items.
-template <bool kMN, bool kBf16>
+template <bool kMN, int kPrec>
 __device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtensorMap &map_b, float *__restrict__ C,
                                           int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
                                           const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale,
+                                          const float *__restrict__ a_scale, const float *__restrict__ b_scale,
                                           int M, int N, int num_kb, int tiles_n, int tiles, int splits) {
-    constexpr int kStages = kBf16 ? kStagesBf : tc::kStages;
-    constexpr int OP_BYTES = kBf16 ? OP_BF_BYTES : tc::OP_BYTES;
+    constexpr bool kBf16 = kPrec == kPrecBf16, kFp8 = kPrec == kPrecFp8;
+    static_assert(!(kFp8 && kMN), "fp8 operands are K-major only");
+    constexpr int kStages = kFp8 ? kStagesFp8 : kBf16 ? kStagesBf : tc::kStages;
+    constexpr int OP_BYTES = kFp8 ? 0 : kBf16 ? OP_BF_BYTES : tc::OP_BYTES;
+    constexpr int kKb = kFp8 ? BK_FP8 : BK;             // contraction elements per k-block
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *base_ptr = smem_raw + (base - smem_u32(smem_raw));
@@ -295,7 +343,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtens
     if (threadIdx.x == 0) {
         for (int s = 0; s < kStages; ++s) {
             mbar_init(full_bar(s), 1);
-            mbar_init(empty_bar(s), 1);
+            mbar_init(empty_bar(s), kFp8 ? kConsumerThreads / 32 : 1);   // fp8: every consumer warp releases
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -323,7 +371,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtens
                     mbar_wait(empty_bar(s), ph ^ 1u);
                     mbar_expect_tx(full_bar(s), RAW_BYTES);
                     const uint32_t a_dst = base + s * RAW_BYTES, b_dst = a_dst + A_BYTES;
-                    const int kc = (kb0 + i) * BK;
+                    const int kc = (kb0 + i) * kKb;
                     if (!kMN) {
                         tma_load_2d(a_dst, &map_a, full_bar(s), kc, m_t * BM);
                         tma_load_2d(b_dst, &map_b, full_bar(s), kc, n_t * BN);
@@ -363,25 +411,43 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtens
         float acc0[64], acc1[64];
 #pragma unroll
         for (int e = 0; e < 64; ++e) acc0[e] = acc1[e] = 0.f;
-        split_kblock(g);
-        publish_kblock(g);
-        for (int i = 0; i < nkb; ++i, ++g) {
-            const uint32_t op = ops + (g & 1u) * OP_BYTES;
-            wgmma_fence();
-            if constexpr (kBf16) {
-                if (i % kAcc == 0) mma_kblock_bf16(acc0, op, wg);
-                else mma_kblock_bf16(acc1, op, wg);
-            } else {
-                if (i % kAcc == 0) mma_kblock(acc0, op, wg);
-                else mma_kblock(acc1, op, wg);
+        if constexpr (kFp8) {
+            // Each k-block's chain of 4 wgmmas starts from zero in acc0 and is added into the f32 sums acc1 on the CUDA
+            // cores: the tensor cores' fp8 accumulation never runs longer than 128 products.  A warp releases the stage
+            // once its wgmmas are complete; the stage is free when all 8 consumer warps have.
+            for (int i = 0; i < nkb; ++i, ++g) {
+                const uint32_t s = g % kStages;
+                mbar_wait(full_bar(s), (g / kStages) & 1u);
+                wgmma_fence();
+                mma_kblock_fp8(acc0, base + s * RAW_BYTES, wg);
+                wgmma_commit();
+                wgmma_wait_all();
+                if (lane == 0) mbar_arrive(empty_bar(s));
+#pragma unroll
+                for (int e = 0; e < 64; ++e) acc1[e] += acc0[e];
             }
-            wgmma_commit();
-            if (i + 1 < nkb) split_kblock(g + 1);            // CUDA cores: next k-block while the tensor cores run
-            wgmma_wait_all();
-            if (i + 1 < nkb) publish_kblock(g + 1);          // after the wait: both warpgroups' reads of buffer g are done
+        } else {
+            split_kblock(g);
+            publish_kblock(g);
+            for (int i = 0; i < nkb; ++i, ++g) {
+                const uint32_t op = ops + (g & 1u) * OP_BYTES;
+                wgmma_fence();
+                if constexpr (kBf16) {
+                    if (i % kAcc == 0) mma_kblock_bf16(acc0, op, wg);
+                    else mma_kblock_bf16(acc1, op, wg);
+                } else {
+                    if (i % kAcc == 0) mma_kblock(acc0, op, wg);
+                    else mma_kblock(acc1, op, wg);
+                }
+                wgmma_commit();
+                if (i + 1 < nkb) split_kblock(g + 1);        // CUDA cores: next k-block while the tensor cores run
+                wgmma_wait_all();
+                if (i + 1 < nkb) publish_kblock(g + 1);      // after the wait: both warpgroups' reads of buffer g are done
+            }
         }
 
-        // ===== epilogue: sum of the chains (fixed order) -> + bias -> + addend -> * row_scale -> global =====
+        // ===== epilogue: sum of the chains (fixed order) [fp8: * a_scale * b_scale] -> + bias -> + addend -> * row_scale
+        // -> global =====
         // fragment: d[4j + 2h + e] = row 16 warp + lane / 4 + 8 h, column 8 j + 2 (lane % 4) + e
         float *Cs = C + (int64_t)split_ * split_stride;
 #pragma unroll
@@ -391,10 +457,19 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap &map_a, const CUtens
             float *Cout = Cs + (int64_t)row * ldc;
             const float *Add = addend ? addend + (int64_t)row * ldadd : nullptr;
             const float rsc = row_scale ? __ldg(row_scale + row) : 1.f;
+            float sa = 1.f;
+            if constexpr (kFp8) sa = __ldg(a_scale + row);
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const int col = n_t * BN + 8 * j + 2 * (lane & 3);
-                float o[2] = {acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h], acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1]};
+                float o[2];
+                if constexpr (kFp8) {
+                    o[0] = col < N ? acc1[4 * j + 2 * h] * sa * __ldg(b_scale + col) : 0.f;
+                    o[1] = col + 1 < N ? acc1[4 * j + 2 * h + 1] * sa * __ldg(b_scale + col + 1) : 0.f;
+                } else {
+                    o[0] = acc0[4 * j + 2 * h] + acc1[4 * j + 2 * h];
+                    o[1] = acc0[4 * j + 2 * h + 1] + acc1[4 * j + 2 * h + 1];
+                }
                 if (col + 1 < N) {
                     if (bias) {
                         const float2 bb = __ldg(reinterpret_cast<const float2 *>(bias + col));
@@ -421,8 +496,8 @@ gemm3x_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
               float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
               const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
               int tiles_n, int tiles, int splits) {
-    gemm_body<kMN, false>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, M, N, num_kb, tiles_n, tiles,
-                          splits);
+    gemm_body<kMN, kPrec3xTf32>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, nullptr, nullptr, M, N,
+                                num_kb, tiles_n, tiles, splits);
 }
 
 // The same GEMM with the operands rounded to bf16 (nearest even) in shared memory: one m64n128k16 wgmma per 16
@@ -433,8 +508,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
                  float *__restrict__ C, int64_t ldc, int64_t split_stride, const float *__restrict__ bias,
                  const float *__restrict__ addend, int64_t ldadd, const float *__restrict__ row_scale, int M, int N, int num_kb,
                  int tiles_n, int tiles, int splits) {
-    gemm_body<kMN, true>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, M, N, num_kb, tiles_n, tiles,
-                         splits);
+    gemm_body<kMN, kPrecBf16>(map_a, map_b, C, ldc, split_stride, bias, addend, ldadd, row_scale, nullptr, nullptr, M, N,
+                              num_kb, tiles_n, tiles, splits);
+}
+
+// The TN GEMM on fp8 rows (bns_dense_tn_fp8): A and B are e4m3 codes with one f32 scale per row, fed by TMA straight to
+// .e4m3 wgmmas, C[m, n] = (sum_k qa[m, k] qb[n, k]) * a_scale[m] * b_scale[n], then the f32 epilogue.
+__global__ void __launch_bounds__(kThreadsTc, 1)
+gemm_fp8_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                const float *__restrict__ a_scale, const float *__restrict__ b_scale, float *__restrict__ C, int64_t ldc,
+                const float *__restrict__ bias, const float *__restrict__ addend, int64_t ldadd,
+                const float *__restrict__ row_scale, int M, int N, int num_kb, int tiles_n, int tiles) {
+    gemm_body<false, kPrecFp8>(map_a, map_b, C, ldc, 0, bias, addend, ldadd, row_scale, a_scale, b_scale, M, N, num_kb,
+                               tiles_n, tiles, 1);
 }
 
 // out[r, c] = sum_s ws[s][r, c]  in split order (deterministic); ws slices are contiguous [rows, cols].  Above
@@ -483,31 +569,33 @@ inline EncodeTiledFn encode_tiled() {
     return fn;
 }
 
-// 2-D f32 tensor map over a row-major [rows, inner] matrix with leading dimension ld (floats), SWIZZLE_128B,
-// out-of-bounds elements read as zero.
-inline int make_map(CUtensorMap *m, const float *ptr, int64_t inner, int64_t rows, int64_t ld, uint32_t box_inner,
-                    uint32_t box_rows) {
+// 2-D tensor map over a row-major [rows, inner] matrix with leading dimension ld (elements), SWIZZLE_128B, out-of-bounds
+// elements read as zero; f32 elements, or bytes (e4m3 codes) when elem_bytes == 1.
+inline int make_map(CUtensorMap *m, const void *ptr, int64_t inner, int64_t rows, int64_t ld, uint32_t box_inner,
+                    uint32_t box_rows, int elem_bytes = 4) {
     EncodeTiledFn enc = encode_tiled();
     if (!enc) return fail(BNS_E_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
     cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
+    cuuint64_t gstride[1] = {(cuuint64_t)ld * elem_bytes};
     cuuint32_t box[2] = {box_inner, box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(ptr), gdim, gstride, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = enc(m, elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                     const_cast<void *>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(BNS_E_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
     return BNS_OK;
 }
 
 inline bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-template <bool kMN, bool kBf16>
+template <bool kMN, int kPrec>
 int configure() {
     static std::atomic<int> done[kMaxDevices];      // the attribute is per function AND per device
     const int dev = current_device();
     if (!done[dev].load(std::memory_order_acquire)) {
-        if (kBf16)
+        if constexpr (kPrec == kPrecFp8)
+            BNS_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_FP8_BYTES));
+        else if (kPrec == kPrecBf16)
             BNS_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BF_BYTES));
         else
             BNS_CUDA(cudaFuncSetAttribute(gemm3x_kernel<kMN>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
@@ -531,7 +619,7 @@ int dense_tn(const char *fn, const float *A, int64_t lda, const float *B, int64_
     if (rc) return rc;
     rc = make_map(&mb, B, K, N, ldb, BK, BN);
     if (rc) return rc;
-    rc = configure<false, kBf16>();
+    rc = configure<false, kBf16 ? kPrecBf16 : kPrec3xTf32>();
     if (rc) return rc;
     const int tiles_m = (int)((M + BM - 1) / BM), tiles_n = (int)((N + BN - 1) / BN);
     const int num_kb = (int)((K + BK - 1) / BK);
@@ -545,6 +633,42 @@ int dense_tn(const char *fn, const float *A, int64_t lda, const float *B, int64_
     else
         gemm3x_kernel<false><<<grid, kThreadsTc, SMEM_BYTES, as_stream(stream)>>>(ma, mb, C, ldc, 0, bias, addend, ldadd,
                                                                                 row_scale, (int)M, (int)N, num_kb, tiles_n, tiles, 1);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// C[M, N] = (qa[M, K] qb[N, K]^T * a_scale[M] * b_scale[N]) (+ bias[N]) (+ addend[M, N]) (* row_scale[M]): A and B
+// are e4m3 code rows (lda / ldb in bytes) with one f32 scale per row.  The tensor maps' inner dimension is K, so TMA
+// zero-fills the contraction tail and never reads the bytes between K and lda / ldb.
+inline int dense_tn_fp8(const uint8_t *A, int64_t lda, const float *a_scale, const uint8_t *B, int64_t ldb,
+                        const float *b_scale, const float *bias, const float *addend, int64_t ldadd, const float *row_scale,
+                        float *C, int64_t ldc, int64_t M, int64_t N, int64_t K, void *stream) {
+    const char *fn = "bns_dense_tn_fp8";
+    BNS_REQUIRE(A && B && C && a_scale && b_scale, "%s: NULL argument", fn);
+    BNS_REQUIRE(M > 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "%s: bad shape", fn);
+    BNS_REQUIRE(lda >= K && ldb >= K && ldc >= N, "%s: leading dimension smaller than the row", fn);
+    BNS_REQUIRE(lda % 16 == 0 && ldb % 16 == 0 && ldc % 4 == 0 && aligned16(A) && aligned16(B) && aligned16(C) &&
+                    (reinterpret_cast<uintptr_t>(a_scale) & 3u) == 0 && (reinterpret_cast<uintptr_t>(b_scale) & 3u) == 0 &&
+                    (!bias || aligned16(bias)) && (!addend || (aligned16(addend) && ldadd % 4 == 0 && ldadd >= N)),
+                "%s: code rows must be 16-byte aligned with leading dimensions that are multiples of 16 bytes, the f32 "
+                "operands 16-byte aligned with leading dimensions that are multiples of 4", fn);
+    CUtensorMap ma, mb;
+    int rc = make_map(&ma, A, K, M, lda, BK_FP8, BM, 1);
+    if (rc) return rc;
+    rc = make_map(&mb, B, K, N, ldb, BK_FP8, BN, 1);
+    if (rc) return rc;
+    rc = configure<false, kPrecFp8>();
+    if (rc) return rc;
+    const int tiles_m = (int)((M + BM - 1) / BM), tiles_n = (int)((N + BN - 1) / BN);
+    const int num_kb = (int)((K + BK_FP8 - 1) / BK_FP8);
+    const int64_t tiles64 = tiles_m * (int64_t)tiles_n;
+    BNS_REQUIRE(tiles64 < (1ll << 31), "%s: too many tiles", fn);
+    const int tiles = (int)tiles64;
+    dim3 grid((unsigned)(tiles < sm_count() ? tiles : sm_count()), 1, 1);
+    gemm_fp8_kernel<<<grid, kThreadsTc, SMEM_FP8_BYTES, as_stream(stream)>>>(ma, mb, a_scale, b_scale, C, ldc, bias, addend,
+                                                                            ldadd, row_scale, (int)M, (int)N, num_kb,
+                                                                            tiles_n, tiles);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -596,7 +720,7 @@ int dense_nt(const char *fn, const float *A, int64_t lda, const float *B, int64_
     if (rc) return rc;
     rc = make_map(&mb, B, N2, R, ldb, 32, BK);
     if (rc) return rc;
-    rc = configure<true, kBf16>();
+    rc = configure<true, kBf16 ? kPrecBf16 : kPrec3xTf32>();
     if (rc) return rc;
     const int tiles_m = (int)((N1 + BM - 1) / BM), tiles_n = (int)((N2 + BN - 1) / BN);
     const int num_kb = (int)((R + BK - 1) / BK);
@@ -653,4 +777,10 @@ extern "C" int bns_dense_nt_3xtf32(const float *A, int64_t lda, const float *B, 
 extern "C" int bns_dense_nt_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, float *C, int64_t ldc,
                                  int64_t R, int64_t N1, int64_t N2, void *ws, size_t ws_bytes, void *stream) {
     return tc::dense_nt<true>("bns_dense_nt_bf16", A, lda, B, ldb, C, ldc, R, N1, N2, ws, ws_bytes, stream);
+}
+
+extern "C" int bns_dense_tn_fp8(const uint8_t *A, int64_t lda, const float *a_scale, const uint8_t *B, int64_t ldb,
+                                const float *b_scale, const float *bias, const float *addend, int64_t ldadd,
+                                const float *row_scale, float *C, int64_t ldc, int64_t M, int64_t N, int64_t K, void *stream) {
+    return tc::dense_tn_fp8(A, lda, a_scale, B, ldb, b_scale, bias, addend, ldadd, row_scale, C, ldc, M, N, K, stream);
 }

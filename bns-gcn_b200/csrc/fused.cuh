@@ -184,6 +184,15 @@ __global__ void __launch_bounds__(256) derive_kernel(const bns_derive_entry *__r
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < e.rows; i += gridDim.x * blockDim.x) e.dst[i] = e.a[i] + e.b[i];
         return;
     }
+    if (e.op == 2 || e.op == 3) {                                   // fp8 rows of a (op 2) or of a^T (op 3), a warp per row
+        uint8_t *codes = reinterpret_cast<uint8_t *>(e.dst);
+        float *scale = reinterpret_cast<float *>(codes + (int64_t)e.rows * e.ld_dst);
+        for (int r = blockIdx.x * 8 + (threadIdx.x >> 5); r < e.rows; r += gridDim.x * 8) {
+            const float *x = e.op == 2 ? e.a + (int64_t)r * e.ld_a : e.a + r;
+            fp8_row_any(x, e.op == 2 ? 1 : e.ld_a, e.cols, codes + (int64_t)r * e.ld_dst, scale + r, threadIdx.x & 31);
+        }
+        return;
+    }
     const int tiles_c = (e.cols + 31) / 32, tiles_r = (e.rows + 31) / 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;        // 32 x 8
     for (int t = blockIdx.x; t < tiles_c * tiles_r; t += gridDim.x) {
@@ -250,6 +259,21 @@ extern "C" int bns_derive_refresh(const void *table_dev, int32_t n_entries, int6
 // =====================================================================================================================
 namespace {
 
+// By one warp: row `row` of dropout_p, y[0:F] = x[0:F] masked and scaled -- the one statement of the layer-0 input
+// dropout that dropout_kernel and dropout_fp8_kernel share, so that their kept values are the same bits.
+__device__ __forceinline__ void dropout_row(const float *__restrict__ x, float *__restrict__ y, int64_t row, int32_t F,
+                                            float p, float keep_scale, uint64_t seed, uint64_t offset, int lane) {
+    for (int vec = lane; vec * 4 < F; vec += 32) {
+        const float4 v = *reinterpret_cast<const float4 *>(x + vec * 4);
+        bool keep[4];
+        drop_mask4(seed, offset, row, vec, p, keep);
+        float4 o;
+        o.x = keep[0] ? v.x * keep_scale : 0.f; o.y = keep[1] ? v.y * keep_scale : 0.f;
+        o.z = keep[2] ? v.z * keep_scale : 0.f; o.w = keep[3] ? v.w * keep_scale : 0.f;
+        *reinterpret_cast<float4 *>(y + vec * 4) = o;
+    }
+}
+
 __global__ void __launch_bounds__(kThreads) dropout_kernel(const float *__restrict__ x, int64_t ldx, int64_t n, int32_t F,
                                                            float p, float keep_scale, uint64_t seed, uint64_t offset,
                                                            const uint64_t *__restrict__ offset_dev, float *__restrict__ y,
@@ -258,15 +282,23 @@ __global__ void __launch_bounds__(kThreads) dropout_kernel(const float *__restri
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
     for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < n; row += warps_total) {
-        for (int vec = lane; vec * 4 < F; vec += 32) {
-            const float4 v = *reinterpret_cast<const float4 *>(x + row * ldx + vec * 4);
-            bool keep[4];
-            drop_mask4(seed, offset, row, vec, p, keep);
-            float4 o;
-            o.x = keep[0] ? v.x * keep_scale : 0.f; o.y = keep[1] ? v.y * keep_scale : 0.f;
-            o.z = keep[2] ? v.z * keep_scale : 0.f; o.w = keep[3] ? v.w * keep_scale : 0.f;
-            *reinterpret_cast<float4 *>(y + row * ldy + vec * 4) = o;
-        }
+        dropout_row(x + row * ldx, y + row * ldy, row, F, p, keep_scale, seed, offset, lane);
+    }
+}
+
+// dropout_kernel's rows, each also stored as an fp8 row (Fp8Row) of the dropped values; one warp per row, so the codes
+// pass re-reads the values this lane just stored.
+__global__ void __launch_bounds__(kThreads) dropout_fp8_kernel(const float *__restrict__ x, int64_t ldx, int64_t n, int32_t F,
+                                                               float p, float keep_scale, uint64_t seed, uint64_t offset,
+                                                               const uint64_t *__restrict__ offset_dev, float *y, int64_t ldy,
+                                                               uint8_t *__restrict__ codes, int64_t ldc,
+                                                               float *__restrict__ scale) {
+    if (offset_dev) offset += *offset_dev;
+    const int lane = threadIdx.x & 31;
+    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+    for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < n; row += warps_total) {
+        dropout_row(x + row * ldx, y + row * ldy, row, F, p, keep_scale, seed, offset, lane);
+        fp8_row_any(y + row * ldy, 1, F, codes + row * ldc, scale + row, lane);
     }
 }
 
@@ -300,6 +332,23 @@ extern "C" int bns_dropout_f32(const float *x, int64_t ldx, int64_t n, int64_t F
     BNS_REQUIRE(p >= 0.f && p < 1.f, "bns_dropout_f32: p must be in [0, 1)");
     dropout_kernel<<<ln_grid(n), kThreads, 0, as_stream(stream)>>>(x, ldx, n, (int32_t)F, p, 1.f / (1.f - p), seed, offset,
                                                                    offset_dev, y, ldy);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_dropout_fp8(const float *x, int64_t ldx, int64_t n, int64_t F, float p, uint64_t seed, uint64_t offset,
+                               const uint64_t *offset_dev, float *y, int64_t ldy, uint8_t *codes, int64_t ldc, float *scale,
+                               void *stream) {
+    BNS_REQUIRE(n >= 0 && F > 0 && F % 4 == 0 && F < (1 << 24), "bns_dropout_fp8: need F %% 4 == 0");
+    if (n == 0) return BNS_OK;
+    BNS_REQUIRE(x && y && codes && scale && ldx >= F && ldy >= F && ldc >= F && ldx % 4 == 0 && ldy % 4 == 0 &&
+                    ldc % 16 == 0, "bns_dropout_fp8: bad pointer / leading dimension");
+    BNS_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(codes)) & 15u) == 0 &&
+                    (reinterpret_cast<uintptr_t>(scale) & 3u) == 0, "bns_dropout_fp8: unaligned");
+    BNS_REQUIRE(p >= 0.f && p < 1.f, "bns_dropout_fp8: p must be in [0, 1)");
+    dropout_fp8_kernel<<<ln_grid(n), kThreads, 0, as_stream(stream)>>>(x, ldx, n, (int32_t)F, p, 1.f / (1.f - p), seed, offset,
+                                                                       offset_dev, y, ldy, codes, ldc, scale);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

@@ -91,6 +91,9 @@ class ParamArena:
         # --dense-dtype bf16: every GEMM of the fused layers rounds its operands to bf16 inside the kernel (f32 sums);
         # per run, never global: ranks that are threads of one process may differ
         self.dense_bf16 = False
+        # --dense-dtype fp8: the forward and input-gradient GEMMs (TN) take fp8 rows of both operands (the weights' as
+        # derived parameters, ``fp8_rows``); the weight gradients (NT) take the bf16 products.  Per run, as dense_bf16
+        self.dense_fp8 = False
 
     def __deepcopy__(self, memo):
         """A copied model (evaluate.py's snapshots) owns plain parameter tensors and takes the op-by-op path."""
@@ -151,6 +154,25 @@ class ParamArena:
         e = DeriveEntry()
         e.op, e.rows, e.cols, e.ld_a, e.ld_dst = 1, x.numel(), 1, 1, 1
         e.a, e.b, e.dst = x.data_ptr(), y.data_ptr(), out.data_ptr()
+        return self._add(key, e, out)
+
+    def fp8_rows(self, p: torch.nn.Parameter, transposed: bool = False) -> ops.Fp8Rows:
+        """The fp8 rows (``ops.cvt_rows_fp8``'s rule) of ``padded(p)``, the B operand of the forward GEMMs under
+        ``--dense-dtype fp8``, or (``transposed``) of ``transposed(p)``, the input gradients'.  Codes and scales share one
+        allocation; refreshed with the other derived parameters after every optimizer step (a pad row: zero codes)."""
+        key = ("QT" if transposed else "Q", id(p))
+        hit = self._derived.get(key)
+        if hit is not None:
+            return hit
+        w = self.padded(p)
+        rows, k = (w.shape[1], w.shape[0]) if transposed else (w.shape[0], w.shape[1])
+        ld = (k + 15) // 16 * 16
+        buf = torch.zeros(rows * ld + 4 * rows, dtype=torch.uint8, device=self.device)
+        out = ops.Fp8Rows(buf[:rows * ld].view(rows, ld)[:, :k].view(torch.float8_e4m3fn),
+                          buf[rows * ld:].view(torch.float32))
+        e = DeriveEntry()
+        e.op, e.rows, e.cols, e.ld_a, e.ld_dst = 3 if transposed else 2, rows, k, w.stride(0), ld
+        e.a, e.b, e.dst = w.data_ptr(), None, buf.data_ptr()
         return self._add(key, e, out)
 
     def refresh(self, advance: Optional[torch.Tensor]) -> None:
@@ -276,6 +298,23 @@ def dropout(x: torch.Tensor, p: float, seed: int) -> torch.Tensor:
     return y
 
 
+def dropout_fp8(x: torch.Tensor, p: float, seed: int):
+    """``(dropout(x, p, seed), its fp8 rows)`` in one pass (``bns_dropout_fp8``: the same mask and kept values, bit
+    for bit); ``p == 0``: ``x`` and ``ops.cvt_rows_fp8_any(x)``."""
+    if p <= 0.0:
+        return x, ops.cvt_rows_fp8_any(x)
+    x = x.contiguous()
+    y = torch.empty_like(x)
+    q = ops._fp8_rows_like(x.shape[0], x.shape[1], x.device)
+    off, off_dev = ops.RNG["offset"], ops.RNG["offset_dev"]
+    with torch.cuda.device(x.device):
+        check(lib.bns_dropout_fp8(x.data_ptr(), x.stride(0), x.shape[0], x.shape[1], float(p), seed & (2 ** 64 - 1),
+                                  off & (2 ** 64 - 1), ops._ptr(off_dev), y.data_ptr(), y.stride(0), q.codes.data_ptr(),
+                                  q.codes.stride(0), q.scale.data_ptr(), torch.cuda.current_stream(x.device).cuda_stream),
+              "bns_dropout_fp8")
+    return y, q
+
+
 class DropoutFn(torch.autograd.Function):
     """``dropout_p`` as an autograd node on ``bns_dropout_f32``: the backward regenerates the Philox mask of the forward
     (same seed, same epoch offset) instead of storing it."""
@@ -321,14 +360,40 @@ def dropout_supported(x: torch.Tensor) -> bool:
 
 
 # ---- layer functions ---------------------------------------------------------------------------------------------------
+def _q(a: ParamArena, x: torch.Tensor, rows=None):
+    """``x`` as the A operand of ``_tn``: ``x`` itself, or under ``--dense-dtype fp8`` its fp8 rows (made once per
+    operand and step, however many products use them).  ``rows``: the same rows as they arrived, when the exchange
+    sent them as fp8 rows (``--comm-dtype fp8``): taken as they are, the same values by the same rule."""
+    if not a.dense_fp8:
+        return x
+    return rows if isinstance(rows, ops.Fp8Rows) else ops.cvt_rows_fp8_any(x)
+
+
+def _tn(a: ParamArena, x, p: torch.nn.Parameter, bias=None, addend=None, row_scale=None, out=None, t: bool = False):
+    """``x @ padded(p)^T`` (``t``: ``x @ transposed(p)^T``, the input gradient) in the arena's dense mode, with the
+    epilogue of ``dense.tc_mm_tn``; ``x`` comes from ``_q``."""
+    if a.dense_fp8:
+        return dense.tc_mm_tn_fp8(x, a.fp8_rows(p, t), bias, addend, row_scale, out)
+    return dense.tc_mm_tn(x, a.transposed(p) if t else a.padded(p), bias, addend, row_scale, out, bf16=a.dense_bf16)
+
+
+def _nt_bf16(a: ParamArena) -> bool:
+    """Whether the weight gradients take the bf16 products: ``--dense-dtype bf16`` and ``fp8`` (a per-row scale does
+    not factor out of a contraction over the nodes)."""
+    return a.dense_bf16 or a.dense_fp8
+
+
 class PPLinearFn(torch.autograd.Function):
     """``dropout(x) @ W^T + b`` for the precomputed layer 0 (module/layer.py:29-30, 82-83 after module/model.py:45/80).
     The parameters are inputs only so that autograd records the node; their gradients are written into the arena."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, arena: ParamArena, p: float, seed: int):
-        xd = dropout(x, p, seed)
-        y = dense.tc_mm_tn(xd, arena.padded(weight), None if bias is None else arena.padded(bias), bf16=arena.dense_bf16)
+        if arena.dense_fp8:
+            xd, xq = dropout_fp8(x, p, seed)
+        else:
+            xd = xq = dropout(x, p, seed)
+        y = _tn(arena, xq, weight, None if bias is None else arena.padded(bias))
         ctx.save_for_backward(xd)
         ctx.arena, ctx.weight, ctx.bias, ctx.p, ctx.seed = arena, weight, bias, p, seed
         ctx.rng = (ops.RNG["seed"], ops.RNG["offset"], ops.RNG["offset_dev"])
@@ -341,10 +406,10 @@ class PPLinearFn(torch.autograd.Function):
         dy = dy.contiguous()
         if ctx.bias is not None:
             dense.colsum(dy, out=a.grad_padded(ctx.bias))
-        dense.tc_mm_nt(dy, xd, out=a.grad_padded(ctx.weight), bf16=a.dense_bf16)
+        dense.tc_mm_nt(dy, xd, out=a.grad_padded(ctx.weight), bf16=_nt_bf16(a))
         dx = None
         if ctx.needs_input_grad[0]:
-            dx = dense.tc_mm_tn(dy, a.transposed(ctx.weight), bf16=a.dense_bf16)
+            dx = _tn(a, _q(a, dy), ctx.weight, t=True)
             if ctx.p > 0.0:                     # d dropout: the same mask, regenerated
                 keep = ops.RNG["seed"], ops.RNG["offset"], ops.RNG["offset_dev"]
                 ops.RNG.update(seed=ctx.rng[0], offset=ctx.rng[1], offset_dev=ctx.rng[2])
@@ -367,12 +432,13 @@ def _gather_table(x: torch.Tensor, mode):
 
 
 def _aggregate(g: PartitionGraph, x_u: torch.Tensor, rs: torch.Tensor, ready, bf16: bool = False,
-               halo: Optional[torch.Tensor] = None) -> torch.Tensor:
+               halo: Optional[torch.Tensor] = None, inner=None) -> torch.Tensor:
     """``rs * (A_in x_u[:n_in] + A_out[:, sampled] x_u[n_in:])`` -- the inner pass first (it needs local rows only), the
     halo pass after the exchange's event.  ``bf16``: the ``_gather_table`` mode of both passes (f32 sums).  ``halo``:
     the halo rows as they arrived, bf16 or an ``ops.Fp8Rows`` table (``--comm-dtype bf16`` / ``fp8``; ``x_u`` is then
-    the inner rows alone), gathered as they are, whatever the mode."""
-    y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16), row_scale=rs)
+    the inner rows alone), gathered as they are, whatever the mode.  ``inner``: the inner pass's table when the caller
+    already made it."""
+    y = ops.spmm_auto(g.a_in, _gather_table(x_u[:g.n_in], bf16) if inner is None else inner, row_scale=rs)
     if ready is not None:
         torch.cuda.current_stream(x_u.device).wait_event(ready)
     if halo is not None:
@@ -443,28 +509,30 @@ class SageConvFn(torch.autograd.Function):
         ctx.exchange, ctx.inner_only = exchange, halo is not None
         n_in = g.n_in
         h_u = h_u.contiguous()
-        W1, W2 = arena.padded(w1), arena.padded(w2)
-        bf = arena.dense_bf16
         h_in = h_u[:n_in]
         if narrow_first:
             # transform, then aggregate; the local rows go first -- their GEMM and the inner-edge pass need nothing from
             # the peers and hide the exchange -- the halo rows after the exchange's event
             n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
-            t = gather_friendly(n_u, W2.shape[0], h_u.device)                   # [n_u, out_p]
-            dense.tc_mm_tn(h_in, W2, out=t[:n_in], bf16=bf)
-            out = dense.tc_mm_tn(h_in, W1, arena.bias_sum(b1, b2), bf16=bf)     # linear1(h) + b1 + b2 ...
+            t = gather_friendly(n_u, arena.padded(w2).shape[0], h_u.device)    # [n_u, out_p]
+            hq = _q(arena, h_in)
+            _tn(arena, hq, w2, out=t[:n_in])
+            out = _tn(arena, hq, w1, arena.bias_sum(b1, b2))                    # linear1(h) + b1 + b2 ...
             ops.spmm_auto(g.a_in, t[:n_in], out, row_scale=rs, accumulate=True)  # ... + (A_in t) / deg
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             h_halo = _halo_rows(h_u, n_in, halo)
             if g.a_out is not None and n_u > n_in:
-                dense.tc_mm_tn(h_halo, W2, out=t[n_in:], bf16=bf)
+                _tn(arena, _q(arena, h_halo, halo), w2, out=t[n_in:])
                 halo_aggregate(g, t[n_in:], out, rs, None)                      # ... + (A_out t_halo) / deg
             ctx.save_for_backward(*((h_u,) if halo is None else (h_in, h_halo)))
         else:
-            ah = _aggregate(g, h_u, rs, ready, _agg_mode(g), halo)              # [n_in, in]
-            t = dense.tc_mm_tn(ah, W2, arena.padded(b2), bf16=bf)
-            out = dense.tc_mm_tn(h_in, W1, arena.padded(b1), addend=t, bf16=bf)
+            mode = _agg_mode(g)
+            # --dense-dtype fp8 with --agg-dtype fp8: linear1 takes the inner pass's fp8 table (the same rule, same rows)
+            inner = _gather_table(h_in, mode) if arena.dense_fp8 and mode == 'fp8' else None
+            ah = _aggregate(g, h_u, rs, ready, mode, halo, inner)               # [n_in, in]
+            t = _tn(arena, _q(arena, ah), w2, arena.padded(b2))
+            out = _tn(arena, _q(arena, h_in) if inner is None else inner, w1, arena.padded(b1), addend=t)
             ctx.save_for_backward(h_u, ah)
         ctx.n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
         ctx.g, ctx.rs, ctx.arena, ctx.narrow = g, rs, arena, narrow_first
@@ -476,8 +544,9 @@ class SageConvFn(torch.autograd.Function):
         g, rs, a = ctx.g, ctx.rs, ctx.arena
         w1, b1, w2, b2 = ctx.params
         n_in = g.n_in
-        bf = a.dense_bf16
+        bf = _nt_bf16(a)
         dout = dout.contiguous()
+        dq = _q(a, dout)
         dense.colsum(dout, out=a.grad_padded(b1), out2=a.grad_padded(b2))
         begin = None
         if ctx.exchange is not None:
@@ -488,22 +557,23 @@ class SageConvFn(torch.autograd.Function):
             h_in, n_u = saved[0][:n_in], ctx.n_u
             dys = scale_rows(dout, rs, out=gather_friendly(n_in, dout.shape[1], dout.device))
             dt = _aggregate_t(g, dys, n_u)                                      # [n_u, out_p]
+            dtq = _q(a, dt)
             du = torch.empty(n_u, h_in.shape[1], dtype=torch.float32, device=dout.device)
             if n_u > n_in:                                                      # halo rows first: they travel ...
-                dense.tc_mm_tn(dt[n_in:], a.transposed(w2), out=du[n_in:], bf16=bf)
+                _tn(a, dtq[n_in:], w2, out=du[n_in:], t=True)
             if begin is not None:
                 begin(du)
-            dense.tc_mm_tn(dt[:n_in], a.transposed(w2), out=du[:n_in], bf16=bf)  # ... while the local rows are computed
+            _tn(a, dtq[:n_in], w2, out=du[:n_in], t=True)                       # ... while the local rows are computed
             dense.tc_mm_nt(dout, h_in, out=a.grad_padded(w1), bf16=bf)
             _weight_grad(dt, saved, n_in, a.grad_padded(w2), bf)
         else:
             h_u, ah = ctx.saved_tensors
-            dys = dense.tc_mm_tn(dout, a.transposed(w2), row_scale=rs, bf16=bf)  # (dout W2) / deg
+            dys = _tn(a, dq, w2, row_scale=rs, t=True)                          # (dout W2) / deg
             du = _aggregate_t(g, dys, ctx.n_u, after_halo=begin, bf16=_agg_mode(g))
             dense.tc_mm_nt(dout, h_u[:n_in], out=a.grad_padded(w1), bf16=bf)
             dense.tc_mm_nt(dout, ah, out=a.grad_padded(w2), bf16=bf)
         inner = du[:n_in]
-        dense.tc_mm_tn(dout, a.transposed(w1), addend=inner, out=inner, bf16=bf)  # += dout W1, in place
+        _tn(a, dq, w1, addend=inner, out=inner, t=True)                         # += dout W1, in place
         return inner if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None, None
 
 
@@ -524,20 +594,19 @@ class GcnConvFn(torch.autograd.Function):
         n_in = g.n_in
         h_u = h_u.contiguous()
         W, bp = arena.padded(w), arena.padded(b)
-        bf = arena.dense_bf16
         cs_in, cs_halo = cs_u[:n_in], cs_u[n_in:]
         n_u = h_u.shape[0] if halo is None else n_in + halo.shape[0]
         has_halo = g.a_out is not None and n_u > n_in
         if narrow_first:
             t = gather_friendly(n_u, W.shape[0], h_u.device)                                          # [n_u, out_p]
-            dense.tc_mm_tn(h_u[:n_in], W, out=t[:n_in], bf16=bf)                                      # local rows first
+            _tn(arena, _q(arena, h_u[:n_in]), w, out=t[:n_in])                                      # local rows first
             ts = scale_rows(t[:n_in], cs_in, out=gather_friendly(n_in, W.shape[0], h_u.device))
             s = ops.spmm_auto(g.a_in, ts)                                                             # raw sums
             if ready is not None:
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             h_halo = _halo_rows(h_u, n_in, halo)
             if has_halo:
-                dense.tc_mm_tn(h_halo, W, out=t[n_in:], bf16=bf)
+                _tn(arena, _q(arena, h_halo, halo), w, out=t[n_in:])
                 halo_aggregate(g, t[n_in:], s, None, cs_halo)
             out = scale_rows(s, rs, bias=bp)                                                          # / in_norm + b
             ctx.save_for_backward(*((h_u,) if halo is None else (h_u[:n_in], h_halo)))
@@ -548,7 +617,7 @@ class GcnConvFn(torch.autograd.Function):
                 torch.cuda.current_stream(h_u.device).wait_event(ready)
             if has_halo:
                 halo_aggregate(g, halo if halo is not None else _gather_table(h_u[n_in:], bf16), y, rs, cs_halo)
-            out = dense.tc_mm_tn(y, W, bp, bf16=bf)
+            out = _tn(arena, _q(arena, y), w, bp)
             ctx.save_for_backward(y)
         ctx.n_u = n_u
         ctx.g, ctx.rs, ctx.cs, ctx.arena, ctx.narrow, ctx.params = g, rs, (cs_in, cs_halo), arena, narrow_first, (w, b)
@@ -559,7 +628,7 @@ class GcnConvFn(torch.autograd.Function):
         g, rs, a = ctx.g, ctx.rs, ctx.arena
         cs_in, cs_halo = ctx.cs
         w, b = ctx.params
-        bf = a.dense_bf16
+        bf = _nt_bf16(a)
         dout = dout.contiguous()
         dense.colsum(dout, out=a.grad_padded(b))
         begin = None
@@ -570,13 +639,13 @@ class GcnConvFn(torch.autograd.Function):
             dys = scale_rows(dout, rs, out=gather_friendly(g.n_in, dout.shape[1], dout.device))
             dt = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo)                  # [n_u, out_p]
             _weight_grad(dt, ctx.saved_tensors, g.n_in, a.grad_padded(w), bf)
-            du = dense.tc_mm_tn(dt, a.transposed(w), bf16=bf)                   # [n_u, in]
+            du = _tn(a, _q(a, dt), w, t=True)                                   # [n_u, in]
             if begin is not None:
                 begin(du)
         else:
             (y,) = ctx.saved_tensors
             dense.tc_mm_nt(dout, y, out=a.grad_padded(w), bf16=bf)
-            dys = dense.tc_mm_tn(dout, a.transposed(w), row_scale=rs, bf16=bf)  # (dout W) / in_norm
+            dys = _tn(a, _q(a, dout), w, row_scale=rs, t=True)                  # (dout W) / in_norm
             du = _aggregate_t(g, dys, ctx.n_u, cs_in, cs_halo, after_halo=begin, bf16=_agg_mode(g))
         return du[:g.n_in] if ctx.inner_only else du, None, None, None, None, None, None, None, None, None, None
 

@@ -80,13 +80,17 @@ def build_parser():
                              "sends each such row as e4m3 codes plus one power-of-two scale (the --agg-dtype fp8 row "
                              "format): F + 4 bytes a row; the hidden width must be a multiple of 16.  Only with the "
                              "fused training step (GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
-    parser.add_argument(*_spellings("dense-dtype"), default="f32", choices=["f32", "bf16"],
+    parser.add_argument(*_spellings("dense-dtype"), default="f32", choices=["f32", "bf16", "fp8"],
                         help="NEW: operand precision of the training step's dense layers.  f32 runs the f32-accurate "
                              "3xTF32 tensor-core scheme; bf16 rounds every GEMM operand to bf16 (nearest even) inside "
                              "the kernel and sums in f32: one bf16 tensor-core product instead of three TF32 ones, and "
-                             "results that no longer match the reference to 1e-4.  Master weights, gradients, the "
-                             "all-reduce, Adam, the loss and evaluation stay f32.  Only with the fused training step "
-                             "(GraphSAGE / GCN, --use-pp, --norm layer, no --n-linear)")
+                             "results that no longer match the reference to 1e-4.  fp8 feeds the forward and "
+                             "input-gradient GEMMs with fp8 rows of both operands (e4m3 codes plus one power-of-two "
+                             "scale per row, the --agg-dtype fp8 format; sums promoted to f32 every 128 products); the "
+                             "weight gradients run the bf16 products, because their contraction runs over the nodes, "
+                             "where a per-row scale does not factor out.  Master weights, gradients, the all-reduce, "
+                             "Adam, the loss and evaluation stay f32.  Only with the fused training step (GraphSAGE / "
+                             "GCN, --use-pp, --norm layer, no --n-linear)")
     parser.add_argument(*_spellings("save-state-every"), type=int, default=0,
                         help="NEW: after every N-th epoch, and after the last one, all ranks write the training state "
                              "(weights, Adam moments and step, the CUDA generators, the evaluator's best model, the "

@@ -199,6 +199,36 @@ def tc_mm_tn(a: torch.Tensor, b: torch.Tensor, bias=None, addend=None, row_scale
     return out
 
 
+def tc_mm_tn_fp8(a, b, bias=None, addend=None, row_scale=None, out=None) -> torch.Tensor:
+    """``tc_mm_tn`` on fp8 rows (``ops.Fp8Rows``, a [M, K], b [N, K]; ``bns_dense_tn_fp8``, ``--dense-dtype fp8``):
+    ``(sum_k qa qb) * a.scale[:, None] * b.scale[None, :]``, the sums of each 128-code block promoted to f32, then the
+    same f32 epilogue (bias, addend -- which ``out`` may alias --, row_scale)."""
+    from .. import ops
+    from .._lib import check, lib
+    ops._table(a, "a")
+    ops._table(b, "b")
+    M, K = a.shape
+    N = b.shape[0]
+    if b.shape[1] != K:
+        raise ValueError(f"tc_mm_tn_fp8: a has {K} columns, b {b.shape[1]}")
+    if out is None:
+        out = torch.empty((M, N), dtype=torch.float32, device=a.device)
+    prof = PROFILE
+    if prof is not None:
+        ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        ev0.record(torch.cuda.current_stream(a.device))
+    with torch.cuda.device(a.device):
+        check(lib.bns_dense_tn_fp8(a.codes.data_ptr(), a.codes.stride(0), a.scale.data_ptr(), b.codes.data_ptr(),
+                                   b.codes.stride(0), b.scale.data_ptr(), None if bias is None else bias.data_ptr(),
+                                   None if addend is None else addend.data_ptr(), 0 if addend is None else addend.stride(0),
+                                   None if row_scale is None else row_scale.data_ptr(), out.data_ptr(), out.stride(0), M, N,
+                                   K, torch.cuda.current_stream().cuda_stream), "bns_dense_tn_fp8")
+    if prof is not None:
+        ev1.record(torch.cuda.current_stream(a.device))
+        prof.append((ev0, ev1, 2.0 * M * N * K, M * K + N * K + 4.0 * (M + N + M * N * (2 if addend is not None else 1))))
+    return out
+
+
 _WS = {}
 
 

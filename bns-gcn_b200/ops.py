@@ -496,6 +496,27 @@ def cvt_rows_fp8(src: torch.Tensor, out: Optional[Fp8Rows] = None) -> Fp8Rows:
     return out
 
 
+def _fp8_rows_like(n: int, F: int, device) -> Fp8Rows:
+    """An uninitialised ``Fp8Rows`` of ``n`` rows of ``F`` codes, each code row 16-byte aligned."""
+    return Fp8Rows(torch.empty(n, (F + 15) // 16 * 16, dtype=torch.float8_e4m3fn, device=device)[:, :F],
+                   torch.empty(n, dtype=torch.float32, device=device))
+
+
+def cvt_rows_fp8_any(src: torch.Tensor) -> Fp8Rows:
+    """``bns_cvt_rows_f32_fp8_any``: ``cvt_rows_fp8`` (the same rule, bit for bit) for rows of any width ``F % 4 == 0``
+    -- the GEMM operands of ``--dense-dtype fp8`` (K = 1204 or 44).  ``src``: 16-byte aligned, row stride a multiple
+    of 4."""
+    _req(src, torch.float32, "src")
+    if src.dim() != 2 or src.stride(1) != 1:
+        raise _lib.BnsError("src must be a row-major 2-D tensor")
+    n, F = src.shape
+    out = _fp8_rows_like(n, F, src.device)
+    with torch.cuda.device(src.device):
+        check(lib.bns_cvt_rows_f32_fp8_any(src.data_ptr(), src.stride(0), out.codes.data_ptr(), out.codes.stride(0),
+                                           out.scale.data_ptr(), n, F, _stream_ptr()), "bns_cvt_rows_f32_fp8_any")
+    return out
+
+
 def cvt_rows_f32(src: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``bns_cvt_rows_bf16_f32``: bf16 rows widened to f32 (exact), into ``out`` or a new ``[rows, F]`` matrix.  An
     ``Fp8Rows`` ``src`` (``bns_cvt_rows_fp8_f32``) gives its codes times their scales (exact)."""

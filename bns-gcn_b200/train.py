@@ -401,7 +401,7 @@ def _exchanged_x16(args, layer_size):
 _DTYPE_FLAGS = {
     'agg': (False, {'bf16': (_hidden_x8, True), 'fp8': (_hidden_x16, 'fp8')}),
     'comm': ('f32', {'bf16': (_exchanged_x8, 'bf16'), 'fp8': (_exchanged_x16, 'fp8')}),
-    'dense': (False, {'bf16': (None, True)}),
+    'dense': (False, {'bf16': (None, True), 'fp8': (None, 'fp8')}),
 }
 
 
@@ -435,9 +435,11 @@ def check_comm_dtype(args, layer_size, dev) -> str:
     return _check_dtype_flag('comm', args, layer_size, dev)
 
 
-def check_dense_dtype(args, layer_size, dev) -> bool:
-    """Whether ``--dense-dtype bf16`` is on: every GEMM of the fused layers (forward, input and weight gradients) takes
-    its operands rounded to bf16 inside the kernel, with f32 sums."""
+def check_dense_dtype(args, layer_size, dev):
+    """``False`` for f32; ``True`` for ``--dense-dtype bf16`` (every GEMM of the fused layers -- forward, input and
+    weight gradients -- takes its operands rounded to bf16 inside the kernel, with f32 sums); ``'fp8'`` for
+    ``--dense-dtype fp8`` (the forward and input-gradient GEMMs take fp8 rows of both operands, the weight gradients the
+    bf16 products).  No width rule of its own: the fp8 operands' code rows are padded to 16 bytes."""
     return _check_dtype_flag('dense', args, layer_size, dev)
 
 
@@ -454,7 +456,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     agg = check_agg_dtype(args, layer_size, dev)
     part.agg_bf16, part.agg_fp8 = agg is True, agg == 'fp8'
     comm_dtype = check_comm_dtype(args, layer_size, dev)
-    dense_bf16 = check_dense_dtype(args, layer_size, dev)
+    dense = check_dense_dtype(args, layer_size, dev)
     _, _, _, node_dict, boundary = move_to_cuda(graph, in_graph, out_graph, node_dict, boundary, dev)
     print(f'Process {rank} has {graph.num_nodes()} nodes, {graph.num_edges()} edges '
           f'{in_graph.n_rows} inner nodes, and {in_graph.nnz} inner edges.')
@@ -473,7 +475,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     if _fused_eligible(args, layer_size, dev):
         from . import fused
         arena = fused.ParamArena(model)
-        arena.dense_bf16 = dense_bf16
+        arena.dense_bf16, arena.dense_fp8 = dense is True, dense == 'fp8'
         model._arena = arena
         ctx.reducer.init_arena(arena)
     else:

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 8
+#define BNS_ABI_VERSION 9
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -526,6 +526,33 @@ int bns_dense_nt_bf16(const float *A, int64_t lda, const float *B, int64_t ldb, 
                       int64_t N2, void *ws, size_t ws_bytes, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * ABI 9: the dense layers' forward and input-gradient products on fp8 rows (--dense-dtype fp8).  Every operand is an
+ * ABI 7 fp8 row: e4m3 codes plus one power-of-two f32 scale per row, by bns_cvt_rows_f32_fp8's rule.
+ * bns_dense_tn_fp8: C[m, n] = (sum_k qa[m, k] qb[n, k]) * a_scale[m] * b_scale[n] (+ bias[n]) (+ addend[m, n])
+ *     (* row_scale[m]), the epilogue in f32 in that order; addend may alias C.  The e4m3 wgmmas of each 128-code block
+ *     start from zero and their sums are added in f32.  A [M, K] and B [N, K] code rows: lda, ldb in bytes, multiples of
+ *     16, 16-byte aligned bases; K is any value >= 1 and the bytes between K and lda / ldb are never read.  Scales 4-byte
+ *     aligned; bias, addend, C, ldc, ldadd as for bns_dense_tn_bf16, with the same BNS_E_INVALID returns before any
+ *     launch.  A NaN scale (a row that held NaN or +-Inf) makes its own output row (a_scale) or column (b_scale) NaN.
+ *     The scales are applied as (sum * a_scale[m]) * b_scale[n] in f32, so with extreme scales of opposite exponent
+ *     (a row near 1e38 against one near 1e-30) the intermediate can overflow to +-Inf or lose bits to underflow even
+ *     where the exact product is representable.
+ * bns_cvt_rows_f32_fp8_any: bns_cvt_rows_f32_fp8 for rows of any width F % 4 == 0 (the codes between F and ldc are not
+ *     written).  ldc % 16 == 0, lds % 4 == 0, 16-byte aligned src and codes, 4-byte aligned scale.
+ * bns_dropout_fp8: bns_dropout_f32 (the same Philox mask, the same kept values bit for bit) that also stores each dropped
+ *     row y[r, :F] as an fp8 row (codes with ldc bytes per row, a multiple of 16; scale[r]).  F % 4 == 0, 16-byte aligned
+ *     x, y and codes.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_dense_tn_fp8(const uint8_t *A /*e4m3*/, int64_t lda, const float *a_scale, const uint8_t *B /*e4m3*/, int64_t ldb,
+                     const float *b_scale, const float *bias, const float *addend, int64_t ldadd, const float *row_scale,
+                     float *C, int64_t ldc, int64_t M, int64_t N, int64_t K, void *stream);
+int bns_cvt_rows_f32_fp8_any(const float *src, int64_t lds, uint8_t *codes /*e4m3*/, int64_t ldc, float *scale,
+                             int64_t n_rows, int64_t F, void *stream);
+int bns_dropout_fp8(const float *x, int64_t ldx, int64_t n, int64_t F, float p, uint64_t seed, uint64_t offset,
+                    const uint64_t *offset_dev, float *y, int64_t ldy, uint8_t *codes /*e4m3*/, int64_t ldc, float *scale,
+                    void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Loss and its gradient in one launch.  Replaces train.py:406-408 for the two losses of train.py:358-361:
  *     loss = CrossEntropyLoss(reduction='sum')(logits[train_mask], labels[train_mask])          (labels != NULL)
  *     loss = BCEWithLogitsLoss(reduction='sum')(logits[train_mask], labels[train_mask])        (labels_f != NULL)
@@ -549,7 +576,11 @@ int bns_xent_f32(const float *logits, int64_t ld, int64_t n_rows, int32_t n_clas
  * gradients, bias sums -- and advances *step_dev.  Entry layout: bns_derive_entry, table in device memory.
  * ----------------------------------------------------------------------------------------------*/
 typedef struct bns_derive_entry {
-    int32_t op;        /* 0: dst[c * ld_dst + r] = a[r * ld_a + c], r < rows, c < cols;  1: dst[i] = a[i] + b[i], i < rows */
+    int32_t op;        /* 0: dst[c * ld_dst + r] = a[r * ld_a + c], r < rows, c < cols;  1: dst[i] = a[i] + b[i], i < rows;
+                          2 / 3 (ABI 9): the fp8 rows (bns_cvt_rows_f32_fp8's rule) of x_r[k] = a[r * ld_a + k] (2) or
+                          a[k * ld_a + r] (3), r < rows, k < cols: codes of row r at (uint8_t *)dst + r * ld_dst (ld_dst in
+                          bytes, a multiple of 16), the rows' scales right after the codes, at (uint8_t *)dst + rows * ld_dst;
+                          cols % 4 == 0, and for op 2 16-byte aligned rows of a */
     int32_t rows, cols, ld_a, ld_dst, pad_;
     const float *a, *b;
     float *dst;

@@ -1,10 +1,13 @@
-"""``--dense-dtype f32`` against ``--dense-dtype bf16`` on the benchmark's workload (BASELINE.json configs[1]: Reddit-shape
-graph, 3-layer GraphSAGE, hidden 256, --use-pp) at ONE partition, both modes in one process:
+"""``--dense-dtype f32`` / ``bf16`` / ``fp8`` on the benchmark's workload (BASELINE.json configs[1]: Reddit-shape graph,
+3-layer GraphSAGE, hidden 256, --use-pp) at ONE partition, all modes in one process:
 
 * the mean time of every dense GEMM call of the epoch (``dense.PROFILE`` CUDA events, eager epochs, modes alternating),
-  by call site in launch order with its shape, and the dense milliseconds per epoch;
-* epochs/s of ``train.GraphedEpoch`` replays in alternating rounds, in two pairings: f32 against ``--dense-dtype bf16``,
-  and ``--agg-dtype bf16`` alone against ``--agg-dtype bf16 --dense-dtype bf16``;
+  by call site in launch order with its shape, and the dense milliseconds per epoch; under fp8 the quantization passes
+  (``ops.cvt_rows_fp8_any`` and layer 0's ``fused.dropout_fp8``, which also does the dropout) are timed on their own;
+* epochs/s of ``train.GraphedEpoch`` replays in alternating rounds, in four pairings: f32 against ``--dense-dtype bf16``,
+  ``--agg-dtype bf16`` alone against ``--agg-dtype bf16 --dense-dtype bf16``, ``--dense-dtype bf16`` against ``fp8``, and
+  ``--agg-dtype fp8`` with ``--dense-dtype bf16`` against it with ``fp8``.  One arena serves every mode, so once the
+  fp8 weights exist every mode's optimizer step also refreshes them (one launch either way);
 * the relative difference of the dropout-free forward loss at the initial weights (``train.probe_loss``) and of the
   same forward's logits (norm of the difference over the norm);
 * the card's name, power limit and maximum SM clock, read in the same run.
@@ -56,25 +59,30 @@ def main():
         st = train.setup(part.graph, part.node_dict, part.gpb, args, dev)
     assert st.arena is not None
 
-    def set_mode(dense_bf16: bool, agg_bf16: bool = False):
-        st.arena.dense_bf16, st.part.agg_bf16 = dense_bf16, agg_bf16
+    from bns_gcn_b200 import fused, ops
+    modes = ("f32", "bf16", "fp8")
+
+    def set_mode(dense_mode: str, agg_mode: str = "f32"):
+        st.arena.dense_bf16, st.arena.dense_fp8 = dense_mode == "bf16", dense_mode == "fp8"
+        st.part.agg_bf16, st.part.agg_fp8 = agg_mode == "bf16", agg_mode == "fp8"
 
     # ---- forward loss at the initial weights, dropout off ----
     loss, logits = {}, {}
-    for m in ("f32", "bf16"):
-        set_mode(m == "bf16")
+    for m in modes:
+        set_mode(m)
         loss[m] = float(train.probe_loss(st, 0).item())
         keep, st.model.dropout.p = st.model.dropout.p, 0.0
         with torch.no_grad():
             logits[m] = train._forward_logits(st, 0).double()
         st.model.dropout.p = keep
         st.epoch_dev.sub_(1)
-    logits_rel = float((logits["bf16"] - logits["f32"]).norm() / logits["f32"].norm())
+    logits_rel = {m: float((logits[m] - logits["f32"]).norm() / logits["f32"].norm()) for m in modes[1:]}
     del logits
 
     # ---- per-GEMM times (eager epochs), call sites in launch order ----
-    sites = []
-    plain = dense.tc_mm_tn, dense.tc_mm_nt
+    sites, quant = [], []
+    plain = dense.tc_mm_tn, dense.tc_mm_nt, dense.tc_mm_tn_fp8
+    plain_q = ops.cvt_rows_fp8_any, fused.dropout_fp8
 
     def tn(a_, b_, *args_, **kw):
         sites.append(f"TN M={a_.shape[0]} K={a_.shape[1]} N={b_.shape[0]}")
@@ -83,16 +91,34 @@ def main():
     def nt(a_, b_, *args_, **kw):
         sites.append(f"NT R={a_.shape[0]} N1={a_.shape[1]} N2={b_.shape[1]}")
         return plain[1](a_, b_, *args_, **kw)
-    dense.tc_mm_tn, dense.tc_mm_nt = tn, nt
+
+    def tn_fp8(a_, b_, *args_, **kw):
+        sites.append(f"TN M={a_.shape[0]} K={a_.shape[1]} N={b_.shape[0]}")
+        return plain[2](a_, b_, *args_, **kw)
+
+    def timed(name, fn):
+        def run(x, *args_, **kw):
+            if dense.PROFILE is None:
+                return fn(x, *args_, **kw)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            out_ = fn(x, *args_, **kw)
+            e1.record()
+            quant.append((f"{name} {x.shape[0]} x {x.shape[1]}", e0, e1))
+            return out_
+        return run
+    dense.tc_mm_tn, dense.tc_mm_nt, dense.tc_mm_tn_fp8 = tn, nt, tn_fp8
+    ops.cvt_rows_fp8_any = timed("cvt_rows_fp8_any", plain_q[0])
+    fused.dropout_fp8 = timed("dropout_fp8", plain_q[1])
     epoch = 0
-    gemm = {}
+    gemm, qpass = {}, {}
     try:
-        for m in ("f32", "bf16", "f32", "bf16"):
-            set_mode(m == "bf16")
+        for m in modes + modes:
+            set_mode(m)
             train.train_epoch(st, epoch)                             # warm the mode's shapes
             epoch += 1
             torch.cuda.synchronize()
-            dense.PROFILE, sites[:] = [], []
+            dense.PROFILE, sites[:], quant[:] = [], [], []
             for _ in range(a.profile_epochs):
                 train.train_epoch(st, epoch)
                 epoch += 1
@@ -102,17 +128,27 @@ def main():
             n = len(ms) // a.profile_epochs
             d = gemm.setdefault(m, {"ms": [], "sites": sites[:n], "flops": [p[2] for p in prof[:n]]})
             d["ms"].append([statistics.mean(ms[i::n]) for i in range(n)])
+            if m == "fp8":
+                nq = len(quant) // a.profile_epochs
+                q = qpass.setdefault("sites", [s_ for s_, _, _ in quant[:nq]])
+                qpass.setdefault("ms", []).append(
+                    [statistics.mean(e0.elapsed_time(e1) for _, e0, e1 in quant[i::nq]) for i in range(len(q))])
     finally:
-        dense.tc_mm_tn, dense.tc_mm_nt = plain
+        dense.tc_mm_tn, dense.tc_mm_nt, dense.tc_mm_tn_fp8 = plain
+        ops.cvt_rows_fp8_any, fused.dropout_fp8 = plain_q
     per_call = {m: [statistics.mean(x) for x in zip(*d["ms"])] for m, d in gemm.items()}
-    calls = [{"site": s, "gflop": f / 1e9, "f32_ms": x, "bf16_ms": y, "speedup": x / y}
-             for s, f, x, y in zip(gemm["f32"]["sites"], gemm["f32"]["flops"], per_call["f32"], per_call["bf16"])]
+    calls = [{"site": s, "gflop": f / 1e9, "f32_ms": x, "bf16_ms": y, "fp8_ms": z, "bf16_over_fp8": y / z}
+             for s, f, x, y, z in zip(gemm["f32"]["sites"], gemm["f32"]["flops"], per_call["f32"], per_call["bf16"],
+                                      per_call["fp8"])]
+    assert all(gemm[m]["sites"] == gemm["f32"]["sites"] for m in modes), "the modes' GEMM call sites differ"
+    quant_ms = [statistics.mean(x) for x in zip(*qpass["ms"])]
+    quant_calls = [{"site": s, "ms": t} for s, t in zip(qpass["sites"], quant_ms)]
 
     # ---- epochs/s of graph replays, modes alternating, one pairing at a time ----
     def pairing(modes):
         graphs = {}
-        for name, (d16, a16) in modes.items():
-            set_mode(d16, a16)
+        for name, (dm, am) in modes.items():
+            set_mode(dm, am)
             graphs[name] = train.GraphedEpoch(st, warmup=1)
             for _ in range(2):
                 graphs[name]()
@@ -139,11 +175,16 @@ def main():
                     "--use-pp, 1 partition",
         "card": card(),
         "gemm_calls": calls,
+        "fp8_quantization_passes": quant_calls,
         "dense_ms_per_epoch": {m: sum(v) for m, v in per_call.items()},
-        "graphed_f32_vs_dense_bf16": pairing({"f32": (False, False), "dense_bf16": (True, False)}),
-        "graphed_agg_bf16_vs_agg_dense_bf16": pairing({"agg_bf16": (False, True), "agg_dense_bf16": (True, True)}),
+        "dense_ms_per_epoch_fp8_with_quantization": sum(per_call["fp8"]) + sum(quant_ms),
+        "graphed_f32_vs_dense_bf16": pairing({"f32": ("f32", "f32"), "dense_bf16": ("bf16", "f32")}),
+        "graphed_agg_bf16_vs_agg_dense_bf16": pairing({"agg_bf16": ("f32", "bf16"), "agg_dense_bf16": ("bf16", "bf16")}),
+        "graphed_dense_bf16_vs_dense_fp8": pairing({"dense_bf16": ("bf16", "f32"), "dense_fp8": ("fp8", "f32")}),
+        "graphed_agg_fp8_dense_bf16_vs_dense_fp8": pairing({"agg_fp8_dense_bf16": ("bf16", "fp8"),
+                                                             "agg_fp8_dense_fp8": ("fp8", "fp8")}),
         "probe_loss": loss,
-        "probe_loss_rel_diff": abs(loss["bf16"] - loss["f32"]) / abs(loss["f32"]),
+        "probe_loss_rel_diff": {m: abs(loss[m] - loss["f32"]) / abs(loss["f32"]) for m in modes[1:]},
         "probe_logits_rel_diff_norm": logits_rel,
     }
     print(json.dumps(out))
