@@ -447,7 +447,7 @@ __device__ __forceinline__ void add_div8(float *v, uint4 r, float div) {
 
 // Lane types: what one lane of a row-wise kernel holds.  Vec<4> is one 16-byte f32 vector, Vec<1> the scalar path
 // for rows that are not 16-byte aligned, Bf16x8 eight bf16 values of one 16-byte load widened into eight f32 sums
-// (E4m3x16, SpMM only, is below).
+// (E4m3x16 is below).
 // T / kN: element type and count of one lane's slice of a row in X (SpMM) or on the wire (exchange).  In: what one
 // gather loads.  The sums, the partial sums of split rows and Y are f32 for every lane type.
 // min_blocks(NV, G, MAP && !CSCALE): the second argument of spmm_kernel's __launch_bounds__.
@@ -565,8 +565,10 @@ __device__ __forceinline__ float2 e4m3x2_f32(uint32_t w16) {
     return __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)w16, __NV_E4M3)));
 }
 
-// E4m3x16: sixteen e4m3 codes of one 16-byte load (--agg-dtype fp8), widened exactly into sixteen f32 sums.  The row's
-// power-of-two scale (SpmmArgsFp8::x_scale) is folded into the entry's weight, so every entry takes fma().  SpMM only.
+// E4m3x16: sixteen e4m3 codes of one 16-byte load (--agg-dtype fp8, --comm-dtype fp8), widened exactly into sixteen
+// f32 sums.  The rows are row-scaled (LaneArgs<E4m3x16>::kRowScaled): in the SpMM the row's power-of-two scale
+// (SpmmArgsFp8::x_scale) is folded into the entry's weight, so every entry takes fma(); the exchange's stores go
+// through quantize_row_fp8 (put_row) and its adds take the scale (add_div).
 struct E4m3x16 {
     using T = uint8_t;
     static constexpr int kN = 16;
@@ -939,19 +941,15 @@ int pick_slab(int64_t F, int64_t x_rows, int32_t forced, int elem_bytes = 4) {
 
 enum class Elem { kF32, kBf16, kFp8 };
 
-// x_scale: the row scales of an fp8 table (Elem::kFp8), NULL otherwise
+// x_scale: the row scales of an fp8 table (Elem::kFp8), NULL otherwise.  A bf16 or fp8 table has the 16-byte layout
+// (spmm_table_ok); an f32 one takes the scalar lanes without it.
 int spmm_dispatch(const SpmmArgs &a, Elem elem, int64_t x_rows, int32_t slab_hint, cudaStream_t st,
                   const float *x_scale = nullptr) {
     const int64_t F = a.F;
     const bool bf16 = elem == Elem::kBf16;
     const bool vec = (F % 4 == 0) && (a.ldx % 4 == 0) && (a.ldy % 4 == 0) &&
                      ((reinterpret_cast<uintptr_t>(a.X) | reinterpret_cast<uintptr_t>(a.Y)) % 16 == 0);
-    BNS_REQUIRE(vec || !bf16, "spmm: bf16 rows need the 16-byte layout (F %lld, ldx %lld, ldy %lld)", (long long)F,
-                (long long)a.ldx, (long long)a.ldy);
     if (elem == Elem::kFp8) {
-        BNS_REQUIRE(vec && F % 16 == 0 && a.ldx % 16 == 0 && (x_scale || a.X == nullptr),
-                    "spmm: fp8 rows need the 16-byte layout and their scales (F %lld, ldx %lld, ldy %lld)", (long long)F,
-                    (long long)a.ldx, (long long)a.ldy);
         SpmmArgsFp8 f;
         static_cast<SpmmArgs &>(f) = a;
         f.x_scale = x_scale;
@@ -1003,33 +1001,75 @@ extern "C" size_t bns_spmm_workspace_bytes(const bns_graph_t *g, int64_t F) {
     return (size_t)g->n_parts * (size_t)ws_ld(F) * sizeof(float);
 }
 
-// the 16-byte gathers and the 2 x 16-byte stores of the bf16 lanes
-#define BNS_BF16_LAYOUT(fn)                                                                                            \
-    BNS_REQUIRE(F % 8 == 0 && ldx % 8 == 0 && ldy % 4 == 0 &&                                                          \
-                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
-                fn ": needs F %% 8 == 0, ldx %% 8 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "   \
-                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
+namespace {
+
+// What every gather-table entry point checks once its matrices are there and their leading dimensions cover F: the
+// 16-byte gathers of a bf16 or fp8 table (8 or 16 elements each) with their 16-byte f32 stores, and the split-row
+// workspace.  fn names the entry point in the message.
+int spmm_table_ok(const char *fn, Elem elem, const bns_graph_t *g, const void *X, int64_t ldx, int64_t F, const float *Y,
+                  int64_t ldy, const void *ws, size_t ws_bytes) {
+    if (elem != Elem::kF32) {
+        const int n = elem == Elem::kFp8 ? 16 : 8;
+        BNS_REQUIRE(F % n == 0 && ldx % n == 0 && ldy % 4 == 0 &&
+                        ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,
+                    "%s: needs F %% %d == 0, ldx %% %d == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "
+                    "ldy %lld)", fn, n, n, (long long)F, (long long)ldx, (long long)ldy);
+    }
+    const size_t need = bns_spmm_workspace_bytes(g, F);
+    if (need > 0 && (ws == nullptr || ws_bytes < need))
+        return fail(BNS_E_WORKSPACE, "%s: workspace %zu bytes < %zu needed", fn, ws_bytes, need);
+    return BNS_OK;
+}
+
+// bns_spmm_sum_f32 / _bf16 / _fp8: X rows of f32, bf16 or e4m3 codes with their scales x_scale (fp8 only)
+int spmm_sum(Elem elem, const bns_graph_t *g, const void *X, const float *x_scale, int64_t ldx, int64_t F, float *Y,
+             int64_t ldy, const float *row_scale, const float *col_scale, const float *edge_weight, const int32_t *row_map,
+             const int32_t *col_map, int64_t n_direct, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws,
+             size_t ws_bytes, void *stream) {
+    const bool fp8 = elem == Elem::kFp8;
+    const char *fn = fp8 ? "bns_spmm_sum_fp8" : elem == Elem::kBf16 ? "bns_spmm_sum_bf16" : "bns_spmm_sum_f32";
+    BNS_REQUIRE(g, "%s: NULL graph", fn);
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "%s: bad feature width %lld", fn, (long long)F);
+    if (g->n_rows == 0) return BNS_OK;      // nothing to write (Y may legitimately be NULL)
+    BNS_REQUIRE(Y, "%s: NULL output matrix", fn);
+    BNS_REQUIRE(X ? x_scale || !fp8 : g->nnz == 0, fp8 ? "%s: NULL input matrix or scales" : "%s: NULL input matrix", fn);
+    BNS_REQUIRE(ldx >= F && ldy >= F, "%s: leading dimension smaller than F", fn);
+    if (const int rc = spmm_table_ok(fn, elem, g, X, ldx, F, Y, ldy, ws, ws_bytes)) return rc;
+    if (col_map == nullptr) n_direct = g->n_cols;
+    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "%s: n_direct out of range", fn);
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
+    a.n_direct = (int32_t)n_direct;
+    return spmm_dispatch(a, elem, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream), x_scale);
+}
+
+// bns_spmm_compact_f32 / _bf16 / _fp8, X as for spmm_sum
+int spmm_compact(Elem elem, const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
+                 const int32_t *chunk_cnt, const void *X, const float *x_scale, int64_t ldx, int64_t F, float *Y, int64_t ldy,
+                 const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes,
+                 void *stream) {
+    const bool fp8 = elem == Elem::kFp8;
+    const char *fn = fp8 ? "bns_spmm_compact_fp8" : elem == Elem::kBf16 ? "bns_spmm_compact_bf16" : "bns_spmm_compact_f32";
+    BNS_REQUIRE(g && cidx && chunk_cnt, "%s: NULL argument", fn);
+    BNS_REQUIRE(F > 0 && F < (1 << 24), "%s: bad feature width %lld", fn, (long long)F);
+    if (g->n_rows == 0) return BNS_OK;
+    BNS_REQUIRE(Y && (X ? x_scale || !fp8 : g->nnz == 0), "%s: NULL matrix", fn);
+    BNS_REQUIRE(ldx >= F && ldy >= F, "%s: leading dimension smaller than F", fn);
+    if (const int rc = spmm_table_ok(fn, elem, g, X, ldx, F, Y, ldy, ws, ws_bytes)) return rc;
+    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
+    a.indices = cidx; a.chunk_cnt = chunk_cnt;
+    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
+    return spmm_dispatch(a, elem, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream), x_scale);
+}
+
+}  // namespace
 
 extern "C" int bns_spmm_sum_f32(const bns_graph_t *g, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                                 const float *row_scale, const float *col_scale, const float *edge_weight,
                                 const int32_t *row_map, const int32_t *col_map, int64_t n_direct, int64_t x_rows,
                                 int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(g, "bns_spmm_sum_f32: NULL graph");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_sum_f32: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;      // nothing to write (Y may legitimately be NULL)
-    BNS_REQUIRE(Y, "bns_spmm_sum_f32: NULL output matrix");
-    BNS_REQUIRE(X || g->nnz == 0, "bns_spmm_sum_f32: NULL input matrix");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_sum_f32: leading dimension smaller than F");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_sum_f32: workspace %zu bytes < %zu needed", ws_bytes, need);
-    if (col_map == nullptr) n_direct = g->n_cols;
-    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_f32: n_direct out of range");
-    if (x_rows <= 0) x_rows = g->n_cols;
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
-    a.n_direct = (int32_t)n_direct;
-    return spmm_dispatch(a, Elem::kF32, x_rows, slab_hint, as_stream(stream));
+    return spmm_sum(Elem::kF32, g, X, nullptr, ldx, F, Y, ldy, row_scale, col_scale, edge_weight, row_map, col_map,
+                    n_direct, x_rows, slab_hint, accumulate, ws, ws_bytes, stream);
 }
 
 // The same kernel over the per-epoch compacted indices of bns_graph_compact_cols: `cidx` already holds rows of X, the
@@ -1040,18 +1080,8 @@ extern "C" int bns_spmm_compact_f32(const bns_graph_t *g, const int32_t *cidx, c
                                     const int32_t *chunk_cnt, const float *X, int64_t ldx, int64_t F, float *Y, int64_t ldy,
                                     const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate, void *ws,
                                     size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(g && cidx && chunk_cnt, "bns_spmm_compact_f32: NULL argument");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_compact_f32: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(Y && (X || g->nnz == 0), "bns_spmm_compact_f32: NULL matrix");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_compact_f32: leading dimension smaller than F");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_compact_f32: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.indices = cidx; a.chunk_cnt = chunk_cnt;
-    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    return spmm_dispatch(a, Elem::kF32, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    return spmm_compact(Elem::kF32, g, cidx, cw, cw_ld, chunk_cnt, X, nullptr, ldx, F, Y, ldy, row_scale, x_rows,
+                        slab_hint, accumulate, ws, ws_bytes, stream);
 }
 
 // Y[orow(r)] (+)= sum_k w_k X[c_k] with w_k = weights[(perm ? perm[k] : k) * ldw]: the weighted aggregation of GATConv
@@ -1065,9 +1095,7 @@ extern "C" int bns_spmm_weighted_f32(const bns_graph_t *g, const float *X, int64
     BNS_REQUIRE(!perm_from_transpose || g->perm, "bns_spmm_weighted_f32: not a graph made by bns_graph_transpose");
     if (g->n_rows == 0) return BNS_OK;
     BNS_REQUIRE(Y && (X || g->nnz == 0) && ldx >= F && ldy >= F, "bns_spmm_weighted_f32: bad matrix");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_weighted_f32: workspace %zu bytes < %zu needed", ws_bytes, need);
+    if (const int rc = spmm_table_ok("bns_spmm_weighted_f32", Elem::kF32, g, X, ldx, F, Y, ldy, ws, ws_bytes)) return rc;
     SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
     a.edge_weight = weights; a.row_map = row_map;
     a.edge_perm = perm_from_transpose ? g->perm : nullptr; a.edge_ld = ldw;
@@ -1080,50 +1108,17 @@ extern "C" int bns_spmm_sum_bf16(const bns_graph_t *g, const uint16_t *X, int64_
                                  const float *row_scale, const float *col_scale, const float *edge_weight,
                                  const int32_t *row_map, const int32_t *col_map, int64_t n_direct, int64_t x_rows,
                                  int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(g, "bns_spmm_sum_bf16: NULL graph");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_sum_bf16: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(Y, "bns_spmm_sum_bf16: NULL output matrix");
-    BNS_REQUIRE(X || g->nnz == 0, "bns_spmm_sum_bf16: NULL input matrix");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_sum_bf16: leading dimension smaller than F");
-    BNS_BF16_LAYOUT("bns_spmm_sum_bf16");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_sum_bf16: workspace %zu bytes < %zu needed", ws_bytes, need);
-    if (col_map == nullptr) n_direct = g->n_cols;
-    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_bf16: n_direct out of range");
-    if (x_rows <= 0) x_rows = g->n_cols;
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
-    a.n_direct = (int32_t)n_direct;
-    return spmm_dispatch(a, Elem::kBf16, x_rows, slab_hint, as_stream(stream));
+    return spmm_sum(Elem::kBf16, g, X, nullptr, ldx, F, Y, ldy, row_scale, col_scale, edge_weight, row_map, col_map,
+                    n_direct, x_rows, slab_hint, accumulate, ws, ws_bytes, stream);
 }
 
 extern "C" int bns_spmm_compact_bf16(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
                                      const int32_t *chunk_cnt, const uint16_t *X, int64_t ldx, int64_t F, float *Y,
                                      int64_t ldy, const float *row_scale, int64_t x_rows, int32_t slab_hint, int accumulate,
                                      void *ws, size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(g && cidx && chunk_cnt, "bns_spmm_compact_bf16: NULL argument");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_compact_bf16: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(Y && (X || g->nnz == 0), "bns_spmm_compact_bf16: NULL matrix");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_compact_bf16: leading dimension smaller than F");
-    BNS_BF16_LAYOUT("bns_spmm_compact_bf16");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_compact_bf16: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.indices = cidx; a.chunk_cnt = chunk_cnt;
-    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    return spmm_dispatch(a, Elem::kBf16, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream));
+    return spmm_compact(Elem::kBf16, g, cidx, cw, cw_ld, chunk_cnt, X, nullptr, ldx, F, Y, ldy, row_scale, x_rows,
+                        slab_hint, accumulate, ws, ws_bytes, stream);
 }
-
-// the 16-byte gathers of the fp8 lanes (16 codes each) and their 16-byte f32 stores
-#define BNS_FP8_LAYOUT(fn)                                                                                             \
-    BNS_REQUIRE(F % 16 == 0 && ldx % 16 == 0 && ldy % 4 == 0 &&                                                        \
-                    ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(Y)) % 16) == 0,                     \
-                fn ": needs F %% 16 == 0, ldx %% 16 == 0, ldy %% 4 == 0 and 16-byte aligned X, Y (F %lld, ldx %lld, "  \
-                   "ldy %lld)", (long long)F, (long long)ldx, (long long)ldy)
 
 // The same sums over an fp8 gather table (--agg-dtype fp8): X rows are e4m3 codes (ldx in bytes) and x_scale holds one
 // f32 scale per row of X.  Entry k adds  w_k * x_scale[xrow(c_k)] * widen(X[xrow(c_k)])  in f32, w_k = col_scale[c_k]
@@ -1133,42 +1128,16 @@ extern "C" int bns_spmm_sum_fp8(const bns_graph_t *g, const uint8_t *X, const fl
                                 const float *edge_weight, const int32_t *row_map, const int32_t *col_map, int64_t n_direct,
                                 int64_t x_rows, int32_t slab_hint, int accumulate, void *ws, size_t ws_bytes,
                                 void *stream) {
-    BNS_REQUIRE(g, "bns_spmm_sum_fp8: NULL graph");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_sum_fp8: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(Y, "bns_spmm_sum_fp8: NULL output matrix");
-    BNS_REQUIRE((X && x_scale) || g->nnz == 0, "bns_spmm_sum_fp8: NULL input matrix or scales");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_sum_fp8: leading dimension smaller than F");
-    BNS_FP8_LAYOUT("bns_spmm_sum_fp8");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_sum_fp8: workspace %zu bytes < %zu needed", ws_bytes, need);
-    if (col_map == nullptr) n_direct = g->n_cols;
-    BNS_REQUIRE(n_direct >= 0 && n_direct <= g->n_cols, "bns_spmm_sum_fp8: n_direct out of range");
-    if (x_rows <= 0) x_rows = g->n_cols;
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.row_scale = row_scale; a.col_scale = col_scale; a.edge_weight = edge_weight; a.row_map = row_map; a.col_map = col_map;
-    a.n_direct = (int32_t)n_direct;
-    return spmm_dispatch(a, Elem::kFp8, x_rows, slab_hint, as_stream(stream), x_scale);
+    return spmm_sum(Elem::kFp8, g, X, x_scale, ldx, F, Y, ldy, row_scale, col_scale, edge_weight, row_map, col_map,
+                    n_direct, x_rows, slab_hint, accumulate, ws, ws_bytes, stream);
 }
 
 extern "C" int bns_spmm_compact_fp8(const bns_graph_t *g, const int32_t *cidx, const float *cw, int64_t cw_ld,
                                     const int32_t *chunk_cnt, const uint8_t *X, const float *x_scale, int64_t ldx, int64_t F,
                                     float *Y, int64_t ldy, const float *row_scale, int64_t x_rows, int32_t slab_hint,
                                     int accumulate, void *ws, size_t ws_bytes, void *stream) {
-    BNS_REQUIRE(g && cidx && chunk_cnt, "bns_spmm_compact_fp8: NULL argument");
-    BNS_REQUIRE(F > 0 && F < (1 << 24), "bns_spmm_compact_fp8: bad feature width %lld", (long long)F);
-    if (g->n_rows == 0) return BNS_OK;
-    BNS_REQUIRE(Y && ((X && x_scale) || g->nnz == 0), "bns_spmm_compact_fp8: NULL matrix");
-    BNS_REQUIRE(ldx >= F && ldy >= F, "bns_spmm_compact_fp8: leading dimension smaller than F");
-    BNS_FP8_LAYOUT("bns_spmm_compact_fp8");
-    const size_t need = bns_spmm_workspace_bytes(g, F);
-    if (need > 0 && (ws == nullptr || ws_bytes < need))
-        return fail(BNS_E_WORKSPACE, "bns_spmm_compact_fp8: workspace %zu bytes < %zu needed", ws_bytes, need);
-    SpmmArgs a = spmm_args(g, X, ldx, F, Y, ldy, accumulate, ws);
-    a.indices = cidx; a.chunk_cnt = chunk_cnt;
-    a.row_scale = row_scale; a.edge_weight = cw; a.edge_ld = cw_ld > 0 ? cw_ld : 1;
-    return spmm_dispatch(a, Elem::kFp8, x_rows > 0 ? x_rows : g->n_cols, slab_hint, as_stream(stream), x_scale);
+    return spmm_compact(Elem::kFp8, g, cidx, cw, cw_ld, chunk_cnt, X, x_scale, ldx, F, Y, ldy, row_scale, x_rows,
+                        slab_hint, accumulate, ws, ws_bytes, stream);
 }
 
 namespace {
@@ -1494,39 +1463,67 @@ extern "C" int bns_sddmm_dot_f32(const bns_graph_t *g, const float *A, int64_t l
 // =================================================================================================
 namespace {
 
+// By one warp: the wire row d[0:F] = src[0:F] / div in the lane type's format.  For a row-scaled lane type (E4m3x16,
+// F <= 1024) that is the fp8 row of the quotients with its scale in *scale; the other types ignore scale.
+template <class L>
+__device__ __forceinline__ void put_row(const float *src, float div, int F, typename L::T *d, float *scale, int lane) {
+    if constexpr (LaneArgs<L>::kRowScaled) {
+        quantize_row_fp8(src, div, F, d, scale, lane);
+    } else {
+        for (int f = lane * L::kN; f < F; f += 32 * L::kN)
+            *reinterpret_cast<typename L::Wire *>(d + f) = L::div_round(src + f, div);
+    }
+}
+
 // One warp per row: the pack  dst[i] = src[idx[i]] / div  or the scatter  dst[idx[i]] += src[i] / div  (the ids of one
 // call are distinct).  The wire side (dst of the pack, src of the scatter) holds the lane type's elements: f32 with
-// 16-byte or scalar lanes, or bf16 x 8 (--comm-dtype bf16); the other side is f32.
+// 16-byte or scalar lanes, bf16 x 8 (--comm-dtype bf16) or e4m3 x 16 (--comm-dtype fp8, whose row i has the scale
+// scale[i]; NULL for the others); the other side is f32.
 template <class L, bool SCATTER>
 __global__ void __launch_bounds__(kThreads) rows_kernel(const std::conditional_t<SCATTER, typename L::T, float> *__restrict__ src,
                                                         int64_t lds, std::conditional_t<SCATTER, float, typename L::T> *dst,
                                                         int64_t ldd, const int64_t *__restrict__ idx, int64_t k,
-                                                        int32_t F, float div) {
+                                                        int32_t F, float div,
+                                                        std::conditional_t<SCATTER, const float, float> *__restrict__ scale) {
+    constexpr bool kRowScaled = LaneArgs<L>::kRowScaled;
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
     for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
-        // The bf16 pack's entry point requires the ids.  Without this the compiler adds a second copy of the row loop
-        // for a NULL idx and spills around the division's slow path.
-        if constexpr (L::kN == 8 && !SCATTER) __builtin_assume(idx != nullptr);
+        // The entry points require the ids.  Without this the compiler adds a second copy of the row loop for a NULL
+        // idx: the bf16 pack then spills around the division's slow path, and the fp8 scatter's code nearly doubles.
+        if constexpr ((L::kN == 8 && !SCATTER) || kRowScaled) __builtin_assume(idx != nullptr);
         const int64_t r = idx ? idx[i] : i;
         const auto *s = SCATTER ? src + i * lds : src + r * lds;
         auto *d = SCATTER ? dst + r * ldd : dst + i * ldd;
-        for (int f = lane * L::kN; f < F; f += 32 * L::kN) {
-            if constexpr (SCATTER) {
+        if constexpr (!SCATTER) {
+            put_row<L>(s, div, F, d, kRowScaled ? scale + i : nullptr, lane);
+        } else {
+            const float sc = kRowScaled ? scale[i] : 1.f;
+            for (int f = lane * L::kN; f < F; f += 32 * L::kN) {
                 L v;
-                v.load_div(s + f, div);
-                v.add_f32(d + f);
+                if constexpr (kRowScaled) {         // d + (code * sc) / div: the sum the f32 lanes make of the widened row
+                    v.load(d + f);
+                    v.add_div(s + f, sc, div);
+                } else {
+                    v.load_div(s + f, div);
+                    v.add_f32(d + f);
+                }
                 v.store(d + f);
-            } else {
-                *reinterpret_cast<typename L::Wire *>(d + f) = L::div_round(s + f, div);
             }
         }
     }
 }
 
-inline bool vec_ok(const void *a, const void *b, int64_t F, int64_t lda, int64_t ldb) {
-    return F % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 &&
-           ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) % 16 == 0);
+// The layout of 16-byte lanes between f32 rows and wire rows of T (float, bf16 as uint16_t, e4m3 codes as uint8_t):
+// F and the wire rows' leading dimension in whole lanes, the f32 rows' in whole float4s (in 8 floats for bf16), both
+// matrices 16-byte aligned, and the wire rows' scales (fp8) 4-byte aligned.  bf16 and fp8 rows need it; f32 rows
+// without it take the scalar lanes.
+template <class T>
+bool rows_ok(const float *f32, int64_t ld32, const T *wire, int64_t ldw, const float *scale, int64_t F) {
+    constexpr int64_t n = 16 / sizeof(T);
+    return F % n == 0 && ldw % n == 0 && ld32 % (sizeof(T) == 2 ? 8 : 4) == 0 &&
+           reinterpret_cast<uintptr_t>(scale) % 4 == 0 &&
+           ((reinterpret_cast<uintptr_t>(f32) | reinterpret_cast<uintptr_t>(wire)) % 16) == 0;
 }
 
 inline unsigned rows_grid(int64_t k) {
@@ -1536,40 +1533,6 @@ inline unsigned rows_grid(int64_t k) {
 }
 
 }  // namespace
-
-extern "C" int bns_gather_div_f32(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
-                                  float *out, int64_t ldo, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_gather_div_f32: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(H && out && idx, "bns_gather_div_f32: NULL pointer");
-    BNS_REQUIRE(ldh >= F && ldo >= F, "bns_gather_div_f32: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_gather_div_f32: division by zero");
-    cudaStream_t st = as_stream(stream);
-    if (vec_ok(H, out, F, ldh, ldo))
-        rows_kernel<Vec<4>, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
-    else
-        rows_kernel<Vec<1>, false><<<rows_grid(k), kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
-
-extern "C" int bns_scatter_add_div_f32(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
-                                       const float *src, int64_t lds, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_scatter_add_div_f32: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(G && src && idx, "bns_scatter_add_div_f32: NULL pointer");
-    BNS_REQUIRE(ldg >= F && lds >= F, "bns_scatter_add_div_f32: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_f32: division by zero");
-    cudaStream_t st = as_stream(stream);
-    if (vec_ok(G, src, F, ldg, lds))
-        rows_kernel<Vec<4>, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
-    else
-        rows_kernel<Vec<1>, true><<<rows_grid(k), kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
 
 extern "C" int bns_copy_rows_f32(const float *src, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
                                  void *stream) {
@@ -2338,7 +2301,7 @@ extern "C" int bns_p2p_put_rows_f32(bns_p2p_t *p, int32_t peer, size_t remote_of
                                                             align256((size_t)p->n_flags * 8)) + peer;
     cudaStream_t st = as_stream(stream);
     const unsigned grid = rows_grid(k);
-    if (vec_ok(H, remote, F, ldh, ld_remote))
+    if (rows_ok(H, ldh, remote, ld_remote, nullptr, F))
         p2p_put_rows_kernel<true><<<grid, kThreads, 0, st>>>(H, ldh, (int32_t)F, idx, k, div, remote, ld_remote, flag,
                                                              flag_value,
                                                              reinterpret_cast<const unsigned long long *>(flag_value_dev), ticket);

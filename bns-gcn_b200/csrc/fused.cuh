@@ -444,31 +444,17 @@ struct PutAllDev {
     unsigned long long flag_value; const unsigned long long *flag_value_dev; unsigned int *ticket;
 };
 
-// one warp per row: the remote row = H[r] / div in the lane type's wire format (f32, or bf16 after the f32 division)
-template <class L>
-__global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllDev a) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
-        int s = 0;
-        while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
-        const int64_t local = i - a.row_begin[s];
-        const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
-        const float *src = a.H + r * a.ldh;
-        typename L::T *d = reinterpret_cast<typename L::T *>(a.remote[s]) + local * a.ld_remote;
-        const float div = a.div[s];
-        for (int f = lane * L::kN; f < a.F; f += 32 * L::kN)
-            *reinterpret_cast<typename L::Wire *>(d + f) = L::div_round(src + f, div);
-    }
-    publish_flags(a);
-}
-
 struct PutAllFp8Dev : PutAllDev {               // remote: the code rows (ld_remote bytes apart)
     float *scale[kMaxPeers];                    // the rows' scales in the peer's slab
 };
 
-// one warp per row: the remote row = the fp8 row of H[r] / div (quantize_row_fp8: codes and scale), F <= 1024
-__global__ void __launch_bounds__(kThreads) p2p_put_all_fp8_kernel(PutAllFp8Dev a) {
+// What p2p_put_all_kernel takes for a lane type: PutAllDev, and for a row-scaled one (E4m3x16) the scales' places
+template <class L> using PutAllArgs = std::conditional_t<LaneArgs<L>::kRowScaled, PutAllFp8Dev, PutAllDev>;
+
+// one warp per row: the remote row = H[r] / div in the lane type's wire format (put_row: f32, bf16 after the f32
+// division, or the fp8 row with its scale)
+template <class L>
+__global__ void __launch_bounds__(kThreads) p2p_put_all_kernel(PutAllArgs<L> a) {
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps, total = a.row_begin[a.n_seg];
     for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < total; i += warps_total) {
@@ -476,8 +462,10 @@ __global__ void __launch_bounds__(kThreads) p2p_put_all_fp8_kernel(PutAllFp8Dev 
         while (s + 1 < a.n_seg && a.row_begin[s + 1] <= i) ++s;
         const int64_t local = i - a.row_begin[s];
         const int64_t r = a.idx ? a.idx[i] : a.src_begin[s] + local;
-        quantize_row_fp8(a.H + r * a.ldh, a.div[s], a.F, reinterpret_cast<uint8_t *>(a.remote[s]) + local * a.ld_remote,
-                         a.scale[s] + local, lane);
+        float *scale = nullptr;
+        if constexpr (LaneArgs<L>::kRowScaled) scale = a.scale[s] + local;
+        put_row<L>(a.H + r * a.ldh, a.div[s], a.F, reinterpret_cast<typename L::T *>(a.remote[s]) + local * a.ld_remote,
+                   scale, lane);
     }
     publish_flags(a);
 }
@@ -534,12 +522,15 @@ struct ScatterAllFp8Dev : ScatterAllDev {      // recv: the code rows (ld_recv b
     const float *scale[kMaxPeers];              // their scales
 };
 
+// What scatter_rows_all_kernel takes for a lane type: ScatterAllDev, and for a row-scaled one (E4m3x16) the scales
+template <class L> using ScatterAllArgs = std::conditional_t<LaneArgs<L>::kRowScaled, ScatterAllFp8Dev, ScatterAllDev>;
+
 // one warp per destination row: contributions of the peers are added in table order (= the reference's ring order,
 // helper/feature_buffer.py:111-129), each with a true division -- bit-identical to P-1 successive scatter-adds.  The
-// column loop is warp-uniform: every lane takes every shuffle, and the lanes past F load and store nothing.
-// D: ScatterAllDev, or ScatterAllFp8Dev for fp8 rows (E4m3x16), whose received row k of segment s is scaled by scale[s][k].
-template <class L, class D>
-__device__ __forceinline__ void scatter_rows_all_body(const D &a) {
+// column loop is warp-uniform: every lane takes every shuffle, and the lanes past F load and store nothing.  The
+// received row k of segment s of a row-scaled lane type is scaled by scale[s][k].
+template <class L>
+__global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllArgs<L> a) {
     const int lane = threadIdx.x & 31;
     const int64_t warps_total = (int64_t)gridDim.x * kWarps;
     for (int64_t row = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); row < a.n_rows; row += warps_total) {
@@ -557,19 +548,12 @@ __device__ __forceinline__ void scatter_rows_all_body(const D &a) {
                 const int32_t k = __shfl_sync(0xffffffffu, mine, s);
                 if (k < 0 || !on) continue;
                 const auto *r = reinterpret_cast<const typename L::T *>(a.recv[s]) + (int64_t)k * a.ld_recv + f;
-                if constexpr (std::is_same_v<D, ScatterAllFp8Dev>) v.add_div(r, a.scale[s][k], a.div[s]);
+                if constexpr (LaneArgs<L>::kRowScaled) v.add_div(r, a.scale[s][k], a.div[s]);
                 else v.add_div(r, a.div[s]);
             }
             if (on) v.store(g + f);
         }
     }
-}
-
-template <class L>
-__global__ void __launch_bounds__(kThreads) scatter_rows_all_kernel(ScatterAllDev a) { scatter_rows_all_body<L>(a); }
-
-__global__ void __launch_bounds__(kThreads) scatter_rows_all_fp8_kernel(ScatterAllFp8Dev a) {
-    scatter_rows_all_body<E4m3x16>(a);
 }
 
 // bns_p2p_put_all_f32 / _bf16 / _fp8 (T = float / uint16_t / uint8_t on the wire): one set of checks and one segment
@@ -628,7 +612,7 @@ int put_all(bns_p2p_t *p, const bns_put_all *segs, const uint64_t *scale_off, in
     a.ticket = reinterpret_cast<unsigned int *>(reinterpret_cast<char *>(p->flags) + align256((size_t)p->n_flags * 8)) + ticket_index;
     const unsigned grid = rows_grid(total);
     const PutAllDev &b = a;
-    if (fp8) p2p_put_all_fp8_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    if (fp8) p2p_put_all_kernel<E4m3x16><<<grid, kThreads, 0, as_stream(stream)>>>(a);
     else if (bf16) p2p_put_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     else if (vec) p2p_put_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     else p2p_put_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
@@ -672,10 +656,68 @@ int scatter_rows_all(float *G, int64_t ldg, int64_t n_rows, int64_t F, int32_t n
     a.ld_recv = ld_recv; a.G = G; a.ldg = ldg; a.F = (int32_t)F; a.n_rows = n_rows;
     const unsigned grid = rows_grid(n_rows);
     const ScatterAllDev &b = a;
-    if (fp8) scatter_rows_all_fp8_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(a);
+    if (fp8) scatter_rows_all_kernel<E4m3x16><<<grid, kThreads, 0, as_stream(stream)>>>(a);
     else if (bf16) scatter_rows_all_kernel<Bf16x8><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     else if (vec) scatter_rows_all_kernel<Vec<4>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
     else scatter_rows_all_kernel<Vec<1>><<<grid, kThreads, 0, as_stream(stream)>>>(b);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// The staged transport's pack (K3): bns_gather_div_f32 / _bf16 / _fp8 (T = float / uint16_t / uint8_t on the wire);
+// out_scale: the fp8 rows' scales (NULL otherwise)
+template <class T>
+int gather_div(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div, T *out, int64_t ldo,
+               float *out_scale, void *stream) {
+    constexpr bool bf16 = sizeof(T) == 2, fp8 = sizeof(T) == 1;
+    const char *fn = fp8 ? "bns_gather_div_fp8" : bf16 ? "bns_gather_div_bf16" : "bns_gather_div_f32";
+    BNS_REQUIRE(k >= 0 && F > 0, "%s: bad size", fn);
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(H && out && idx && (!fp8 || out_scale), "%s: NULL pointer", fn);
+    BNS_REQUIRE(ldh >= F && ldo >= F, "%s: leading dimension smaller than F", fn);
+    BNS_REQUIRE(div != 0.f, "%s: division by zero", fn);
+    const bool vec = rows_ok(H, ldh, out, ldo, out_scale, F);
+    BNS_REQUIRE(!bf16 || vec, "%s: needs F, ldh, ldo multiples of 8 and 16-byte aligned H, out (F %lld, ldh %lld, ldo %lld)",
+                fn, (long long)F, (long long)ldh, (long long)ldo);
+    BNS_REQUIRE(!fp8 || (vec && F <= 1024 && ldh % 16 == 0),
+                "%s: needs F <= 1024, F, ldh, ldo multiples of 16, 16-byte aligned H, out and 4-byte aligned scales "
+                "(F %lld, ldh %lld, ldo %lld)", fn, (long long)F, (long long)ldh, (long long)ldo);
+    const unsigned grid = rows_grid(k);
+    cudaStream_t st = as_stream(stream);
+    if constexpr (fp8) rows_kernel<E4m3x16, false><<<grid, kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div, out_scale);
+    else if constexpr (bf16) rows_kernel<Bf16x8, false><<<grid, kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div, nullptr);
+    else if (vec) rows_kernel<Vec<4>, false><<<grid, kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div, nullptr);
+    else rows_kernel<Vec<1>, false><<<grid, kThreads, 0, st>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div, nullptr);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// The staged transport's scatter (K5): bns_scatter_add_div_f32 / _bf16 / _fp8 (T as for gather_div); src_scale: the fp8
+// rows' scales (NULL otherwise)
+template <class T>
+int scatter_add_div(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div, const T *src, int64_t lds,
+                    const float *src_scale, void *stream) {
+    constexpr bool bf16 = sizeof(T) == 2, fp8 = sizeof(T) == 1;
+    const char *fn = fp8 ? "bns_scatter_add_div_fp8" : bf16 ? "bns_scatter_add_div_bf16" : "bns_scatter_add_div_f32";
+    BNS_REQUIRE(k >= 0 && F > 0, "%s: bad size", fn);
+    if (k == 0) return BNS_OK;
+    BNS_REQUIRE(G && src && idx && (!fp8 || src_scale), "%s: NULL pointer", fn);
+    BNS_REQUIRE(ldg >= F && lds >= F, "%s: leading dimension smaller than F", fn);
+    BNS_REQUIRE(div != 0.f, "%s: division by zero", fn);
+    const bool vec = rows_ok(G, ldg, src, lds, src_scale, F);
+    BNS_REQUIRE(!(bf16 || fp8) || vec,
+                fp8 ? "%s: needs F, lds multiples of 16, ldg of 4, 16-byte aligned G, src and 4-byte aligned scales "
+                      "(F %lld, ldg %lld, lds %lld)"
+                    : "%s: needs F, ldg, lds multiples of 8 and 16-byte aligned G, src (F %lld, ldg %lld, lds %lld)",
+                fn, (long long)F, (long long)ldg, (long long)lds);
+    const unsigned grid = rows_grid(k);
+    cudaStream_t st = as_stream(stream);
+    if constexpr (fp8) rows_kernel<E4m3x16, true><<<grid, kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div, src_scale);
+    else if constexpr (bf16) rows_kernel<Bf16x8, true><<<grid, kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div, nullptr);
+    else if (vec) rows_kernel<Vec<4>, true><<<grid, kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div, nullptr);
+    else rows_kernel<Vec<1>, true><<<grid, kThreads, 0, st>>>(src, lds, G, ldg, idx, k, (int32_t)F, div, nullptr);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -686,8 +728,8 @@ void preload_exchange_kernels() {
     cudaFuncAttributes fa;
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Bf16x8>);
     cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<Bf16x8>);
-    cudaFuncGetAttributes(&fa, p2p_put_all_fp8_kernel);
-    cudaFuncGetAttributes(&fa, scatter_rows_all_fp8_kernel);
+    cudaFuncGetAttributes(&fa, p2p_put_all_kernel<E4m3x16>);
+    cudaFuncGetAttributes(&fa, scatter_rows_all_kernel<E4m3x16>);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<4>>);
     cudaFuncGetAttributes(&fa, p2p_put_all_kernel<Vec<1>>);
     cudaFuncGetAttributes(&fa, p2p_put_ids_kernel);
@@ -794,7 +836,37 @@ extern "C" int bns_scatter_rows_all_fp8(float *G, int64_t ldg, int64_t n_rows, i
     return scatter_rows_all<uint8_t>(G, ldg, n_rows, F, n_seg, inv, recv, recv_scale, ld_recv, div, stream);
 }
 
-// ---- the staged transport's pack (K3) and scatter (K5) with a bf16 wire side, and the exact widening ----
+extern "C" int bns_gather_div_f32(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
+                                  float *out, int64_t ldo, void *stream) {
+    return gather_div<float>(H, ldh, F, idx, k, div, out, ldo, nullptr, stream);
+}
+
+extern "C" int bns_scatter_add_div_f32(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
+                                       const float *src, int64_t lds, void *stream) {
+    return scatter_add_div<float>(G, ldg, F, idx, k, div, src, lds, nullptr, stream);
+}
+
+extern "C" int bns_gather_div_bf16(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
+                                   uint16_t *out, int64_t ldo, void *stream) {
+    return gather_div<uint16_t>(H, ldh, F, idx, k, div, out, ldo, nullptr, stream);
+}
+
+extern "C" int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
+                                        const uint16_t *src, int64_t lds, void *stream) {
+    return scatter_add_div<uint16_t>(G, ldg, F, idx, k, div, src, lds, nullptr, stream);
+}
+
+extern "C" int bns_gather_div_fp8(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
+                                  uint8_t *out, int64_t ldo, float *out_scale, void *stream) {
+    return gather_div<uint8_t>(H, ldh, F, idx, k, div, out, ldo, out_scale, stream);
+}
+
+extern "C" int bns_scatter_add_div_fp8(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
+                                       const uint8_t *src, int64_t lds, const float *src_scale, void *stream) {
+    return scatter_add_div<uint8_t>(G, ldg, F, idx, k, div, src, lds, src_scale, stream);
+}
+
+// ---- the exact widening of bf16 rows ----
 namespace {
 
 __global__ void __launch_bounds__(kThreads) cvt_rows_bf16_f32_kernel(const uint16_t *__restrict__ src, int64_t lds,
@@ -812,44 +884,7 @@ __global__ void __launch_bounds__(kThreads) cvt_rows_bf16_f32_kernel(const uint1
     }
 }
 
-inline bool bf16_rows_ok(const void *f32, const void *b16, int64_t F, int64_t ld32, int64_t ld16) {
-    return F % 8 == 0 && ld32 % 8 == 0 && ld16 % 8 == 0 &&
-           ((reinterpret_cast<uintptr_t>(f32) | reinterpret_cast<uintptr_t>(b16)) % 16) == 0;
-}
-
 }  // namespace
-
-extern "C" int bns_gather_div_bf16(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
-                                   uint16_t *out, int64_t ldo, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_gather_div_bf16: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(H && out && idx, "bns_gather_div_bf16: NULL pointer");
-    BNS_REQUIRE(ldh >= F && ldo >= F, "bns_gather_div_bf16: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_gather_div_bf16: division by zero");
-    BNS_REQUIRE(bf16_rows_ok(H, out, F, ldh, ldo),
-                "bns_gather_div_bf16: needs F, ldh, ldo multiples of 8 and 16-byte aligned H, out (F %lld, ldh %lld, "
-                "ldo %lld)", (long long)F, (long long)ldh, (long long)ldo);
-    rows_kernel<Bf16x8, false><<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, out, ldo, idx, k, (int32_t)F, div);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
-
-extern "C" int bns_scatter_add_div_bf16(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
-                                        const uint16_t *src, int64_t lds, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_scatter_add_div_bf16: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(G && src && idx, "bns_scatter_add_div_bf16: NULL pointer");
-    BNS_REQUIRE(ldg >= F && lds >= F, "bns_scatter_add_div_bf16: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_bf16: division by zero");
-    BNS_REQUIRE(bf16_rows_ok(G, src, F, ldg, lds),
-                "bns_scatter_add_div_bf16: needs F, ldg, lds multiples of 8 and 16-byte aligned G, src (F %lld, "
-                "ldg %lld, lds %lld)", (long long)F, (long long)ldg, (long long)lds);
-    rows_kernel<Bf16x8, true><<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, G, ldg, idx, k, (int32_t)F, div);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
 
 extern "C" int bns_cvt_rows_bf16_f32(const uint16_t *src, int64_t lds, float *dst, int64_t ldd, int64_t n_rows, int64_t F,
                                      void *stream) {
@@ -868,39 +903,8 @@ extern "C" int bns_cvt_rows_bf16_f32(const uint16_t *src, int64_t lds, float *ds
     return BNS_OK;
 }
 
-// ---- the staged transport's pack and scatter with an fp8 wire side, and the exact widening ----
+// ---- the exact widening of fp8 rows ----
 namespace {
-
-// one warp per row: out[i] / out_scale[i] = the fp8 row of H[idx[i]] / div (quantize_row_fp8)
-__global__ void __launch_bounds__(kThreads) gather_div_fp8_kernel(const float *__restrict__ H, int64_t ldh,
-                                                                  const int64_t *__restrict__ idx, int64_t k, int32_t F,
-                                                                  float div, uint8_t *__restrict__ out, int64_t ldo,
-                                                                  float *__restrict__ out_scale) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total)
-        quantize_row_fp8(H + idx[i] * ldh, div, F, out + i * ldo, out_scale + i, lane);
-}
-
-// one warp per row: G[idx[i]] += (src[i] * src_scale[i]) / div, the f32 scatter's arithmetic (E4m3x16::add_div)
-__global__ void __launch_bounds__(kThreads) scatter_add_div_fp8_kernel(const uint8_t *__restrict__ src, int64_t lds,
-                                                                       const float *__restrict__ src_scale,
-                                                                       const int64_t *__restrict__ idx, int64_t k,
-                                                                       int32_t F, float div, float *__restrict__ G,
-                                                                       int64_t ldg) {
-    const int lane = threadIdx.x & 31;
-    const int64_t warps_total = (int64_t)gridDim.x * kWarps;
-    for (int64_t i = (int64_t)blockIdx.x * kWarps + (threadIdx.x >> 5); i < k; i += warps_total) {
-        float *g = G + idx[i] * ldg;
-        const float s = src_scale[i];
-        for (int f = lane * 16; f < F; f += 512) {
-            E4m3x16 v;
-            v.load(g + f);
-            v.add_div(src + i * lds + f, s, div);
-            v.store(g + f);
-        }
-    }
-}
 
 // one thread per 16 codes: dst = codes * scale, exact
 __global__ void __launch_bounds__(kThreads) cvt_rows_fp8_f32_kernel(const uint8_t *__restrict__ codes, int64_t ldc,
@@ -922,55 +926,14 @@ __global__ void __launch_bounds__(kThreads) cvt_rows_fp8_f32_kernel(const uint8_
     }
 }
 
-// fp8 rows with an f32 side: F, both leading dimensions multiples of 16 (f32 side: of 4), 16-byte aligned matrices
-inline bool fp8_rows_ok(const void *f32, const void *codes, const void *scale, int64_t F, int64_t ld32, int64_t ld8) {
-    return F % 16 == 0 && ld32 % 4 == 0 && ld8 % 16 == 0 &&
-           ((reinterpret_cast<uintptr_t>(f32) | reinterpret_cast<uintptr_t>(codes)) % 16) == 0 &&
-           reinterpret_cast<uintptr_t>(scale) % 4 == 0;
-}
-
 }  // namespace
-
-extern "C" int bns_gather_div_fp8(const float *H, int64_t ldh, int64_t F, const int64_t *idx, int64_t k, float div,
-                                  uint8_t *out, int64_t ldo, float *out_scale, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_gather_div_fp8: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(H && out && out_scale && idx, "bns_gather_div_fp8: NULL pointer");
-    BNS_REQUIRE(ldh >= F && ldo >= F, "bns_gather_div_fp8: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_gather_div_fp8: division by zero");
-    BNS_REQUIRE(F <= 1024 && ldh % 16 == 0 && fp8_rows_ok(H, out, out_scale, F, ldh, ldo),
-                "bns_gather_div_fp8: needs F <= 1024, F, ldh, ldo multiples of 16, 16-byte aligned H, out and 4-byte "
-                "aligned scales (F %lld, ldh %lld, ldo %lld)", (long long)F, (long long)ldh, (long long)ldo);
-    gather_div_fp8_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(H, ldh, idx, k, (int32_t)F, div, out, ldo,
-                                                                             out_scale);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
-
-extern "C" int bns_scatter_add_div_fp8(float *G, int64_t ldg, int64_t F, const int64_t *idx, int64_t k, float div,
-                                       const uint8_t *src, int64_t lds, const float *src_scale, void *stream) {
-    BNS_REQUIRE(k >= 0 && F > 0, "bns_scatter_add_div_fp8: bad size");
-    if (k == 0) return BNS_OK;
-    BNS_REQUIRE(G && src && src_scale && idx, "bns_scatter_add_div_fp8: NULL pointer");
-    BNS_REQUIRE(ldg >= F && lds >= F, "bns_scatter_add_div_fp8: leading dimension smaller than F");
-    BNS_REQUIRE(div != 0.f, "bns_scatter_add_div_fp8: division by zero");
-    BNS_REQUIRE(fp8_rows_ok(G, src, src_scale, F, ldg, lds),
-                "bns_scatter_add_div_fp8: needs F, lds multiples of 16, ldg of 4, 16-byte aligned G, src and 4-byte "
-                "aligned scales (F %lld, ldg %lld, lds %lld)", (long long)F, (long long)ldg, (long long)lds);
-    scatter_add_div_fp8_kernel<<<rows_grid(k), kThreads, 0, as_stream(stream)>>>(src, lds, src_scale, idx, k, (int32_t)F,
-                                                                                  div, G, ldg);
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
-}
 
 extern "C" int bns_cvt_rows_fp8_f32(const uint8_t *codes, int64_t ldc, const float *scale, float *dst, int64_t ldd,
                                     int64_t n_rows, int64_t F, void *stream) {
     BNS_REQUIRE(n_rows >= 0 && F >= 0 && ldc >= F && ldd >= F, "bns_cvt_rows_fp8_f32: bad shape");
     if (n_rows == 0 || F == 0) return BNS_OK;
     BNS_REQUIRE(codes && scale && dst, "bns_cvt_rows_fp8_f32: NULL matrix");
-    BNS_REQUIRE(fp8_rows_ok(dst, codes, scale, F, ldd, ldc),
+    BNS_REQUIRE(rows_ok(dst, ldd, codes, ldc, scale, F),
                 "bns_cvt_rows_fp8_f32: needs F, ldc multiples of 16, ldd of 4, 16-byte aligned codes, dst and 4-byte "
                 "aligned scales (F %lld, ldc %lld, ldd %lld)", (long long)F, (long long)ldc, (long long)ldd);
     const int64_t work = n_rows * (F / 16);
