@@ -26,15 +26,18 @@ import numpy as np
 import torch
 
 from .partition import NID, GraphPartitionBook, LocalGraph, Partition, partition_graph
-from .synthetic import FullGraph, make_graph
+from .files import data_source, load_graph
+from .synthetic import FullGraph
 
 FORMAT_VERSION = 1
 _BOOL_KEYS = ("inner_node", "train_mask", "val_mask", "test_mask")
 
 
 def default_graph_name(args) -> str:
-    """main.py:17-23 of the reference."""
-    return '%s-%d-%s-%s-%s' % (args.dataset, args.n_partitions, args.partition_method,
+    """main.py:17-23 of the reference.  A graph read with ``--data-source files`` gets a ``files`` token after the
+    dataset (``reddit-files-2-metis-vol-induc``), so that its store is never taken for the generated shape's."""
+    dataset = args.dataset + ('-files' if data_source(args) == 'files' else '')
+    return '%s-%d-%s-%s-%s' % (dataset, args.n_partitions, args.partition_method,
                                getattr(args, 'partition_obj', 'vol'), 'induc' if args.inductive else 'trans')
 
 
@@ -43,6 +46,14 @@ def _dirs(args) -> Tuple[str, str]:
         args.graph_name = default_graph_name(args)
     graph_dir = os.path.join(args.part_path, args.graph_name)
     return graph_dir, os.path.join(graph_dir, args.graph_name + '.json')
+
+
+def _check_source(cfg: dict, args, part_config: str) -> None:
+    """Refuse a store built from the other ``--data-source`` (a config without the key was generated)."""
+    stored, wanted = cfg.get("data_source", "synthetic"), data_source(args)
+    if stored != wanted:
+        raise RuntimeError(f"{part_config} was partitioned from --data-source {stored}, this run reads --data-source "
+                           f"{wanted}; pick another --graph-name or remove the store")
 
 
 def _save_array(path: str, t: torch.Tensor) -> Dict[str, object]:
@@ -70,11 +81,15 @@ def save_partition(p: Partition, graph_dir: str) -> Dict[str, object]:
 
 
 def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch.device] = None) -> str:
-    """helper/utils.py:73-98: build the graph (``load_data`` -> the seeded generator here), partition it unless the
-    part config already exists, always (re)write ``meta.json``.  Returns the part-config path."""
+    """helper/utils.py:73-98: build the graph (``load_data`` -> ``load_graph``: the seeded generator, or the published
+    files with ``--data-source files``), partition it unless the part config already exists, always (re)write
+    ``meta.json``.  Returns the part-config path.  Nothing is written before the graph is built and checked."""
     graph_dir, part_config = _dirs(args)
+    if os.path.exists(part_config):
+        with open(part_config) as f:
+            _check_source(json.load(f), args, part_config)
     if fg is None:
-        fg = make_graph(args.dataset, seed=getattr(args, 'graph_seed', 0), device=device)
+        fg = load_graph(args, device)
     n_feat, n_class = fg.n_feat, fg.n_class
     n_train = int(fg.train_mask.sum())                     # utils.py:81 (after the inductive subgraph: the same count)
     os.makedirs(graph_dir, exist_ok=True)
@@ -82,8 +97,8 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
         parts = partition_graph(fg, args.n_partitions, args.partition_method, seed=getattr(args, 'graph_seed', 0),
                                 inductive=args.inductive, device=device,
                                 objective=getattr(args, 'partition_obj', 'vol'))
-        cfg = {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "num_parts": args.n_partitions,
-               "part_method": args.partition_method, "inductive": bool(args.inductive),
+        cfg = {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "data_source": data_source(args),
+               "num_parts": args.n_partitions, "part_method": args.partition_method, "inductive": bool(args.inductive),
                "node_map": [int(x) for x in parts[0].gpb.ranges.tolist()],
                "num_nodes": int(parts[0].gpb.ranges[-1]), "num_edges": int(sum(p.graph.num_edges() for p in parts))}
         for p in parts:
@@ -114,6 +129,7 @@ def load_partition(args, rank: int, device: Optional[torch.device] = None, mmap:
         cfg = json.load(f)
     if cfg.get("format_version") != FORMAT_VERSION:
         raise RuntimeError(f"{part_config}: format version {cfg.get('format_version')} != {FORMAT_VERSION}")
+    _check_source(cfg, args, part_config)
     if not 0 <= rank < cfg["num_parts"]:
         raise IndexError(f"part {rank} of {cfg['num_parts']}")
     if cfg["num_parts"] != args.n_partitions:

@@ -6,7 +6,8 @@ import argparse
 # (flag, type or None for a switch, default, extra argparse keywords)
 _REFERENCE_FLAGS = [
     ("dataset", str, "reddit", dict(help="synthetic shape to generate: reddit | ogbn-products | yelp | synthetic-10k | "
-                                         "small | tiny")),
+                                         "small | tiny; with --data-source files, the dataset to read: reddit | "
+                                         "ogbn-products | yelp")),
     ("data-path", str, "./dataset/", {}),
     ("part-path", str, "./partition/", {}),
     ("graph-name", str, "", {}),
@@ -65,6 +66,11 @@ def build_parser():
                         help="NEW: with --eval, every rank evaluates its own nodes on its partition (the whole halo "
                              "exchanged layer by layer) instead of rank 0 evaluating the full graph alone; the full "
                              "graph is never built.  Transductive runs only")
+    parser.add_argument(*_spellings("data-source"), default="synthetic", choices=["synthetic", "files"],
+                        help="NEW: where the graph comes from.  synthetic generates the --dataset shape from a seed.  "
+                             "files reads reddit, yelp or ogbn-products from the files DGL / OGB leave under "
+                             "--data-path (reddit/, yelp/, ogbn_products/raw and split/); the store's default graph "
+                             "name then carries a 'files' token")
     parser.add_argument(*_spellings("agg-dtype"), default="f32", choices=["f32", "bf16", "fp8"],
                         help="NEW: element type of the rows the wide (hidden-width) aggregation passes gather.  bf16 "
                              "rounds them to bf16 (nearest even) before each pass -- h_u forward, the transposed "

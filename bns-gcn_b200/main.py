@@ -1,6 +1,7 @@
-"""Launcher with the reference's flags (main.py:10-64): generate (instead of download) the graph, partition it into
-the on-disk store (``data/store.py``: ``graph_partition`` unless ``--skip-partition``), start one process per
-partition / GPU; each loads its part (``load_partition``) and runs ``train.run``.
+"""Launcher with the reference's flags (main.py:10-64): generate the graph (or read its published files with
+``--data-source files``; nothing is downloaded), partition it into the on-disk store (``data/store.py``:
+``graph_partition`` unless ``--skip-partition``), start one process per partition / GPU; each loads its part
+(``load_partition``) and runs ``train.run``.
 
     python -m bns_gcn_b200.main --dataset reddit --n-partitions 4 --model graphsage --n-layers 3 --n-hidden 256 \
         --sampling-rate 0.1 --use-pp --partition-method random --n-epochs 50 --no-eval

@@ -679,7 +679,8 @@ class GraphedEpoch:
 def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     """train.py:300-456.  With ``args.eval`` rank 0 also runs the evaluation / checkpoint branch (:308-321, 427-456)
     through ``evaluate.Evaluator`` -- on the GPU with the same kernels, synchronously, instead of a CPU thread pool;
-    ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: regenerated from ``args.dataset``).
+    ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: ``data.load_graph(args)``, regenerated or
+    read again from ``--data-path``).
     With ``args.parallel_eval`` as well, EVERY rank evaluates its own nodes on its partition instead
     (``evaluate.ParallelEvaluator``) and the full graph is never built; inductive runs are refused.
     ``args.save_state_every`` / ``args.resume``: write the training state every N epochs and after the last one, or
@@ -704,10 +705,9 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
         evaluator = ParallelEvaluator(args, eg, st.feat, st.labels, node_dict['val_mask'].to(dev),
                                       node_dict['test_mask'].to(dev), ctx.comm())
     elif getattr(args, 'eval', False) and rank == 0:
-        from .data import make_graph
+        from .data import load_graph
         from .evaluate import Evaluator
-        fg = full_graph if full_graph is not None else make_graph(args.dataset, seed=getattr(args, 'graph_seed', 0),
-                                                                  device=dev)
+        fg = full_graph if full_graph is not None else load_graph(args, dev)
         evaluator = Evaluator(args, fg, dev)
     start = 0
     if saved is not None:
