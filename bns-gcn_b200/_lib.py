@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -187,6 +187,17 @@ SIGNATURES = {
     "bns_cvt_rows_f32_fp8_any": (c_int, [c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int64, c_void_p]),
     "bns_dropout_fp8": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_float, c_uint64, c_uint64, c_void_p, c_void_p,
                                 c_int64, c_void_p, c_int64, c_void_p, c_void_p]),
+    # ---- ABI 10 ----
+    "bns_part_edges_workspace_bytes": (c_size_t, [c_int64]),
+    "bns_part_edges": (c_int, [c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
+                               c_int64, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p, c_size_t, c_void_p]),
+    "bns_part_conn": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p,
+                              c_void_p]),
+    "bns_part_gains": (c_int, [c_int32, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                               c_uint64, c_void_p, c_void_p, c_void_p]),
+    "bns_part_cluster": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_uint64,
+                                 c_void_p, c_void_p, c_void_p]),
+    "bns_part_weights": (c_int, [c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
 }
 
 

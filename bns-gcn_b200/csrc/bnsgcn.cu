@@ -8,6 +8,7 @@
 //   gather / scatter   K3/K5      boundary pack and gradient scatter-add, f32 or bf16 (--comm-dtype bf16) wire rows
 //   philox_key / take  K6         counter-based exactly-k sampling (with cub radix sort)
 //   p2p_put_rows       K3+C1      pack straight into the peer's receive slab over NVLink + flag
+//   part_*             partition.cuh: the multilevel partitioner (contraction, conn table, gains, clustering)
 //
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 --shared -Xcompiler -fPIC
 #include "bnsgcn.h"
@@ -16,6 +17,7 @@
 #include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_reduce.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <cstdarg>
@@ -2332,6 +2334,11 @@ extern "C" int bns_p2p_wait_flag(bns_p2p_t *p, int32_t flag_index, uint64_t flag
 #include "fused.cuh"
 #include "gat.cuh"
 #include "comm.cuh"
+
+// =================================================================================================
+// the multilevel partitioner's hot loops (--partition-method multilevel)
+// =================================================================================================
+#include "partition.cuh"
 
 // =================================================================================================
 // K8: dense layers on wgmma (3xTF32 with the operand split fused into the pipeline)

@@ -20,7 +20,7 @@ relies on (SURVEY.md §3.2):
 label propagation (``refine_label_propagation``) on the objective ``--partition-obj`` names (``cut``: edges between
 parts; ``vol``: communication volume = halo nodes summed over the parts, the reference's default, parser.py:35-36).
 It is structure-aware and never worse than its starting point, but it is not a multilevel partitioner: expect METIS to
-cut fewer edges on real graphs.  The contract is the same.
+cut fewer edges on real graphs.  ``multilevel`` is one, on the GPU (``data/multilevel.py``).  The contract is the same.
 """
 from __future__ import annotations
 
@@ -170,13 +170,17 @@ def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, ob
 
 
 def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective: str = "vol", device=None) -> torch.Tensor:
-    """Owner of every node, int64 ``[N]``: ``random`` balanced to ±1 node, ``metis`` (stand-in) within 3 %."""
+    """Owner of every node, int64 ``[N]``: ``random`` balanced to ±1 node, ``metis`` (stand-in) and ``multilevel`` (the
+    GPU partitioner; ``device`` None = the current CUDA device) within 3 %."""
     n = fg.n_nodes
     if n_parts == 1:
         return torch.zeros(n, dtype=torch.int64)
     if method == "random":
         gen = torch.Generator().manual_seed(seed + 7919)
         order = torch.randperm(n, generator=gen)
+    elif method == "multilevel":                      # the GPU partitioner (data/multilevel.py)
+        from .multilevel import multilevel_partition
+        return multilevel_partition(fg, n_parts, objective, seed, device)[0]
     elif method == "metis":
         import scipy.sparse as sp
         from scipy.sparse.csgraph import reverse_cuthill_mckee
@@ -273,7 +277,7 @@ def partition_graph(fg: FullGraph, n_parts: int, method: str = "random", seed: i
                     inductive: bool = False, ranks: Optional[List[int]] = None,
                     device: Optional[torch.device] = None, objective: str = "vol") -> List[Partition]:
     """``graph_partition`` + ``load_partition`` in one call; returns the pieces for ``ranks`` (default all).
-    ``objective``: ``--partition-obj`` (``vol`` | ``cut``), used by the ``metis`` stand-in only."""
+    ``objective``: ``--partition-obj`` (``vol`` | ``cut``), used by ``metis`` (the stand-in) and ``multilevel``."""
     if inductive:
         fg = induced_subgraph(fg, fg.train_mask)
     part = assign_parts(fg, n_parts, method, seed, objective, device)

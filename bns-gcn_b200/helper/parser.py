@@ -24,7 +24,11 @@ _REFERENCE_FLAGS = [
     ("weight-decay", float, 0, {}),
     ("norm", None, "layer", dict(choices=["layer", "batch"])),
     ("partition-obj", None, "vol", dict(choices=["vol", "cut"])),
-    ("partition-method", None, "metis", dict(choices=["metis", "random"])),
+    ("partition-method", None, "metis", dict(choices=["metis", "random", "multilevel"],
+                                             help="metis: the stand-in (reverse Cuthill-McKee blocks refined by balanced "
+                                                  "label propagation, on the host or the given device); random; "
+                                                  "NEW multilevel: a multilevel k-way partitioner on the GPU (coarsen, "
+                                                  "initial partition, refine on --partition-obj), 2 to 64 parts")),
     ("n-linear", int, 0, {}),
     ("use-pp", "switch", False, {}),
     ("inductive", "switch", False, {}),

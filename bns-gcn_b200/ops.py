@@ -685,3 +685,85 @@ class LnReluDropout(torch.autograd.Function):
 
 def ln_relu_dropout_supported(x: torch.Tensor, F: int) -> bool:
     return x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and F % 4 == 0 and F <= 1024
+
+
+# ---- the multilevel partitioner (data/multilevel.py): thin wrappers over the bns_part_* entry points ----
+
+def part_edges(indptr: torch.Tensor, idx: torch.Tensor, w: Optional[torch.Tensor], n_out_rows: int, mode: int,
+               drop_loops: bool, row_map: Optional[torch.Tensor] = None, col_map: Optional[torch.Tensor] = None):
+    """``bns_part_edges``: the merged (row_map[r], col_map[c]) CSR of a CSR; mode 0 as is, 1 transposed, 2 both.
+    Returns (indptr int64, idx int32, w int32), trimmed to the merged entry count.  Synchronises."""
+    _req(indptr, torch.int64, "indptr")
+    _req(idx, torch.int32, "idx")
+    for t, name in ((w, "w"), (row_map, "row_map"), (col_map, "col_map")):
+        if t is not None:
+            _req(t, torch.int32, name)
+    nnz = idx.numel()
+    cap = 2 * nnz if mode == 2 else nnz
+    dev = indptr.device
+    out_indptr = torch.empty(n_out_rows + 1, dtype=torch.int64, device=dev)
+    out_idx = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+    out_w = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+    ws = torch.empty(max(int(lib.bns_part_edges_workspace_bytes(cap)), 1), dtype=torch.uint8, device=dev)
+    n_out = ctypes.c_int64()
+    check(lib.bns_part_edges(indptr.numel() - 1, nnz, indptr.data_ptr(), _ptr(idx) if nnz else None, _ptr(w),
+                             _ptr(row_map), _ptr(col_map), mode, 1 if drop_loops else 0, n_out_rows,
+                             out_indptr.data_ptr(), out_idx.data_ptr(), out_w.data_ptr(), ctypes.byref(n_out),
+                             ws.data_ptr(), ws.numel(), _stream_ptr()), "bns_part_edges")
+    m = n_out.value
+    if m == 0:
+        return out_indptr, out_idx[:0], out_w[:0]           # views of one element: their data pointers are not NULL
+    return out_indptr, out_idx[:m].clone(), out_w[:m].clone()
+
+
+def part_conn(indptr: torch.Tensor, idx: torch.Tensor, w: Optional[torch.Tensor], part: torch.Tensor, n_parts: int, *,
+              table: bool = True, occ: bool = False, quality: bool = False):
+    """``bns_part_conn``: (conn int32 [n, P] or None, occ int64 [n] bit sets or None, quality int64 [2] (cut, vol) or None)."""
+    _req(part, torch.int32, "part")
+    n, dev = part.numel(), part.device
+    conn = torch.empty(n, n_parts, dtype=torch.int32, device=dev) if table else None
+    o = torch.empty(n, dtype=torch.int64, device=dev) if occ else None
+    q = torch.empty(2, dtype=torch.int64, device=dev) if quality else None
+    check(lib.bns_part_conn(n, indptr.data_ptr(), idx.data_ptr(), _ptr(w), part.data_ptr(), n_parts, _ptr(conn), _ptr(o),
+                            _ptr(q), _stream_ptr()), "bns_part_conn")
+    return conn, o, q
+
+
+def part_gains(objective: str, part: torch.Tensor, conn: torch.Tensor, n_parts: int, allowed: int, *,
+               in_graph=None, occ: Optional[torch.Tensor] = None):
+    """``bns_part_gains``: each node's best allowed target part (-1: none) and its exact gain (int64).  ``objective``
+    "cut": conn of the undirected weighted graph; "vol": conn / occ of the out-CSR and ``in_graph`` = (indptr, idx, w)
+    the in-CSR with multiplicities."""
+    _req(part, torch.int32, "part")
+    _req(conn, torch.int32, "conn")
+    n, dev = part.numel(), part.device
+    target = torch.empty(n, dtype=torch.int32, device=dev)
+    gain = torch.empty(n, dtype=torch.int64, device=dev)
+    ip, ix, iw = in_graph if in_graph is not None else (None, None, None)
+    check(lib.bns_part_gains(1 if objective == "vol" else 0, n, n_parts, _ptr(ip), _ptr(ix), _ptr(iw), part.data_ptr(),
+                             conn.data_ptr(), _ptr(occ), allowed & 0xFFFFFFFFFFFFFFFF, target.data_ptr(),
+                             gain.data_ptr(), _stream_ptr()), "bns_part_gains")
+    return target, gain
+
+
+def part_cluster(rating, label: torch.Tensor, nw: Optional[torch.Tensor], cw: torch.Tensor, cap: int, seed: int):
+    """``bns_part_cluster``: one size-constrained label-propagation proposal per node (target -1: stay)."""
+    _req(label, torch.int32, "label")
+    _req(cw, torch.int64, "cw")
+    ip, cid, wt = rating
+    n, dev = label.numel(), label.device
+    target = torch.empty(n, dtype=torch.int32, device=dev)
+    gain = torch.empty(n, dtype=torch.int64, device=dev)
+    check(lib.bns_part_cluster(n, ip.data_ptr(), cid.data_ptr(), wt.data_ptr(), label.data_ptr(), _ptr(nw), cw.data_ptr(),
+                               int(cap), seed & 0xFFFFFFFFFFFFFFFF, target.data_ptr(), gain.data_ptr(), _stream_ptr()),
+          "bns_part_cluster")
+    return target, gain
+
+
+def part_weights(label: torch.Tensor, nw: Optional[torch.Tensor], n_labels: int) -> torch.Tensor:
+    """``bns_part_weights``: int64 [n_labels] sums of the node weights per label."""
+    _req(label, torch.int32, "label")
+    out = torch.empty(n_labels, dtype=torch.int64, device=label.device)
+    check(lib.bns_part_weights(label.numel(), label.data_ptr(), _ptr(nw), n_labels, out.data_ptr(), _stream_ptr()),
+          "bns_part_weights")
+    return out

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 9
+#define BNS_ABI_VERSION 10
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -641,6 +641,51 @@ int bns_dropout_f32(const float *x, int64_t ldx, int64_t n, int64_t F, float p, 
 /* y[r, :] = x[r, :] * row_scale[r] + bias[:]      (row_scale / bias may be NULL: 1 / 0) */
 int bns_scale_rows_f32(const float *x, int64_t ldx, int64_t n, int64_t F, const float *row_scale, const float *bias, float *y,
                        int64_t ldy, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 10: the multilevel graph partitioner (--partition-method multilevel; data/multilevel.py runs the level loop).
+ * The reference partitions with METIS through dgl.distributed.partition_graph (helper/utils.py:94).  Graphs here are
+ * CSRs: indptr int64 [n+1], column ids int32, optional int32 weights (NULL = 1 each).  Every result is integer and
+ * independent of the order atomics land in, so two calls give bit-identical output.  Malformed arguments return
+ * BNS_E_INVALID before any launch.
+ * bns_part_edges: the entries (r, c, w) of the input, mapped to (row_map[r], col_map[c]) (NULL maps = identity), emitted
+ *     as (R, C) (mode 0), (C, R) (mode 1) or both (mode 2); with drop_loops, entries with R == C are dropped; equal
+ *     (R, C) are merged with their weights summed.  Output: a CSR with n_out_rows rows, columns ascending within a
+ *     row, capacity nnz (modes 0, 1) or 2 nnz (mode 2) entries; *out_nnz (host) = its entry count.  Every R must be
+ *     < n_out_rows (without a row map, modes 0 and 2 refuse n_rows > n_out_rows), and the summed weights must stay
+ *     < 2^31.  One radix sort of 64-bit keys and a reduce-by-key.
+ *     Synchronises the stream.  ws: bns_part_edges_workspace_bytes(nnz or 2 nnz).
+ * bns_part_conn: conn[v * P + p] (device int32 [n, P], or NULL) = sum of the weights of row v's entries whose column u
+ *     has part[u] == p; occ[v] (device [n], or NULL) = the bits p with conn[v][p] > 0; quality (device int64 [2], or
+ *     NULL) = { sum over v of conn[v][p] for p != part[v],  number of (v, p) with p != part[v] and conn[v][p] > 0 }:
+ *     on the out-CSR with multiplicities, the directed edge cut and the communication volume of partition_quality.
+ *     1 <= P <= 64.
+ * bns_part_gains: target[v] = the allowed part b != part[v] (bit b of `allowed`) with the largest gain, ties to the
+ *     lowest b, or -1; gain[v] its gain = objective before - objective after the move of v alone.  objective 0 (cut):
+ *     conn is the table of an undirected weighted graph, gain = conn[v][b] - conn[v][part[v]].  objective 1 (vol):
+ *     conn / occ are those of the out-CSR with multiplicities and (indptr, idx, w) the in-CSR with multiplicities, loops
+ *     dropped (bns_part_edges modes 1 and 0).  2 <= P <= 64.
+ * bns_part_cluster: one size-constrained label-propagation step.  (indptr, cid, cw_edge): per node v, the clusters of its
+ *     neighbours with the summed edge weight into each (bns_part_edges with col_map = label), cw: cluster weights.
+ *     target[v] = the heaviest neighbouring cluster c != label[v] with cw[c] + nw[v] <= cap, when it beats v's weight
+ *     into its own cluster (gain[v] = the difference), else -1.  Only the nodes whose coin (a hash of v and seed) is odd
+ *     propose.  nw NULL = 1 each.
+ * bns_part_weights: out[l] (device int64 [n_labels]) = sum of nw[v] (NULL = 1) over v with label[v] == l.
+ * ----------------------------------------------------------------------------------------------*/
+size_t bns_part_edges_workspace_bytes(int64_t n_entries);
+int bns_part_edges(int64_t n_rows, int64_t nnz, const int64_t *indptr, const int32_t *idx, const int32_t *w,
+                   const int32_t *row_map, const int32_t *col_map, int32_t mode, int32_t drop_loops, int64_t n_out_rows,
+                   int64_t *out_indptr, int32_t *out_idx, int32_t *out_w, int64_t *out_nnz /*host*/, void *ws,
+                   size_t ws_bytes, void *stream);
+int bns_part_conn(int64_t n, const int64_t *indptr, const int32_t *idx, const int32_t *w, const int32_t *part, int32_t P,
+                  int32_t *conn, uint64_t *occ, int64_t *quality, void *stream);
+int bns_part_gains(int32_t objective, int64_t n, int32_t P, const int64_t *indptr, const int32_t *idx, const int32_t *w,
+                   const int32_t *part, const int32_t *conn, const uint64_t *occ, uint64_t allowed, int32_t *target,
+                   int64_t *gain, void *stream);
+int bns_part_cluster(int64_t n, const int64_t *indptr, const int32_t *cid, const int32_t *cw_edge, const int32_t *label,
+                     const int32_t *nw, const int64_t *cw, int64_t cap, uint64_t seed, int32_t *target, int64_t *gain,
+                     void *stream);
+int bns_part_weights(int64_t n, const int32_t *label, const int32_t *nw, int64_t n_labels, int64_t *out, void *stream);
 
 #ifdef __cplusplus
 }
