@@ -44,15 +44,68 @@ def conn(indptr, idx, w, part, P):
     return c.int(), occ, (int(c[other].sum()), int((c[other] > 0).sum()))
 
 
-def best_target(g, part):
-    """bns_part_gains' choice from a full gain table [n, P]: the largest gain over the parts != own, ties to the lowest."""
+def best_target(g, part, allowed=None):
+    """bns_part_gains' choice from a full gain table [n, P]: the largest gain over the allowed parts != own (bit b of
+    ``allowed``, None = all), ties to the lowest; target -1 and gain 0 where no such part exists."""
     part = part.cpu().long()
     n, P = g.shape
     mask = torch.ones(n, P, dtype=torch.bool)
     mask[torch.arange(n), part] = False
+    if allowed is not None:
+        mask &= torch.tensor([(int(allowed) >> b) & 1 == 1 for b in range(P)])[None, :]
     gm = torch.where(mask, g, torch.full_like(g, -(1 << 62)))
     best = gm.max(1).values
-    return (gm == best[:, None]).int().argmax(1).int(), best
+    tgt = (gm == best[:, None]).int().argmax(1).int()
+    none = ~mask.any(1)
+    return torch.where(none, -1, tgt).int(), torch.where(none, 0, best)
+
+
+def cut_gains(indptr, idx, w, part, P, nodes):
+    """The edge-cut gain of moving v alone to b, [len(nodes), P] int64, from the definition: the sum over v's row of
+    w(u, v) ([part u = b] - [part u = a]), a = part v (0 at b = a)."""
+    indptr, idx, part = indptr.cpu().long(), idx.cpu().long(), part.cpu().long()
+    wt = w.cpu().long() if w is not None else torch.ones(idx.numel(), dtype=torch.int64)
+    out = torch.zeros(len(nodes), P, dtype=torch.int64)
+    for i, v in enumerate(nodes):
+        s, e = int(indptr[v]), int(indptr[v + 1])
+        a = int(part[v])
+        pu, wu = part[idx[s:e]], wt[s:e]
+        for b in range(P):
+            if b != a:
+                out[i, b] = int((wu * ((pu == b).long() - (pu == a).long())).sum())
+    return out
+
+
+def vol_gains(out_csr, in_csr, part, P, nodes):
+    """The communication-volume gain of moving v alone to b, [len(nodes), P] int64, by recomputing the terms that can
+    change: v's own (its out-neighbour parts other than its own) and each in-neighbour u's, from u's per-part out-edge
+    counts with v's m(u, v) edges taken out of a and put into b.  ``out_csr`` / ``in_csr``: the merged out- and in-CSRs
+    with multiplicities, loops dropped (bns_part_edges modes 1 and 0)."""
+    part = part.cpu().long()
+    cnt = conn(*out_csr, part, P)[0].long()                 # cnt[u][p]: u's out-edges into part p
+    ip, ix = in_csr[0].cpu().long(), in_csr[1].cpu().long()
+    iw = in_csr[2].cpu().long() if in_csr[2] is not None else torch.ones(ix.numel(), dtype=torch.int64)
+    ar = torch.arange(P)
+
+    def term(c, own):                                       # parts in c's support other than own, per row
+        return ((c > 0) & (ar[None, :] != own[:, None])).sum(1)
+
+    out = torch.zeros(len(nodes), P, dtype=torch.int64)
+    for i, v in enumerate(nodes):
+        a = int(part[v])
+        s, e = int(ip[v]), int(ip[v + 1])
+        u, m = ix[s:e], iw[s:e]
+        cu, pu = cnt[u], part[u]
+        before = int(term(cnt[v][None], part[v][None]).sum()) + int(term(cu, pu).sum())
+        for b in range(P):
+            if b == a:
+                continue
+            c2 = cu.clone()
+            c2[:, a] -= m
+            c2[:, b] += m
+            after = int(term(cnt[v][None], torch.tensor([b])).sum()) + int(term(c2, pu).sum())
+            out[i, b] = before - after
+    return out
 
 
 def part_hash(x):
@@ -89,6 +142,29 @@ def cluster_step(rating, label, nw, cw, cap, seed):
         if best is not None and -best[0] > cur:
             tgt[v], gain[v] = best[2], -best[0] - cur
     return tgt, gain
+
+
+def admit(nodes, to, gain, wt, frm, sizes, hi, lo=None, need_in=None, need_out=None):
+    """multilevel.admit, move by move: the admitted (node, target) pairs, sorted.  Per target, in (gain descending, id
+    ascending) order, a move is kept while the target's size plus the running weight of every candidate so far (kept or
+    not) is at most ``hi`` and, with ``need_in``, the weight before it is below the target's need; then the same per
+    source over the kept moves, with the floor ``lo`` and ``need_out``."""
+    L = [dict(v=int(nodes[i]), t=int(to[i]), g=int(gain[i]), w=int(wt[i]), f=int(frm[i])) for i in range(len(nodes))]
+    sizes = [int(s) for s in sizes]
+    kept, run = [], {}
+    for x in sorted(L, key=lambda x: (x["t"], -x["g"], x["v"])):
+        before = run.get(x["t"], 0)
+        run[x["t"]] = before + x["w"]
+        if sizes[x["t"]] + run[x["t"]] <= hi and (need_in is None or before < int(need_in[x["t"]])):
+            kept.append(x)
+    if lo is not None or need_out is not None:
+        L, kept, run = kept, [], {}
+        for x in sorted(L, key=lambda x: (x["f"], -x["g"], x["v"])):
+            before = run.get(x["f"], 0)
+            run[x["f"]] = before + x["w"]
+            if (lo is None or sizes[x["f"]] - run[x["f"]] >= lo) and (need_out is None or before < int(need_out[x["f"]])):
+                kept.append(x)
+    return sorted((x["v"], x["t"]) for x in kept)
 
 
 def directed_objective(src, dst, part, P):
@@ -151,6 +227,28 @@ def grid_graph(side):
     a = torch.cat([right, right + 1, down, down + side, i])
     b = torch.cat([right + 1, right, down + side, down, i])
     return graph_from_edges(side * side, a, b)
+
+
+def equal_planted_blocks(n, n_blocks, deg_in, deg_out, seed=0):
+    """A symmetric planted partition with ``n_blocks`` blocks of equal size (n / n_blocks, rounded), so that the planted
+    grouping lies inside the partitioner's size bounds at any block count: ``deg_in`` / 2 edges per node drawn inside its
+    block, ``deg_out`` / 2 anywhere, duplicates and loops merged away, then one loop per node.  Returns the graph and
+    the planted grouping (int64 [n])."""
+    g = torch.Generator().manual_seed(seed)
+    blk = (torch.arange(n) % n_blocks)[torch.randperm(n, generator=g)]
+    order = torch.argsort(blk, stable=True)
+    sizes = torch.bincount(blk, minlength=n_blocks)
+    starts = torch.cumsum(sizes, 0) - sizes
+    m_in, m_out = n * deg_in // 2, n * deg_out // 2
+    u = torch.randint(0, n, (m_in,), generator=g)
+    v = order[starts[blk[u]] + (torch.rand(m_in, generator=g) * sizes[blk[u]]).long().clamp(max=sizes[blk[u]] - 1)]
+    a = torch.cat([u, torch.randint(0, n, (m_out,), generator=g)])
+    b = torch.cat([v, torch.randint(0, n, (m_out,), generator=g)])
+    keep = a != b
+    lo, hi = torch.minimum(a[keep], b[keep]), torch.maximum(a[keep], b[keep])
+    key = torch.unique(lo * n + hi)
+    lo, hi = key // n, key % n
+    return graph_from_edges(n, torch.cat([lo, hi, torch.arange(n)]), torch.cat([hi, lo, torch.arange(n)])), blk
 
 
 def degree_corrected_blocks(n, n_blocks, avg_deg, mix, seed=0, alpha=2.5):

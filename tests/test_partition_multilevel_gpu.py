@@ -90,7 +90,7 @@ def test_clustering_respects_the_cap_and_contraction_is_exact(built, name):
 
 
 @pytest.mark.parametrize("name", sorted(_graphs()))
-@pytest.mark.parametrize("P", [2, 3, 5])
+@pytest.mark.parametrize("P", [2, 3, 5, 31, 32, 33, 63, 64])
 def test_conn_and_quality_are_exact(built, name, P):
     from bns_gcn_b200 import ops
     from bns_gcn_b200.data import partition_quality
@@ -111,11 +111,12 @@ def test_conn_and_quality_are_exact(built, name, P):
 
 @pytest.mark.parametrize("name", sorted(_graphs()))
 @pytest.mark.parametrize("objective", ["cut", "vol"])
-def test_every_gain_is_the_single_move_delta(built, name, objective):
+@pytest.mark.parametrize("P", [4, 31, 32, 33, 63, 64])
+def test_every_gain_is_the_single_move_delta(built, P, name, objective):
     """gain(v, b) == objective(before) - objective(after) of moving v alone to b, for every node and every target."""
     from bns_gcn_b200 import ops
     fg = _graphs()[name]
-    n, P = fg.n_nodes, 4
+    n = fg.n_nodes
     ip, ix = _csr(fg)
     part = torch.randint(0, P, (n,), generator=torch.Generator().manual_seed(7)).to(DEV, torch.int32)
     if objective == "cut":
