@@ -12,7 +12,10 @@
 //   part_gain_kernel     each node's best target among the allowed parts and its exact gain: the weighted edge cut
 //                        from conn, or the communication volume from the out-edge counts of the in-neighbours
 //   part_cluster_kernel  size-constrained label propagation: each node's heaviest neighbouring cluster with room
-//   part_weight_kernel   integer weight sums per label (part sizes, cluster weights)
+//                        (kEdges: room under the node-weight cap and under the int64 in-edge cap, --partition-balance
+//                        edges)
+//   part_weight_kernel   integer weight sums per label (part sizes, cluster weights; int32 node weights or int64
+//                        in-edge weights)
 // Rows are walked by one warp per node: the longest rows of the Reddit shape hold about 19 k entries.
 
 namespace {
@@ -234,8 +237,10 @@ __global__ void __launch_bounds__(kThreads) part_gain_kernel(int64_t n, int P, c
 
 // One label-propagation step.  The rating CSR lists, for node v, (cluster c, total weight of v's edges into c), sorted
 // by c.  A node whose coin (hash of node and seed) comes up odd proposes the heaviest neighbouring cluster other than
-// its own that still has room for it (cw[c] + nw[v] <= cap; ties: the lower seeded hash, then the lower id), if that
-// weight beats its connection to its own cluster.  Otherwise target = -1.
+// its own that still has room for it (cw[c] + nw[v] <= cap and, with kEdges, ce[c] + ew[v] <= ecap; ties: the lower
+// seeded hash, then the lower id), if that weight beats its connection to its own cluster.  Otherwise target = -1.
+// The in-edge arguments come last, so that kEdges == false reads its parameters where the one-cap kernel did.
+template <bool kEdges>
 __global__ void __launch_bounds__(kThreads) part_cluster_kernel(int64_t n, const int64_t *__restrict__ indptr,
                                                                 const int32_t *__restrict__ cid,
                                                                 const int32_t *__restrict__ cw_edge,
@@ -243,7 +248,9 @@ __global__ void __launch_bounds__(kThreads) part_cluster_kernel(int64_t n, const
                                                                 const int32_t *__restrict__ nw,
                                                                 const int64_t *__restrict__ cw, int64_t cap,
                                                                 uint64_t seed, int32_t *__restrict__ target,
-                                                                int64_t *__restrict__ gain) {
+                                                                int64_t *__restrict__ gain,
+                                                                const int64_t *__restrict__ ew,
+                                                                const int64_t *__restrict__ ce, int64_t ecap) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t v = blockIdx.x * (int64_t)kWarps + warp;
     if (v >= n) return;
@@ -254,6 +261,7 @@ __global__ void __launch_bounds__(kThreads) part_cluster_kernel(int64_t n, const
     }
     const int32_t own = label[v];
     const int64_t wv = nw ? nw[v] : 1;
+    const int64_t ev = kEdges ? ew[v] : 0;
     long long cur = 0, best = -1;
     uint32_t best_h = 0;
     int bc = -1;
@@ -262,6 +270,7 @@ __global__ void __launch_bounds__(kThreads) part_cluster_kernel(int64_t n, const
         const long long wt = cw_edge[k];
         if (c == own) { cur = wt; continue; }
         if (cw[c] + wv > cap) continue;
+        if (kEdges && ce[c] + ev > ecap) continue;
         const uint32_t h = part_hash(seed + (uint64_t)c);
         if (bc < 0 || wt > best || (wt == best && (h < best_h || (h == best_h && c < bc)))) {
             best = wt; best_h = h; bc = c;
@@ -283,7 +292,8 @@ __global__ void __launch_bounds__(kThreads) part_cluster_kernel(int64_t n, const
     }
 }
 
-__global__ void part_weight_kernel(int64_t n, const int32_t *__restrict__ label, const int32_t *__restrict__ nw,
+template <typename W>
+__global__ void part_weight_kernel(int64_t n, const int32_t *__restrict__ label, const W *__restrict__ nw,
                                    unsigned long long *__restrict__ out) {
     const int64_t v = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
     if (v < n) atomicAdd(out + label[v], (unsigned long long)(nw ? nw[v] : 1));
@@ -401,8 +411,38 @@ extern "C" int bns_part_cluster(int64_t n, const int64_t *indptr, const int32_t 
     BNS_REQUIRE(n == 0 || (cw_edge && label && cw && target && gain), "bns_part_cluster: NULL argument");
     BNS_REQUIRE(cap >= 1, "bns_part_cluster: cap %lld < 1", (long long)cap);
     if (n == 0) return BNS_OK;
-    part_cluster_kernel<<<part_warp_grid(n), kThreads, 0, as_stream(stream)>>>(n, indptr, cid, cw_edge, label, nw, cw,
-                                                                               cap, seed, target, gain);
+    part_cluster_kernel<false><<<part_warp_grid(n), kThreads, 0, as_stream(stream)>>>(
+        n, indptr, cid, cw_edge, label, nw, cw, cap, seed, target, gain, nullptr, nullptr, 0);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+extern "C" int bns_part_cluster_edges(int64_t n, const int64_t *indptr, const int32_t *cid, const int32_t *cw_edge,
+                                      const int32_t *label, const int32_t *nw, const int64_t *cw, int64_t cap,
+                                      const int64_t *ew, const int64_t *ce, int64_t ecap, uint64_t seed,
+                                      int32_t *target, int64_t *gain, void *stream) {
+    BNS_REQUIRE(part_graph_ok(n, indptr, cid), "bns_part_cluster_edges: bad rating graph");
+    BNS_REQUIRE(n == 0 || (cw_edge && label && cw && ew && ce && target && gain), "bns_part_cluster_edges: NULL argument");
+    BNS_REQUIRE(cap >= 1 && ecap >= 1, "bns_part_cluster_edges: cap %lld or in-edge cap %lld < 1", (long long)cap,
+                (long long)ecap);
+    if (n == 0) return BNS_OK;
+    part_cluster_kernel<true><<<part_warp_grid(n), kThreads, 0, as_stream(stream)>>>(
+        n, indptr, cid, cw_edge, label, nw, cw, cap, seed, target, gain, ew, ce, ecap);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+template <typename W>
+static int part_weights(const char *what, int64_t n, const int32_t *label, const W *nw, int64_t n_labels, int64_t *out,
+                 void *stream) {
+    BNS_REQUIRE(n >= 0 && n < INT32_MAX && n_labels >= 1 && n_labels < INT32_MAX, "%s: bad size", what);
+    BNS_REQUIRE(out && (n == 0 || label), "%s: NULL argument", what);
+    cudaStream_t st = as_stream(stream);
+    BNS_CUDA(cudaMemsetAsync(out, 0, (size_t)n_labels * sizeof(int64_t), st));
+    if (n == 0) return BNS_OK;
+    part_weight_kernel<W><<<part_grid(n), kThreads, 0, st>>>(n, label, nw, reinterpret_cast<unsigned long long *>(out));
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;
@@ -410,13 +450,10 @@ extern "C" int bns_part_cluster(int64_t n, const int64_t *indptr, const int32_t 
 
 extern "C" int bns_part_weights(int64_t n, const int32_t *label, const int32_t *nw, int64_t n_labels, int64_t *out,
                                 void *stream) {
-    BNS_REQUIRE(n >= 0 && n < INT32_MAX && n_labels >= 1 && n_labels < INT32_MAX, "bns_part_weights: bad size");
-    BNS_REQUIRE(out && (n == 0 || label), "bns_part_weights: NULL argument");
-    cudaStream_t st = as_stream(stream);
-    BNS_CUDA(cudaMemsetAsync(out, 0, (size_t)n_labels * sizeof(int64_t), st));
-    if (n == 0) return BNS_OK;
-    part_weight_kernel<<<part_grid(n), kThreads, 0, st>>>(n, label, nw, reinterpret_cast<unsigned long long *>(out));
-    ++g_launches;
-    BNS_CUDA(cudaGetLastError());
-    return BNS_OK;
+    return part_weights("bns_part_weights", n, label, nw, n_labels, out, stream);
+}
+
+extern "C" int bns_part_weights_i64(int64_t n, const int32_t *label, const int64_t *nw, int64_t n_labels, int64_t *out,
+                                    void *stream) {
+    return part_weights("bns_part_weights_i64", n, label, nw, n_labels, out, stream);
 }

@@ -21,6 +21,12 @@ label propagation (``refine_label_propagation``) on the objective ``--partition-
 parts; ``vol``: communication volume = halo nodes summed over the parts, the reference's default, parser.py:35-36).
 It is structure-aware and never worse than its starting point, but it is not a multilevel partitioner: expect METIS to
 cut fewer edges on real graphs.  ``multilevel`` is one, on the GPU (``data/multilevel.py``).  The contract is the same.
+
+``--partition-balance`` picks what every method balances.  ``nodes`` (the default): each part's node count lies in
+``[max(int(0.97 N / P), 1), int(1.03 N / P) + 1]``.  ``edges``: those node bounds, and each part's in-edge count (the
+directed edges whose destination it owns, loops included: the nnz of its ``a_in`` plus ``a_out`` rows) is at most
+``in_edge_bound`` = ``int(1.03 E / P)`` plus the largest in-degree, the slack of one indivisible node.  A rank's
+aggregation work is its in-edges, so on power-law graphs a node-balanced part can carry twice the mean rank's work.
 """
 from __future__ import annotations
 
@@ -33,6 +39,44 @@ import torch
 from .synthetic import FullGraph
 
 NID = "_ID"   # the key DGL uses for ``dgl.NID``
+BALANCES = ("nodes", "edges")
+IMBALANCE = 0.03
+
+
+def in_edge_bound(in_edges: torch.Tensor, n_parts: int, imbalance: float = IMBALANCE) -> int:
+    """``--partition-balance edges``: the most in-edges a part may own, ``int((1 + imbalance) E / P)`` plus the largest
+    in-degree (``in_edges``: every node's in-edge count, loops included)."""
+    if in_edges.numel() == 0:
+        return 0
+    return int((1.0 + imbalance) * int(in_edges.sum()) / n_parts) + int(in_edges.max())
+
+
+def check_balance(balance: str) -> None:
+    if balance not in BALANCES:
+        raise ValueError(f"--partition-balance must be one of {', '.join(BALANCES)}, got {balance!r}")
+
+
+def check_bounds(fg: FullGraph, part: torch.Tensor, n_parts: int, method: str, balance: str) -> None:
+    """Raise unless every part of ``part`` is within the node bounds and, with ``edges``, the in-edge bound; the
+    message names the bound and the first part outside it."""
+    n = fg.n_nodes
+    lo, hi = max(int((1.0 - IMBALANCE) * n / n_parts), 1), int((1.0 + IMBALANCE) * n / n_parts) + 1
+    part = part.cpu()
+    sizes = torch.bincount(part, minlength=n_parts)
+    bad = torch.nonzero((sizes < lo) | (sizes > hi), as_tuple=True)[0]
+    if bad.numel():
+        p = int(bad[0])
+        raise RuntimeError(f"--partition-method {method} --partition-balance {balance}: part {p} has {int(sizes[p])} "
+                           f"nodes, outside the node bounds [{lo}, {hi}]")
+    if balance == "edges":
+        deg = fg.in_degrees()
+        ehi = in_edge_bound(deg, n_parts)
+        esizes = torch.zeros(n_parts, dtype=torch.int64).index_add_(0, part, deg)
+        bad = torch.nonzero(esizes > ehi, as_tuple=True)[0]
+        if bad.numel():
+            p = int(bad[0])
+            raise RuntimeError(f"--partition-method {method} --partition-balance edges: part {p} owns "
+                               f"{int(esizes[p])} in-edges, above the in-edge bound {ehi} = int(1.03 E / P) + d_max")
 
 
 @dataclasses.dataclass
@@ -75,9 +119,42 @@ class Partition:
     meta: Dict[str, int]
 
 
+def shed_in_edges(part: torch.Tensor, in_edges: torch.Tensor, n_parts: int, bound: int, method: str) -> torch.Tensor:
+    """Bring every part's in-edges within ``bound`` without changing any part's node count: while a part is above it,
+    its highest in-degree nodes are swapped, one for one, with the lowest in-degree nodes of the part with the fewest
+    in-edges (ties: the lower id), as few pairs as bring the heavy part down to the mean ``E / P`` or the light part up
+    to it.  Raises, naming the bound and the part, when a swap can no longer help."""
+    part = part.clone()
+    target = -(-int(in_edges.sum()) // n_parts)
+    for _ in range(4 * n_parts + 8):
+        esizes = torch.zeros(n_parts, dtype=torch.int64).index_add_(0, part, in_edges)
+        a = int(torch.argmax(esizes))
+        if int(esizes[a]) <= bound:
+            return part
+        b = int(torch.argmin(esizes))
+        want = min(int(esizes[a]) - target, target - int(esizes[b]))
+        heavy = torch.nonzero(part == a, as_tuple=True)[0]
+        light = torch.nonzero(part == b, as_tuple=True)[0]
+        heavy = heavy[torch.sort(-in_edges[heavy], stable=True)[1]]
+        light = light[torch.sort(in_edges[light], stable=True)[1]]
+        k = min(heavy.numel(), light.numel())
+        net = torch.cumsum(in_edges[heavy[:k]] - in_edges[light[:k]], 0)
+        reach = torch.nonzero(net >= want, as_tuple=True)[0]
+        m = int(reach[0]) + 1 if reach.numel() else int(torch.argmax(net)) + 1 if k else 0
+        if m == 0 or int(net[m - 1]) <= 0:
+            break
+        part[heavy[:m]], part[light[:m]] = b, a
+    esizes = torch.zeros(n_parts, dtype=torch.int64).index_add_(0, part, in_edges)
+    a = int(torch.argmax(esizes))
+    raise RuntimeError(f"--partition-method {method} --partition-balance edges: part {a} owns {int(esizes[a])} "
+                       f"in-edges, above the in-edge bound {bound} = int(1.03 E / P) + d_max, and no swap of nodes "
+                       "lowers it")
+
+
 def partition_quality(fg: FullGraph, part: torch.Tensor, n_parts: int, device=None) -> Dict[str, float]:
     """``cut``: directed non-loop edges whose ends have different owners; ``vol``: communication volume =
-    sum over parts of their halo size (distinct (source node, destination part) pairs across parts); sizes."""
+    sum over parts of their halo size (distinct (source node, destination part) pairs across parts); sizes; the fewest
+    and most in-edges a part owns (directed edges by the owner of their destination, loops included)."""
     dev = torch.device(device) if device is not None else torch.device("cpu")
     part = part.to(dev)
     src, dst = fg.src.to(dev), fg.dst().to(dev)
@@ -86,18 +163,21 @@ def partition_quality(fg: FullGraph, part: torch.Tensor, n_parts: int, device=No
     cut = int(cross.sum())
     vol = int(torch.unique(src[cross] * n_parts + pd[cross]).numel())
     sizes = torch.bincount(part, minlength=n_parts)
+    in_edges = torch.bincount(pd, minlength=n_parts)
     return {"cut": cut, "vol": vol, "edges": int((src != dst).sum()), "max_size": int(sizes.max()),
-            "min_size": int(sizes.min())}
+            "min_size": int(sizes.min()), "min_in_edges": int(in_edges.min()), "max_in_edges": int(in_edges.max())}
 
 
 def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, objective: str = "vol",
-                             rounds: int = 24, imbalance: float = 0.03, seed: int = 0, device=None) -> torch.Tensor:
+                             rounds: int = 24, imbalance: float = 0.03, seed: int = 0, device=None,
+                             in_edge_cap: Optional[int] = None) -> torch.Tensor:
     """Balanced label propagation: every round each node looks at the owners of its neighbours, the nodes that would
     gain most by joining the majority owner move -- as many as the target part has room for under the size cap
     ``(1 + imbalance) N / P`` (and the source part above the floor ``(1 - imbalance) N / P``), and only a random half of
     them per round (simultaneous moves of neighbours can undo
-    each other).  A round that does not improve ``objective`` ("cut" | "vol") is rolled back (three in a row end the
-    refinement), so the result is never worse than the input.  Pure torch (sorting / unique / scatter): runs on
+    each other).  With ``in_edge_cap``, a move is also admitted only while its target part's in-edges (loops included)
+    stay within the cap, counted the same way as the room.  A round that does not improve ``objective`` ("cut" |
+    "vol") is rolled back (three in a row end the refinement), so the result is never worse than the input.  Pure torch (sorting / unique / scatter): runs on
     ``device``."""
     dev = torch.device(device) if device is not None else torch.device("cpu")
     n, P = fg.n_nodes, n_parts
@@ -110,6 +190,7 @@ def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, ob
     part = part.to(dev).clone()
     cap = int((1.0 + imbalance) * n / P) + 1
     floor = max(int((1.0 - imbalance) * n / P), 1)
+    deg = fg.in_degrees().to(dev) if in_edge_cap is not None else None
 
     def score(p):
         ps, pd = p[src], p[dst]
@@ -146,6 +227,11 @@ def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, ob
         first = torch.searchsorted(tgt, torch.arange(P, device=dev))
         rank = torch.arange(cand.numel(), device=dev) - first[tgt]
         ok = rank < room[tgt]
+        if deg is not None:                                          # and the target's in-edges under their cap
+            esizes = torch.zeros(P, dtype=torch.int64, device=dev).index_add_(0, part, deg)
+            cs = torch.cumsum(deg[cand], 0)
+            before = torch.where(first > 0, cs[(first - 1).clamp(min=0)], torch.zeros_like(first))
+            ok &= esizes[tgt] + cs - before[tgt] <= in_edge_cap
         movers, to = cand[ok], tgt[ok]
         if movers.numel():                                           # nor may a part shrink below the floor
             frm = part[movers]
@@ -169,9 +255,12 @@ def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, ob
     return part.cpu()
 
 
-def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective: str = "vol", device=None) -> torch.Tensor:
+def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective: str = "vol", device=None,
+                 balance: str = "nodes") -> torch.Tensor:
     """Owner of every node, int64 ``[N]``: ``random`` balanced to ±1 node, ``metis`` (stand-in) and ``multilevel`` (the
-    GPU partitioner; ``device`` None = the current CUDA device) within 3 %."""
+    GPU partitioner; ``device`` None = the current CUDA device) within 3 %.  ``balance="edges"``: every method keeps
+    each part within the node bounds and the in-edge bound (``in_edge_bound``), or raises naming the bound and part."""
+    check_balance(balance)
     n = fg.n_nodes
     if n_parts == 1:
         return torch.zeros(n, dtype=torch.int64)
@@ -180,7 +269,7 @@ def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective:
         order = torch.randperm(n, generator=gen)
     elif method == "multilevel":                      # the GPU partitioner (data/multilevel.py)
         from .multilevel import multilevel_partition
-        return multilevel_partition(fg, n_parts, objective, seed, device)[0]
+        return multilevel_partition(fg, n_parts, objective, seed, device, balance)[0]
     elif method == "metis":
         import scipy.sparse as sp
         from scipy.sparse.csgraph import reverse_cuthill_mckee
@@ -190,8 +279,16 @@ def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective:
         raise ValueError(f"unknown partition method {method!r}")
     part = torch.empty(n, dtype=torch.int64)
     part[order] = (torch.arange(n, dtype=torch.int64) * n_parts) // n
+    ehi = None
+    if balance == "edges":                            # the same blocks with their in-edges evened out by swaps
+        deg = fg.in_degrees()
+        ehi = in_edge_bound(deg, n_parts)
+        part = shed_in_edges(part, deg, n_parts, ehi, method)
     if method == "metis":
-        part = refine_label_propagation(fg, part, n_parts, objective=objective, seed=seed, device=device)
+        part = refine_label_propagation(fg, part, n_parts, objective=objective, seed=seed, device=device,
+                                        in_edge_cap=ehi)
+    if balance == "edges":
+        check_bounds(fg, part, n_parts, method, balance)
     return part
 
 
@@ -275,12 +372,15 @@ def extract_partition(g: FullGraph, ranges: torch.Tensor, rank: int, inductive: 
 
 def partition_graph(fg: FullGraph, n_parts: int, method: str = "random", seed: int = 0,
                     inductive: bool = False, ranks: Optional[List[int]] = None,
-                    device: Optional[torch.device] = None, objective: str = "vol") -> List[Partition]:
+                    device: Optional[torch.device] = None, objective: str = "vol",
+                    balance: str = "nodes") -> List[Partition]:
     """``graph_partition`` + ``load_partition`` in one call; returns the pieces for ``ranks`` (default all).
-    ``objective``: ``--partition-obj`` (``vol`` | ``cut``), used by ``metis`` (the stand-in) and ``multilevel``."""
+    ``objective``: ``--partition-obj`` (``vol`` | ``cut``), used by ``metis`` (the stand-in) and ``multilevel``.
+    ``balance``: ``--partition-balance`` (``nodes`` | ``edges``), for every method; under ``inductive`` the bounds are
+    those of the train-node subgraph."""
     if inductive:
         fg = induced_subgraph(fg, fg.train_mask)
-    part = assign_parts(fg, n_parts, method, seed, objective, device)
+    part = assign_parts(fg, n_parts, method, seed, objective, device, balance)
     g, ranges = relabel(fg, part, n_parts, device)
     in_deg, out_deg = g.in_degrees(), g.out_degrees()
     if ranks is None:

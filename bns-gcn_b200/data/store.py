@@ -33,12 +33,19 @@ FORMAT_VERSION = 1
 _BOOL_KEYS = ("inner_node", "train_mask", "val_mask", "test_mask")
 
 
+def partition_balance(args) -> str:
+    """``--partition-balance``; an ``args`` built without the field balances node counts."""
+    return getattr(args, 'partition_balance', 'nodes')
+
+
 def default_graph_name(args) -> str:
     """main.py:17-23 of the reference.  A graph read with ``--data-source files`` gets a ``files`` token after the
-    dataset (``reddit-files-2-metis-vol-induc``), so that its store is never taken for the generated shape's."""
+    dataset (``reddit-files-2-metis-vol-induc``), so that its store is never taken for the generated shape's; an
+    edge-balanced partition gets an ``edges`` token after the objective (``reddit-4-metis-vol-edges-induc``)."""
     dataset = args.dataset + ('-files' if data_source(args) == 'files' else '')
-    return '%s-%d-%s-%s-%s' % (dataset, args.n_partitions, args.partition_method,
-                               getattr(args, 'partition_obj', 'vol'), 'induc' if args.inductive else 'trans')
+    obj = getattr(args, 'partition_obj', 'vol') + ('-edges' if partition_balance(args) == 'edges' else '')
+    return '%s-%d-%s-%s-%s' % (dataset, args.n_partitions, args.partition_method, obj,
+                               'induc' if args.inductive else 'trans')
 
 
 def _dirs(args) -> Tuple[str, str]:
@@ -54,6 +61,14 @@ def _check_source(cfg: dict, args, part_config: str) -> None:
     if stored != wanted:
         raise RuntimeError(f"{part_config} was partitioned from --data-source {stored}, this run reads --data-source "
                            f"{wanted}; pick another --graph-name or remove the store")
+
+
+def _check_balance(cfg: dict, args, part_config: str) -> None:
+    """Refuse a store partitioned under the other ``--partition-balance`` (a config without the key balanced nodes)."""
+    stored, wanted = cfg.get("balance", "nodes"), partition_balance(args)
+    if stored != wanted:
+        raise RuntimeError(f"{part_config} was partitioned with --partition-balance {stored}, this run asks for "
+                           f"--partition-balance {wanted}; pick another --graph-name or remove the store")
 
 
 def _save_array(path: str, t: torch.Tensor) -> Dict[str, object]:
@@ -87,7 +102,9 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
     graph_dir, part_config = _dirs(args)
     if os.path.exists(part_config):
         with open(part_config) as f:
-            _check_source(json.load(f), args, part_config)
+            cfg = json.load(f)
+        _check_source(cfg, args, part_config)
+        _check_balance(cfg, args, part_config)
     if fg is None:
         fg = load_graph(args, device)
     n_feat, n_class = fg.n_feat, fg.n_class
@@ -96,9 +113,10 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
     if not os.path.exists(part_config):                    # utils.py:86
         parts = partition_graph(fg, args.n_partitions, args.partition_method, seed=getattr(args, 'graph_seed', 0),
                                 inductive=args.inductive, device=device,
-                                objective=getattr(args, 'partition_obj', 'vol'))
+                                objective=getattr(args, 'partition_obj', 'vol'), balance=partition_balance(args))
         cfg = {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "data_source": data_source(args),
                "num_parts": args.n_partitions, "part_method": args.partition_method, "inductive": bool(args.inductive),
+               "balance": partition_balance(args),
                "node_map": [int(x) for x in parts[0].gpb.ranges.tolist()],
                "num_nodes": int(parts[0].gpb.ranges[-1]), "num_edges": int(sum(p.graph.num_edges() for p in parts))}
         for p in parts:
@@ -130,6 +148,7 @@ def load_partition(args, rank: int, device: Optional[torch.device] = None, mmap:
     if cfg.get("format_version") != FORMAT_VERSION:
         raise RuntimeError(f"{part_config}: format version {cfg.get('format_version')} != {FORMAT_VERSION}")
     _check_source(cfg, args, part_config)
+    _check_balance(cfg, args, part_config)
     if not 0 <= rank < cfg["num_parts"]:
         raise IndexError(f"part {rank} of {cfg['num_parts']}")
     if cfg["num_parts"] != args.n_partitions:

@@ -101,6 +101,12 @@ def build_parser():
                              "where a per-row scale does not factor out.  Master weights, gradients, the all-reduce, "
                              "Adam, the loss and evaluation stay f32.  Only with the fused training step (GraphSAGE / "
                              "GCN, --use-pp, --norm layer, no --n-linear)")
+    parser.add_argument(*_spellings("partition-balance"), default="nodes", choices=["nodes", "edges"],
+                        help="NEW: what every --partition-method balances.  nodes: each part's node count within 3 %% "
+                             "of N / P.  edges: that, and each part's in-edges (the edges whose destination it owns, "
+                             "loops included: a rank's aggregation work) at most int(1.03 E / P) plus the largest "
+                             "in-degree; a method that cannot meet a bound raises.  The store's default graph name "
+                             "then carries an 'edges' token")
     parser.add_argument(*_spellings("save-state-every"), type=int, default=0,
                         help="NEW: after every N-th epoch, and after the last one, all ranks write the training state "
                              "(weights, Adam moments and step, the CUDA generators, the evaluator's best model, the "

@@ -746,24 +746,41 @@ def part_gains(objective: str, part: torch.Tensor, conn: torch.Tensor, n_parts: 
     return target, gain
 
 
-def part_cluster(rating, label: torch.Tensor, nw: Optional[torch.Tensor], cw: torch.Tensor, cap: int, seed: int):
-    """``bns_part_cluster``: one size-constrained label-propagation proposal per node (target -1: stay)."""
+def part_cluster(rating, label: torch.Tensor, nw: Optional[torch.Tensor], cw: torch.Tensor, cap: int, seed: int, *,
+                 ew: Optional[torch.Tensor] = None, ce: Optional[torch.Tensor] = None, ecap: int = 0):
+    """``bns_part_cluster``: one size-constrained label-propagation proposal per node (target -1: stay).  With ``ew``
+    (int64 in-edge weight per node), ``ce`` (the clusters' in-edge weights) and ``ecap``: ``bns_part_cluster_edges``,
+    which also keeps every proposed cluster's in-edge weight within ``ecap``."""
     _req(label, torch.int32, "label")
     _req(cw, torch.int64, "cw")
     ip, cid, wt = rating
     n, dev = label.numel(), label.device
     target = torch.empty(n, dtype=torch.int32, device=dev)
     gain = torch.empty(n, dtype=torch.int64, device=dev)
-    check(lib.bns_part_cluster(n, ip.data_ptr(), cid.data_ptr(), wt.data_ptr(), label.data_ptr(), _ptr(nw), cw.data_ptr(),
-                               int(cap), seed & 0xFFFFFFFFFFFFFFFF, target.data_ptr(), gain.data_ptr(), _stream_ptr()),
-          "bns_part_cluster")
+    if ew is None:
+        check(lib.bns_part_cluster(n, ip.data_ptr(), cid.data_ptr(), wt.data_ptr(), label.data_ptr(), _ptr(nw),
+                                   cw.data_ptr(), int(cap), seed & 0xFFFFFFFFFFFFFFFF, target.data_ptr(),
+                                   gain.data_ptr(), _stream_ptr()), "bns_part_cluster")
+        return target, gain
+    _req(ew, torch.int64, "ew")
+    _req(ce, torch.int64, "ce")
+    check(lib.bns_part_cluster_edges(n, ip.data_ptr(), cid.data_ptr(), wt.data_ptr(), label.data_ptr(), _ptr(nw),
+                                     cw.data_ptr(), int(cap), ew.data_ptr(), ce.data_ptr(), int(ecap),
+                                     seed & 0xFFFFFFFFFFFFFFFF, target.data_ptr(), gain.data_ptr(), _stream_ptr()),
+          "bns_part_cluster_edges")
     return target, gain
 
 
 def part_weights(label: torch.Tensor, nw: Optional[torch.Tensor], n_labels: int) -> torch.Tensor:
-    """``bns_part_weights``: int64 [n_labels] sums of the node weights per label."""
+    """``bns_part_weights``: int64 [n_labels] sums of the node weights per label.  int32 or int64 weights (the latter
+    through ``bns_part_weights_i64``: in-edge weights, whose coarse sums pass 2^31)."""
     _req(label, torch.int32, "label")
     out = torch.empty(n_labels, dtype=torch.int64, device=label.device)
+    if nw is not None and nw.dtype == torch.int64:
+        _req(nw, torch.int64, "nw")
+        check(lib.bns_part_weights_i64(label.numel(), label.data_ptr(), nw.data_ptr(), n_labels, out.data_ptr(),
+                                       _stream_ptr()), "bns_part_weights_i64")
+        return out
     check(lib.bns_part_weights(label.numel(), label.data_ptr(), _ptr(nw), n_labels, out.data_ptr(), _stream_ptr()),
           "bns_part_weights")
     return out

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 10
+#define BNS_ABI_VERSION 11
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -686,6 +686,20 @@ int bns_part_cluster(int64_t n, const int64_t *indptr, const int32_t *cid, const
                      const int32_t *nw, const int64_t *cw, int64_t cap, uint64_t seed, int32_t *target, int64_t *gain,
                      void *stream);
 int bns_part_weights(int64_t n, const int32_t *label, const int32_t *nw, int64_t n_labels, int64_t *out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 11: edge-balanced partitions (--partition-balance edges): a second node weight, the in-edge count (int64, since
+ * coarse sums pass 2^31), carried through the multilevel partitioner's coarsening.
+ * bns_part_cluster_edges: bns_part_cluster with a second cap: a cluster c is a candidate only while cw[c] + nw[v] <= cap
+ *     and ce[c] + ew[v] <= ecap (ew: device int64 [n] in-edge weight of each node; ce: the clusters' summed in-edge
+ *     weights, bns_part_weights_i64 of ew).  Everything else, coin and tie breaks included, is bns_part_cluster's.
+ * bns_part_weights_i64: bns_part_weights over int64 weights nw (NULL = 1 each).
+ * ----------------------------------------------------------------------------------------------*/
+int bns_part_cluster_edges(int64_t n, const int64_t *indptr, const int32_t *cid, const int32_t *cw_edge,
+                           const int32_t *label, const int32_t *nw, const int64_t *cw, int64_t cap, const int64_t *ew,
+                           const int64_t *ce, int64_t ecap, uint64_t seed, int32_t *target, int64_t *gain, void *stream);
+int bns_part_weights_i64(int64_t n, const int32_t *label, const int64_t *nw, int64_t n_labels, int64_t *out,
+                         void *stream);
 
 #ifdef __cplusplus
 }

@@ -3,11 +3,14 @@ ogbn-products and Yelp shapes and on a Reddit-sized degree-corrected block model
 average about 50, 20 % of the edge ends leaving their community), for P in {2, 4, 8} and both objectives.
 
 Reports per run: wall time (host clock around synchronised work, after a warm-up run on a small graph), peak device
-memory, the exact cut and vol (``partition_quality``), the smallest and largest part, and the boundary rows each epoch
-moves at sampling rate 0.1 (each of the ``vol`` halo rows is sampled with probability 0.1: ``vol * 0.1``).  The card's
-name and power limit are printed in the same run.  One JSON line per run, then a markdown table.
+memory, the exact cut and vol (``partition_quality``), the smallest and largest part, the most in-edges a part owns
+over the mean ``E / P`` (a rank's aggregation work), and the boundary rows each epoch moves at sampling rate 0.1 (each
+of the ``vol`` halo rows is sampled with probability 0.1: ``vol * 0.1``).  ``--balance nodes,edges`` runs every
+configuration under each ``--partition-balance``.  The card's name and power limit are printed in the same run.  One
+JSON line per run, then a markdown table.
 
-  python tools/bench_partition.py [--shapes reddit,blocks,yelp,ogbn-products] [--parts 2,4,8] [--budget-s 1500]
+  python tools/bench_partition.py [--shapes reddit,blocks,yelp,ogbn-products] [--parts 2,4,8] [--balance nodes,edges]
+                                  [--budget-s 1500]
 """
 from __future__ import annotations
 
@@ -41,19 +44,20 @@ def graph(name: str):
     return make_graph(name, seed=0)
 
 
-def run(fg, P, method, objective, dev):
+def run(fg, P, method, objective, dev, balance="nodes"):
     from bns_gcn_b200.data import assign_parts, partition_quality
     torch.cuda.synchronize(dev)
     torch.cuda.reset_peak_memory_stats(dev)
     base = torch.cuda.memory_allocated(dev)
     t0 = time.perf_counter()
-    part = assign_parts(fg, P, method, 0, objective, dev)
+    part = assign_parts(fg, P, method, 0, objective, dev, balance)
     torch.cuda.synchronize(dev)
     dt = time.perf_counter() - t0
     peak = torch.cuda.max_memory_allocated(dev) - base
     q = partition_quality(fg, part, P, dev)
     return {"method": method, "P": P, "obj": objective, "time_s": round(dt, 3), "peak_mem_gb": round(peak / 2 ** 30, 3),
             "cut": q["cut"], "vol": q["vol"], "min_size": q["min_size"], "max_size": q["max_size"],
+            "balance": balance, "max_over_mean_in_edges": round(q["max_in_edges"] * P / fg.n_edges, 4),
             "rows_per_epoch_p0.1": round(0.1 * q["vol"], 1)}
 
 
@@ -62,10 +66,12 @@ def main(argv=None):
     ap.add_argument("--shapes", default="reddit,blocks,yelp,ogbn-products")
     ap.add_argument("--parts", default="2,4,8")
     ap.add_argument("--methods", default="random,metis,multilevel")
+    ap.add_argument("--balance", default="nodes", help="comma-separated --partition-balance values: nodes, edges")
     ap.add_argument("--budget-s", type=float, default=1e9, help="skip (and list as not measured) what starts later")
     ap.add_argument("--out", default="")
     a = ap.parse_args(argv)
-    assert torch.cuda.is_available(), "bench_partition.py measures on a GPU"
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_partition.py measures on a GPU and there is none; it does not fall back to the CPU")
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
     import bns_gcn_b200  # noqa: F401
@@ -82,19 +88,22 @@ def main(argv=None):
                 for m in a.methods.split(","):
                     if m == "random" and objective == "cut":
                         continue                        # random ignores the objective
-                    if time.perf_counter() - start > a.budget_s:
-                        skipped.append(f"{shape} P={P} {objective} {m}")
-                        continue
-                    if fg is None:
-                        fg = graph(shape)
-                    r = dict(shape=shape, n=fg.n_nodes, edges=fg.n_edges, **run(fg, P, m, objective, dev))
-                    rows.append(r)
-                    print(json.dumps(r), flush=True)
-    print("\n| shape | P | obj | method | time (s) | peak mem (GB) | cut | vol | min / max part | rows / epoch at p=0.1 |")
-    print("|---|---|---|---|---|---|---|---|---|---|")
+                    for balance in a.balance.split(","):
+                        if time.perf_counter() - start > a.budget_s:
+                            skipped.append(f"{shape} P={P} {objective} {m} {balance}")
+                            continue
+                        if fg is None:
+                            fg = graph(shape)
+                        r = dict(shape=shape, n=fg.n_nodes, edges=fg.n_edges, **run(fg, P, m, objective, dev, balance))
+                        rows.append(r)
+                        print(json.dumps(r), flush=True)
+    print("\n| shape | P | obj | method | balance | time (s) | peak mem (GB) | cut | vol | min / max part | "
+          "max / mean in-edges | rows / epoch at p=0.1 |")
+    print("|---|---|---|---|---|---|---|---|---|---|---|---|")
     for r in rows:
-        print(f"| {r['shape']} | {r['P']} | {r['obj']} | {r['method']} | {r['time_s']} | {r['peak_mem_gb']} | "
-              f"{r['cut']:,} | {r['vol']:,} | {r['min_size']:,} / {r['max_size']:,} | {r['rows_per_epoch_p0.1']:,} |")
+        print(f"| {r['shape']} | {r['P']} | {r['obj']} | {r['method']} | {r['balance']} | {r['time_s']} | "
+              f"{r['peak_mem_gb']} | {r['cut']:,} | {r['vol']:,} | {r['min_size']:,} / {r['max_size']:,} | "
+              f"{r['max_over_mean_in_edges']} | {r['rows_per_epoch_p0.1']:,} |")
     for s in skipped:
         print("not measured:", s)
     if a.out:
