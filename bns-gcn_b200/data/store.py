@@ -10,6 +10,8 @@ value ``(subg, node_dict, gpb)`` that ``train.run`` consumes -- over a format ma
     <part_path>/<graph_name>/<graph_name>.json     part config: counts, node ranges, per-part array table
     <part_path>/<graph_name>/meta.json             {"n_feat": .., "n_class": .., "n_train": ..}
     <part_path>/<graph_name>/part<r>/<key>.npy     one plain ``.npy`` per array (CSR + node_dict entries)
+    <part_path>/<graph_name>/{val,test}/...        inductive runs with ``--eval --parallel-eval``: the same layout for
+                                                   a partition of each evaluation graph (``load_eval_partition``)
 
 Every array is its own ``.npy`` so a rank maps only what it needs (``np.load(mmap_mode='r')``) and copies it
 straight to its GPU; boolean masks are stored as uint8 and cast back on load, exactly the wart the reference
@@ -25,12 +27,13 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 import torch
 
-from .partition import NID, GraphPartitionBook, LocalGraph, Partition, partition_graph
+from .partition import NID, GraphPartitionBook, LocalGraph, Partition, induced_subgraph, partition_graph
 from .files import data_source, load_graph
 from .synthetic import FullGraph
 
 FORMAT_VERSION = 1
 _BOOL_KEYS = ("inner_node", "train_mask", "val_mask", "test_mask")
+EVAL_GRAPHS = ("val", "test")
 
 
 def partition_balance(args) -> str:
@@ -95,16 +98,91 @@ def save_partition(p: Partition, graph_dir: str) -> Dict[str, object]:
             "arrays": arrays}
 
 
+def _write_parts(parts, graph_dir: str, part_config: str, cfg: dict) -> None:
+    """Write every part, then the part config (through a temporary file: the config appears only when every part is
+    complete)."""
+    os.makedirs(graph_dir, exist_ok=True)
+    for p in parts:
+        cfg[f"part-{p.rank}"] = save_partition(p, graph_dir)
+    tmp = part_config + ".tmp"
+    with open(tmp, 'w') as f:
+        json.dump(cfg, f, indent=1)
+    os.replace(tmp, part_config)
+
+
+def _config_head(args, parts) -> dict:
+    return {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "data_source": data_source(args),
+            "num_parts": args.n_partitions, "part_method": args.partition_method, "inductive": bool(args.inductive),
+            "balance": partition_balance(args),
+            "node_map": [int(x) for x in parts[0].gpb.ranges.tolist()],
+            "num_nodes": int(parts[0].gpb.ranges[-1]), "num_edges": int(sum(p.graph.num_edges() for p in parts))}
+
+
+def wants_eval_partitions(args) -> bool:
+    """``--eval --parallel-eval --inductive``: every rank evaluates its own part of the two evaluation graphs."""
+    return bool(getattr(args, 'eval', False) and getattr(args, 'parallel_eval', False) and args.inductive)
+
+
+def _eval_dirs(args, which: str) -> Tuple[str, str]:
+    if which not in EVAL_GRAPHS:
+        raise ValueError(f"evaluation graph {which!r}: expected one of {', '.join(EVAL_GRAPHS)}")
+    graph_dir, _ = _dirs(args)
+    d = os.path.join(graph_dir, which)
+    return d, os.path.join(d, args.graph_name + '.json')
+
+
+def _check_eval(cfg: dict, args, which: str, part_config: str) -> None:
+    """Refuse an evaluation set of another graph, source, balance, method or part count."""
+    _check_source(cfg, args, part_config)
+    _check_balance(cfg, args, part_config)
+    for key, stored, wanted in (("eval_graph", cfg.get("eval_graph"), which),
+                                ("--partition-method", cfg.get("part_method"), args.partition_method),
+                                ("--n-partitions", cfg.get("num_parts"), args.n_partitions)):
+        if stored != wanted:
+            raise RuntimeError(f"{part_config} was partitioned with {key} {stored}, this run asks for {key} {wanted}; "
+                               "pick another --graph-name or remove the store")
+
+
+def eval_graph_of(fg: FullGraph, which: str) -> FullGraph:
+    """The graph an inductive run evaluates on: ``val`` -> the train | val subgraph, ``test`` -> the full graph
+    (the reference's ``val_g`` / ``test_g``, helper/utils.py:226-230)."""
+    return induced_subgraph(fg, fg.train_mask | fg.val_mask) if which == 'val' else fg
+
+
+def eval_partitions(fg: FullGraph, which: str, args, device: Optional[torch.device] = None):
+    """``partition_graph`` of ``eval_graph_of(fg, which)`` with the run's method, objective, balance and seed.  Each
+    part keeps what its evaluation reads: ids and owners, ``feat``, ``label``, the degrees of THAT graph, and the mask
+    it is scored on (``val_mask`` / ``test_mask``)."""
+    parts = partition_graph(eval_graph_of(fg, which), args.n_partitions, args.partition_method,
+                            seed=getattr(args, 'graph_seed', 0), device=device,
+                            objective=getattr(args, 'partition_obj', 'vol'), balance=partition_balance(args))
+    keep = (NID, "part_id", "inner_node", "feat", "label", "in_deg", "out_deg", which + "_mask")
+    for p in parts:
+        p.node_dict = {k: p.node_dict[k] for k in keep}
+    return parts
+
+
 def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch.device] = None) -> str:
     """helper/utils.py:73-98: build the graph (``load_data`` -> ``load_graph``: the seeded generator, or the published
     files with ``--data-source files``), partition it unless the part config already exists, always (re)write
-    ``meta.json``.  Returns the part-config path.  Nothing is written before the graph is built and checked."""
+    ``meta.json``.  Returns the part-config path.  Nothing is written before the graph is built and checked.
+    With ``--eval --parallel-eval --inductive`` the two evaluation sets (``val/``, ``test/``: ``eval_partitions``) are
+    written too, each unless its own config exists, from the same ``FullGraph``."""
     graph_dir, part_config = _dirs(args)
     if os.path.exists(part_config):
         with open(part_config) as f:
             cfg = json.load(f)
         _check_source(cfg, args, part_config)
         _check_balance(cfg, args, part_config)
+    todo = []
+    if wants_eval_partitions(args):
+        for which in EVAL_GRAPHS:
+            _, eval_config = _eval_dirs(args, which)
+            if os.path.exists(eval_config):
+                with open(eval_config) as f:
+                    _check_eval(json.load(f), args, which, eval_config)
+            else:
+                todo.append(which)
     if fg is None:
         fg = load_graph(args, device)
     n_feat, n_class = fg.n_feat, fg.n_class
@@ -114,17 +192,15 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
         parts = partition_graph(fg, args.n_partitions, args.partition_method, seed=getattr(args, 'graph_seed', 0),
                                 inductive=args.inductive, device=device,
                                 objective=getattr(args, 'partition_obj', 'vol'), balance=partition_balance(args))
-        cfg = {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "data_source": data_source(args),
-               "num_parts": args.n_partitions, "part_method": args.partition_method, "inductive": bool(args.inductive),
-               "balance": partition_balance(args),
-               "node_map": [int(x) for x in parts[0].gpb.ranges.tolist()],
-               "num_nodes": int(parts[0].gpb.ranges[-1]), "num_edges": int(sum(p.graph.num_edges() for p in parts))}
-        for p in parts:
-            cfg[f"part-{p.rank}"] = save_partition(p, graph_dir)
-        tmp = part_config + ".tmp"
-        with open(tmp, 'w') as f:
-            json.dump(cfg, f, indent=1)
-        os.replace(tmp, part_config)                       # the config appears only when every part is complete
+        _write_parts(parts, graph_dir, part_config, _config_head(args, parts))
+        del parts
+    for which in todo:
+        eval_dir, eval_config = _eval_dirs(args, which)
+        parts = eval_partitions(fg, which, args, device)
+        cfg = _config_head(args, parts)
+        cfg["inductive"], cfg["eval_graph"] = False, which     # a partition of the whole evaluation graph
+        _write_parts(parts, eval_dir, eval_config, cfg)
+        del parts
     with open(os.path.join(graph_dir, 'meta.json'), 'w') as f:
         json.dump({'n_feat': n_feat, 'n_class': n_class, 'n_train': n_train}, f)
     return part_config
@@ -135,24 +211,8 @@ def _load_array(path: str, mmap: bool) -> torch.Tensor:
     return torch.from_numpy(np.array(a))        # a private, writable copy (the mapping itself is read-only)
 
 
-def load_partition(args, rank: int, device: Optional[torch.device] = None, mmap: bool = True):
-    """helper/utils.py:101-140: ``(subg, node_dict, gpb)`` of part ``rank``; fills ``args.n_feat / n_class / n_train``
-    from ``meta.json``.  ``device``: where the tensors go (default: stay on the host)."""
-    graph_dir, part_config = _dirs(args)
-    if not os.path.exists(part_config):
-        raise FileNotFoundError(f"{part_config}: no such partition config; run graph_partition(args) first "
-                                "(main.py does unless --skip-partition)")
-    print('loading partitions')
-    with open(part_config) as f:
-        cfg = json.load(f)
-    if cfg.get("format_version") != FORMAT_VERSION:
-        raise RuntimeError(f"{part_config}: format version {cfg.get('format_version')} != {FORMAT_VERSION}")
-    _check_source(cfg, args, part_config)
-    _check_balance(cfg, args, part_config)
-    if not 0 <= rank < cfg["num_parts"]:
-        raise IndexError(f"part {rank} of {cfg['num_parts']}")
-    if cfg["num_parts"] != args.n_partitions:
-        raise RuntimeError(f"{part_config} holds {cfg['num_parts']} parts, --n-partitions is {args.n_partitions}")
+def _read_part(graph_dir: str, part_config: str, cfg: dict, rank: int, device, mmap: bool):
+    """``(subg, node_dict, gpb)`` of part ``rank`` of the (checked) part config ``cfg``, read from ``part_config``."""
     ent = cfg[f"part-{rank}"]
     d = os.path.join(graph_dir, ent["dir"])
 
@@ -180,10 +240,49 @@ def load_partition(args, rank: int, device: Optional[torch.device] = None, mmap:
         node_dict = {k: v.to(device) for k, v in node_dict.items()}
     subg = LocalGraph(int(ent["n_in"]), int(ent["n_halo"]), indptr, indices)
     gpb = GraphPartitionBook(torch.tensor(cfg["node_map"], dtype=torch.int64))
+    return subg, node_dict, gpb
+
+
+def load_partition(args, rank: int, device: Optional[torch.device] = None, mmap: bool = True):
+    """helper/utils.py:101-140: ``(subg, node_dict, gpb)`` of part ``rank``; fills ``args.n_feat / n_class / n_train``
+    from ``meta.json``.  ``device``: where the tensors go (default: stay on the host)."""
+    graph_dir, part_config = _dirs(args)
+    if not os.path.exists(part_config):
+        raise FileNotFoundError(f"{part_config}: no such partition config; run graph_partition(args) first "
+                                "(main.py does unless --skip-partition)")
+    print('loading partitions')
+    with open(part_config) as f:
+        cfg = json.load(f)
+    if cfg.get("format_version") != FORMAT_VERSION:
+        raise RuntimeError(f"{part_config}: format version {cfg.get('format_version')} != {FORMAT_VERSION}")
+    _check_source(cfg, args, part_config)
+    _check_balance(cfg, args, part_config)
+    if not 0 <= rank < cfg["num_parts"]:
+        raise IndexError(f"part {rank} of {cfg['num_parts']}")
+    if cfg["num_parts"] != args.n_partitions:
+        raise RuntimeError(f"{part_config} holds {cfg['num_parts']} parts, --n-partitions is {args.n_partitions}")
+    subg, node_dict, gpb = _read_part(graph_dir, part_config, cfg, rank, device, mmap)
     with open(os.path.join(graph_dir, 'meta.json')) as f:
         meta = json.load(f)
     args.n_feat, args.n_class, args.n_train = meta['n_feat'], meta['n_class'], meta['n_train']   # utils.py:134-138
     return subg, node_dict, gpb
+
+
+def load_eval_partition(args, which: str, rank: int, device: Optional[torch.device] = None, mmap: bool = True):
+    """``(subg, node_dict, gpb)`` of part ``rank`` of the evaluation set ``which`` (``'val'`` | ``'test'``), the
+    contract of ``load_partition``; ``node_dict`` holds ``which + '_mask'`` and the degrees of that graph."""
+    eval_dir, eval_config = _eval_dirs(args, which)
+    if not os.path.exists(eval_config):
+        raise FileNotFoundError(f"{eval_config}: no such evaluation partition config; run graph_partition(args) with "
+                                "--eval --parallel-eval --inductive first (main.py does unless --skip-partition)")
+    with open(eval_config) as f:
+        cfg = json.load(f)
+    if cfg.get("format_version") != FORMAT_VERSION:
+        raise RuntimeError(f"{eval_config}: format version {cfg.get('format_version')} != {FORMAT_VERSION}")
+    _check_eval(cfg, args, which, eval_config)
+    if not 0 <= rank < cfg["num_parts"]:
+        raise IndexError(f"part {rank} of {cfg['num_parts']}")
+    return _read_part(eval_dir, eval_config, cfg, rank, device, mmap)
 
 
 def load_as_partition(args, rank: int, device: Optional[torch.device] = None) -> Partition:

@@ -69,7 +69,8 @@ def build_parser():
     parser.add_argument(*_spellings("parallel-eval"), action='store_true',
                         help="NEW: with --eval, every rank evaluates its own nodes on its partition (the whole halo "
                              "exchanged layer by layer) instead of rank 0 evaluating the full graph alone; the full "
-                             "graph is never built.  Transductive runs only")
+                             "graph is never built.  With --inductive, on partitions of the train | val subgraph "
+                             "and of the full graph, which the partition step writes beside the training parts")
     parser.add_argument(*_spellings("data-source"), default="synthetic", choices=["synthetic", "files"],
                         help="NEW: where the graph comes from.  synthetic generates the --dataset shape from a seed.  "
                              "files reads reddit, yelp or ogbn-products from the files DGL / OGB leave under "

@@ -1,7 +1,8 @@
 """Launcher with the reference's flags (main.py:10-64): generate the graph (or read its published files with
 ``--data-source files``; nothing is downloaded), partition it into the on-disk store (``data/store.py``:
 ``graph_partition`` unless ``--skip-partition``), start one process per partition / GPU; each loads its part
-(``load_partition``) and runs ``train.run``.
+(``load_partition``; with ``--eval --parallel-eval --inductive`` also its parts of the two evaluation graphs,
+``load_eval_partition``) and runs ``train.run``.
 
     python -m bns_gcn_b200.main --dataset reddit --n-partitions 4 --model graphsage --n-layers 3 --n-hidden 256 \
         --sampling-rate 0.1 --use-pp --partition-method random --n-epochs 50 --no-eval
@@ -16,7 +17,8 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from .data.store import default_graph_name, graph_partition, load_partition
+from .data.store import (EVAL_GRAPHS, default_graph_name, graph_partition, load_eval_partition, load_partition,
+                         wants_eval_partitions)
 from .helper.parser import create_parser
 
 
@@ -40,7 +42,10 @@ def init_processes(rank, size, args):
             graph_partition(args, device=dev)
         dist.barrier()
     g, node_dict, gpb = load_partition(args, rank)          # train.py:469 (fills args.n_feat / n_class / n_train)
-    train.run(g, node_dict, gpb, args, dev)
+    eval_parts = None
+    if wants_eval_partitions(args):                         # --eval --parallel-eval --inductive
+        eval_parts = {w: load_eval_partition(args, w, rank) for w in EVAL_GRAPHS}
+    train.run(g, node_dict, gpb, args, dev, eval_parts=eval_parts)
     dist.destroy_process_group()
 
 

@@ -676,20 +676,24 @@ class GraphedEpoch:
         return self.loss
 
 
-def run(graph, node_dict, gpb, args, device=None, full_graph=None):
+def run(graph, node_dict, gpb, args, device=None, full_graph=None, eval_parts=None):
     """train.py:300-456.  With ``args.eval`` rank 0 also runs the evaluation / checkpoint branch (:308-321, 427-456)
     through ``evaluate.Evaluator`` -- on the GPU with the same kernels, synchronously, instead of a CPU thread pool;
     ``full_graph``: the un-partitioned ``FullGraph`` to evaluate on (default: ``data.load_graph(args)``, regenerated or
     read again from ``--data-path``).
     With ``args.parallel_eval`` as well, EVERY rank evaluates its own nodes on its partition instead
-    (``evaluate.ParallelEvaluator``) and the full graph is never built; inductive runs are refused.
+    (``evaluate.ParallelEvaluator``) and the full graph is never built.  Inductive runs evaluate on their own graphs:
+    ``eval_parts = {'val': ..., 'test': ...}``, this rank's parts of them (``data.load_eval_partition``); without
+    ``eval_parts`` an inductive run with ``--parallel-eval`` is refused.
     ``args.save_state_every`` / ``args.resume``: write the training state every N epochs and after the last one, or
     continue from the saved one (``state.py``)."""
     rank, size = _rank_size()
     parallel = getattr(args, 'eval', False) and getattr(args, 'parallel_eval', False)
-    if parallel and args.inductive:
+    if parallel and args.inductive and eval_parts is None:
         raise ValueError("--parallel-eval: inductive runs evaluate on the train | val subgraph and the full graph, "
-                         "which the training partitions do not hold; drop --parallel-eval to evaluate them on rank 0")
+                         "which the training partitions do not hold; pass their partitions (eval_parts, "
+                         "data.load_eval_partition, which main.py does) or drop --parallel-eval to evaluate them on "
+                         "rank 0")
     from . import state
     save_every = getattr(args, 'save_state_every', 0)
     saved = None
@@ -699,7 +703,10 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None):
     st = setup(graph, node_dict, gpb, args, device)
     dev = st.feat.device
     evaluator = None
-    if parallel:
+    if parallel and args.inductive:
+        from .evaluate import ParallelEvaluator
+        evaluator = ParallelEvaluator.inductive_from_parts(args, eval_parts, dev, ctx.comm())
+    elif parallel:
         from .evaluate import ParallelEvaluator, build_partition_eval_graph
         eg = build_partition_eval_graph(st.part, node_dict, st.boundary, ctx.comm())
         evaluator = ParallelEvaluator(args, eg, st.feat, st.labels, node_dict['val_mask'].to(dev),

@@ -8,6 +8,8 @@ power limit read in the same run.
   python tools/bench_eval.py --mode parallel --shape reddit --model gat --heads 4                 # P = 1
   torchrun --nproc-per-node 8 tools/bench_eval.py --mode parallel --shape reddit --model gcn        # P = 8
   torchrun --nproc-per-node 8 tools/bench_eval.py --mode parallel --shape papers100m --scale 0.1    # generated per rank
+  python tools/bench_eval.py --inductive --mode whole --shape reddit --model gcn    # val_g and test_g, one forward each
+  python tools/bench_eval.py --inductive --mode parallel --shape reddit --model gcn # their partitions (+ set-up ms)
 
 The papers100M shape is never built as one graph: every rank generates its piece (``data.make_local_partition``), so
 only ``--mode parallel`` takes it.  The other shapes are generated whole on every rank and cut by ``partition_graph``
@@ -21,6 +23,7 @@ import argparse
 import json
 import os
 import sys
+import time
 
 import torch
 
@@ -91,6 +94,85 @@ def whole(a, dev):
             "extra_GB": [round((peak - base) / 2 ** 30, 3)]}
 
 
+def max_sm_clock():
+    """The card's max SM clock (read-only query), reported beside the times."""
+    import subprocess
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=clocks.max.sm", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception:                       # noqa: BLE001 - the times stand without it
+        return "unknown"
+
+
+def _model(a, args, fg, dev):
+    args.n_feat, args.n_class, args.n_train = fg.n_feat, fg.n_class, int(fg.train_mask.sum())
+    torch.manual_seed(args.seed)
+    return train.create_model(get_layer_size(fg.n_feat, a.hidden, fg.n_class, a.layers), args).to(dev).eval()
+
+
+def _ms(t0):
+    torch.cuda.synchronize()
+    return round((time.perf_counter() - t0) * 1e3, 3)
+
+
+def inductive_whole(a, dev):
+    """``--inductive --mode whole``: rank 0's ``Evaluator``, which holds the train | val subgraph (``val_g``) and the
+    full graph (``test_g``) for the whole run; one forward on each."""
+    from bns_gcn_b200.evaluate import eval_graphs
+    fg = make_graph(a.shape, seed=0, device=dev)
+    args = make_args(a, 1)
+    args.inductive = True
+    net = _model(a, args, fg, dev)
+    torch.cuda.synchronize(dev)
+    base = torch.cuda.memory_allocated(dev)
+    torch.cuda.reset_peak_memory_stats(dev)
+    val_g, test_g = eval_graphs(fg, True, dev)
+    del fg
+    rec = {"P": 1}
+    with torch.no_grad():
+        for w, g in (("val", val_g), ("test", test_g)):
+            med, mn = timed(lambda: net(g.handle, g.ndata["feat"]), a.warmup, a.iters)
+            rec[w + "_ms_median"], rec[w + "_ms_min"] = round(med, 3), round(mn, 3)
+    peak = torch.cuda.max_memory_allocated(dev)
+    rec.update(peak_GB=[round(peak / 2 ** 30, 3)], extra_GB=[round((peak - base) / 2 ** 30, 3)])
+    return rec
+
+
+def inductive_parallel(a, rank, world, dev, comm):
+    """``--inductive --mode parallel``: this rank's parts of the two evaluation graphs (``data.eval_partitions``, what
+    the store holds), each turned into the ``evaluate.EvalPart`` ``ParallelEvaluator`` evaluates (set-up: degrees,
+    boundary, the layer-0 precompute) when it is needed -- the val graph first, the test graph in its place."""
+    from bns_gcn_b200.data import eval_partitions
+    from bns_gcn_b200.evaluate import build_eval_part
+    fg = make_graph(a.shape, seed=0, device=dev)
+    args = make_args(a, world)
+    args.inductive = True
+    net = _model(a, args, fg, dev)
+    parts = {w: eval_partitions(fg, w, args, dev)[rank] for w in ("val", "test")}
+    del fg
+    torch.cuda.synchronize(dev)
+    base = torch.cuda.memory_allocated(dev)
+    torch.cuda.reset_peak_memory_stats(dev)
+    rec, ep = {}, None
+    for w in ("val", "test"):
+        ep = None                                    # the val graph goes before the test graph is built
+        comm.barrier()
+        t0 = time.perf_counter()
+        ep = build_eval_part(args, (parts[w].graph, parts[w].node_dict, parts[w].gpb), w, dev, comm)
+        with torch.no_grad():
+            net(ep.graph, ep.feat)                   # the first forward also cuts the peer blocks
+        rec[w + "_setup_ms"] = _ms(t0)
+
+        def fwd():
+            comm.barrier()
+            with torch.no_grad():
+                net(ep.graph, ep.feat)
+        rec[w + "_ms"] = timed(fwd, a.warmup, a.iters)
+    peak = torch.cuda.max_memory_allocated(dev)
+    rec.update(peak_GB=peak / 2 ** 30, extra_GB=(peak - base) / 2 ** 30)
+    return rec
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--mode", choices=["whole", "parallel"], default="parallel")
@@ -106,6 +188,9 @@ def main():
     ap.add_argument("--comm", default="torch", choices=["torch", "abi"],
                     help="abi: collectives through libbnsgcn.so's own communicator")
     ap.add_argument("--out", default=None, help="directory to append the JSON line to (eval.jsonl)")
+    ap.add_argument("--inductive", action="store_true",
+                    help="evaluate as an inductive run does: one forward on the train | val subgraph and one on the "
+                         "full graph (parallel: on partitions of each, with the set-up time of each)")
     a = ap.parse_args()
     os.environ["BNS_COMM"] = a.comm
     dist_run = "WORLD_SIZE" in os.environ
@@ -113,10 +198,31 @@ def main():
         if dist_run else (0, 1, 0)
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
+    if a.inductive and (a.shape == "papers100m" or a.check):
+        raise SystemExit("--inductive: not with the papers100m shape (never built whole) or --check")
     if a.mode == "whole":
         if dist_run or a.shape == "papers100m":
             raise SystemExit("--mode whole: one process on one GPU, and not the papers100m shape (never built whole)")
-        rec = whole(a, dev)
+        rec = inductive_whole(a, dev) if a.inductive else whole(a, dev)
+    elif a.inductive:
+        from bns_gcn_b200.helper.comm import DistComm, SoloComm
+        if dist_run:
+            import torch.distributed as dist
+            dist.init_process_group("nccl", device_id=dev)
+            comm = DistComm()
+        else:
+            comm = SoloComm()
+        ctx.set_comm(comm)
+        torch.cuda.set_stream(torch.cuda.Stream(dev))
+        mine = inductive_parallel(a, rank, world, dev, comm)
+        import pickle
+        every = [pickle.loads(b) for b in comm.all_gather_bytes(pickle.dumps(mine))]
+        rec = {"P": world}
+        for w in ("val", "test"):
+            rec[w + "_ms_median"] = round(max(e[w + "_ms"][0] for e in every), 3)
+            rec[w + "_ms_min"] = round(max(e[w + "_ms"][1] for e in every), 3)
+            rec[w + "_setup_ms"] = round(max(e[w + "_setup_ms"] for e in every), 3)
+        rec.update(peak_GB=[round(e["peak_GB"], 3) for e in every], extra_GB=[round(e["extra_GB"], 3) for e in every])
     else:
         from bns_gcn_b200.helper.comm import DistComm, SoloComm
         if dist_run:
@@ -161,8 +267,11 @@ def main():
             comm.barrier()
     if rank == 0:
         name, power = gpu_info()
+        if a.inductive:
+            rec["max_sm_clock"] = max_sm_clock()
         rec = {"mode": a.mode, "shape": a.shape, "scale": a.scale, "model": a.model, "heads": a.heads,
-               "layers": a.layers, "hidden": a.hidden, "comm": a.comm, **rec, "gpu": name, "power_limit": power}
+               "layers": a.layers, "hidden": a.hidden, "comm": a.comm, "inductive": a.inductive, **rec, "gpu": name,
+               "power_limit": power}
         line = json.dumps(rec)
         print(line)
         if a.out:
