@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -202,6 +202,8 @@ SIGNATURES = {
     "bns_part_cluster_edges": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
                                        c_void_p, c_void_p, c_int64, c_uint64, c_void_p, c_void_p, c_void_p]),
     "bns_part_weights_i64": (c_int, [c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
+    # ---- ABI 12 ----
+    "bns_stamp_globaltimer": (c_int, [c_void_p, c_void_p]),
 }
 
 

@@ -2068,6 +2068,13 @@ __global__ void halo_slot_kernel(const int64_t *__restrict__ pos, const int64_t 
     if (local >= n_in) slot[local - n_in] = slab_offset + (int32_t)k;
 }
 
+// one thread: the GPU's nanosecond clock, when the stream reaches this point (bns_stamp_globaltimer)
+__global__ void stamp_globaltimer_kernel(uint64_t *__restrict__ dst) {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    *dst = t;
+}
+
 }  // namespace
 
 extern "C" int bns_fill_i32(int32_t *dst, int64_t n, int32_t value, void *stream) {
@@ -2086,6 +2093,18 @@ extern "C" int bns_halo_slot_update(const int64_t *pos, const int64_t *one_hops,
     if (r == 0) return BNS_OK;
     BNS_REQUIRE(pos && one_hops && slot, "bns_halo_slot_update: NULL pointer");
     halo_slot_kernel<<<(unsigned)((r + 255) / 256), 256, 0, as_stream(stream)>>>(pos, one_hops, r, n_in, slab_offset, slot);
+    ++g_launches;
+    BNS_CUDA(cudaGetLastError());
+    return BNS_OK;
+}
+
+// =================================================================================================
+// interval stamps inside a CUDA graph (train.GraphedEpoch(timed=True)): events cannot be timed there
+// =================================================================================================
+extern "C" int bns_stamp_globaltimer(uint64_t *dst, void *stream) {
+    BNS_REQUIRE(dst, "bns_stamp_globaltimer: NULL pointer");
+    BNS_REQUIRE(reinterpret_cast<uintptr_t>(dst) % 8 == 0, "bns_stamp_globaltimer: dst is not 8-byte aligned");
+    stamp_globaltimer_kernel<<<1, 1, 0, as_stream(stream)>>>(dst);
     ++g_launches;
     BNS_CUDA(cudaGetLastError());
     return BNS_OK;

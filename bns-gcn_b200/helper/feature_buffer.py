@@ -115,6 +115,7 @@ class Buffer(object):
         self._seq = {}
         # CUDA-graph mode (train.GraphedEpoch): no timing events; flag sequence numbers = seq_base + *seq_dev
         self.graph_mode = False
+        self.stamps = None                      # a timed capture: timer.ReplayStamps in place of the events
         self.seq_dev = None
         self.seq_base = 0
         self._maps = None
@@ -345,7 +346,9 @@ class Buffer(object):
 
     def _timer_ctx(self, name, stream):
         import contextlib
-        return contextlib.nullcontext() if self.graph_mode else self._timer.timer(name, stream=stream)
+        if not self.graph_mode:
+            return self._timer.timer(name, stream=stream)
+        return self.stamps.interval(name, stream) if self.stamps is not None else contextlib.nullcontext()
 
     def _seq_args(self, layer, backward):
         """(immediate, device pointer) of this exchange's flag value."""

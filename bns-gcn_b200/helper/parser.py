@@ -117,6 +117,12 @@ def build_parser():
                         help="NEW: before the first epoch, load the state saved under this run's graph name and "
                              "continue with the next epoch up to --n-epochs (which counts all epochs).  The resumed run "
                              "is bit-identical to an uninterrupted one")
+    parser.add_argument(*_spellings("cuda-graph"), action='store_true',
+                        help="NEW: after this process's first three epochs, which run eagerly, capture one epoch into a "
+                             "CUDA graph and run every later epoch as one replay of it: the same losses and weights, "
+                             "bit for bit, without the host enqueueing each epoch's launches.  Comm(s) / Reduce(s) are "
+                             "timed inside the replay by GPU clock stamps.  Refused (before any setup) for ranks that "
+                             "are threads of one process and for the staged --backend nccl at more than 2 partitions")
     return parser
 
 

@@ -23,6 +23,7 @@ class Reducer(object):
         self._pending = []
         self._events = None
         self.graph_mode = False
+        self.stamps = None          # a timed capture (train.GraphedEpoch): timer.ReplayStamps bracket the all-reduce
 
     def init(self, model):
         params = [(n, p) for n, p in model.named_parameters()]
@@ -61,7 +62,10 @@ class Reducer(object):
                 cur = torch.cuda.current_stream(self._flat.device)
                 self._stream.wait_stream(cur)
                 with torch.cuda.stream(self._stream):
-                    if self.graph_mode:
+                    if self.graph_mode and self.stamps is not None:
+                        with self.stamps.interval("reduce", self._stream, kind="reduce"):
+                            c.all_reduce_sum(self._flat)
+                    elif self.graph_mode:
                         c.all_reduce_sum(self._flat)
                     else:
                         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

@@ -599,6 +599,17 @@ def halo_slot_update(pos: torch.Tensor, one_hops: torch.Tensor, n_in: int, slab_
                                        slot.data_ptr(), _stream_ptr()), "bns_halo_slot_update")
 
 
+def stamp_globaltimer(dst: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
+    """Store the GPU's ``%globaltimer`` (nanoseconds) into the one-element int64 view ``dst`` on ``stream`` (default:
+    the current stream) -- when the stream reaches this point, also inside a captured CUDA graph."""
+    _req(dst, torch.int64, "dst")
+    if dst.numel() != 1:
+        raise _lib.BnsError(f"dst must be one element, got {dst.numel()}")
+    s = stream if stream is not None else torch.cuda.current_stream(dst.device)
+    with torch.cuda.device(dst.device):
+        check(lib.bns_stamp_globaltimer(dst.data_ptr(), s.cuda_stream), "bns_stamp_globaltimer")
+
+
 # ---- fused LayerNorm -> ReLU -> dropout --------------------------------------------------------------------------
 # Philox stream of the dropout masks: (seed, offset [+ *offset_dev]); train.train_epoch sets it once per epoch
 # (offset = epoch index; under CUDA-graph replay the epoch index comes from the device counter).

@@ -632,9 +632,14 @@ class GraphedEpoch:
     offset of the fused step's dropout masks (``ops.RNG["offset_dev"]``: LayerNorm -> ReLU -> dropout and layer 0's
     input dropout draw their Philox counters from ``2**64 - 1 + epoch_dev``, i.e. the epoch index; ``nn.Dropout`` of
     the op-by-op path uses torch's graph-safe Philox state).  Sizes (sample counts, slab rows) are fixed for the run (train.py:344-345).
+
+    ``timed=True`` (``run`` with ``--cuda-graph``): the capture brackets every exchange interval ``CommTimer`` names in
+    an eager epoch, on the comm stream, and the gradient all-reduce, on the reducer's stream, with two
+    ``ops.stamp_globaltimer`` kernels each (``timer.ReplayStamps``); ``interval_seconds()`` reads them after a replay.
+    ``timed=False`` captures no stamp.
     """
 
-    def __init__(self, st: TrainState, warmup: int = 3):
+    def __init__(self, st: TrainState, warmup: int = 3, timed: bool = False):
         self.st = st
         dev = st.feat.device
         cur = torch.cuda.current_stream(dev)
@@ -661,6 +666,12 @@ class GraphedEpoch:
         # forward-only probe) have already published
         # (the staged transport publishes no flags: its dict of sequence numbers is empty)
         buf.seq_base = max(max(buf._seq.values(), default=0) - int(st.epoch_dev.item()), 0)
+        self.stamps = None
+        if timed:
+            from .helper.timer.replay_stamps import ReplayStamps
+            # at most one forward and one backward exchange per layer, and the all-reduce
+            self.stamps = ReplayStamps(2 * max(buf._n_layers, 1) + 1, dev)
+        buf.stamps = red.stamps = self.stamps
         self.graph = torch.cuda.CUDAGraph()
         try:
             # thread_local: other threads of the process (NCCL watchdog, copy threads) may keep calling CUDA meanwhile
@@ -669,11 +680,39 @@ class GraphedEpoch:
         except BaseException:
             st.graph_mode = buf.graph_mode = red.graph_mode = False      # stay usable in eager mode
             raise
+        finally:
+            buf.stamps = red.stamps = None
         torch.cuda.synchronize(dev)
 
     def __call__(self) -> torch.Tensor:
         self.graph.replay()
         return self.loss
+
+    def interval_seconds(self):
+        """``(Comm(s), Reduce(s))`` of the last replay, which must have been waited for (``timed=True`` only): one copy
+        of the stamps to the host."""
+        sec = self.stamps.seconds(self.stamps.read())
+        return sec["comm"], sec["reduce"]
+
+
+def cuda_graph_refusals(args, comm) -> list:
+    """Every reason why ``run`` cannot replay this configuration's epochs from a CUDA graph (``--cuda-graph``); empty:
+    it can."""
+    why = []
+    if getattr(comm, "kind", None) == "thread":
+        why.append("the ranks are threads of one process, whose exchanges hand CUDA events between threads (they "
+                   "cannot be captured); run one process per GPU")
+    if comm.size > 2 and getattr(args, "backend", "nccl") in ("nccl", "staged"):
+        why.append(f"the staged --backend {args.backend} at {comm.size} partitions (replays of its grouped NCCL "
+                   f"send / receive are only bit-identical at 2 ranks); use --backend p2p")
+    return why
+
+
+def log_line(rank, epoch, train_dur, comm_dur, reduce_dur, loss_per_node) -> str:
+    """train.py:419-421: the means over this process's timed epochs (nan before the first one)."""
+    return "Process {:03d} | Epoch {:05d} | Time(s) {:.4f} | Comm(s) {:.4f} | Reduce(s) {:.4f} | Loss {:.4f}".format(
+        rank, epoch, np.mean(train_dur) if train_dur else float('nan'), np.mean(comm_dur) if comm_dur else float('nan'),
+        np.mean(reduce_dur) if reduce_dur else float('nan'), loss_per_node)
 
 
 def run(graph, node_dict, gpb, args, device=None, full_graph=None, eval_parts=None):
@@ -686,7 +725,26 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None, eval_parts=No
     ``eval_parts = {'val': ..., 'test': ...}``, this rank's parts of them (``data.load_eval_partition``); without
     ``eval_parts`` an inductive run with ``--parallel-eval`` is refused.
     ``args.save_state_every`` / ``args.resume``: write the training state every N epochs and after the last one, or
-    continue from the saved one (``state.py``)."""
+    continue from the saved one (``state.py``).
+    ``args.cuda_graph``: everything runs on one non-default stream; the first ``min(3, n_epochs - start)`` epochs of
+    this process run eagerly, then one epoch is captured (``GraphedEpoch(st, warmup=0, timed=True)``) and every later
+    epoch is one replay of it.  Configurations it cannot replay are refused before any setup work
+    (``cuda_graph_refusals``)."""
+    if getattr(args, 'cuda_graph', False):
+        why = cuda_graph_refusals(args, ctx.comm())
+        if why:
+            raise ValueError("--cuda-graph: " + "; ".join(why))
+        dev = torch.device(device if device is not None else torch.cuda.current_device())
+        # setup registers the gradient hooks, whose accumulators bind to the current stream: it must be the capture's;
+        # backward runs on this thread, as in the capture
+        with torch.cuda.stream(torch.cuda.Stream(dev)), torch.autograd.set_multithreading_enabled(False):
+            out = _run(graph, node_dict, gpb, args, device, full_graph, eval_parts)
+            torch.cuda.synchronize(dev)
+        return out
+    return _run(graph, node_dict, gpb, args, device, full_graph, eval_parts)
+
+
+def _run(graph, node_dict, gpb, args, device, full_graph, eval_parts):
     rank, size = _rank_size()
     parallel = getattr(args, 'eval', False) and getattr(args, 'parallel_eval', False)
     if parallel and args.inductive and eval_parts is None:
@@ -724,20 +782,25 @@ def run(graph, node_dict, gpb, args, device=None, full_graph=None, eval_parts=No
     torch.cuda.reset_peak_memory_stats(dev)
     print(f'Process {rank} start training')
     loss = None
+    graphed = None
+    n_eager = min(3, args.n_epochs - start) if getattr(args, 'cuda_graph', False) else None
     for epoch in range(start, args.n_epochs):
+        if epoch - start == n_eager:
+            graphed = GraphedEpoch(st, warmup=0, timed=True)               # the eager epochs were its warm-up
         torch.cuda.synchronize(dev)
         t0 = time.time()
-        loss = train_epoch(st, epoch)
+        loss = graphed() if graphed is not None else train_epoch(st, epoch)
         torch.cuda.synchronize(dev)
         if epoch - start >= 5:                                              # train.py:415-418 (epochs of this process)
             train_dur.append(time.time() - t0)
-            comm_dur.append(comm_timer.tot_time())
-            reduce_dur.append(ctx.reducer.last_reduce_seconds())
+            if graphed is not None:
+                comm_s, reduce_s = graphed.interval_seconds()
+            else:
+                comm_s, reduce_s = comm_timer.tot_time(), ctx.reducer.last_reduce_seconds()
+            comm_dur.append(comm_s)
+            reduce_dur.append(reduce_s)
         if (epoch + 1) % args.log_every == 0:
-            print("Process {:03d} | Epoch {:05d} | Time(s) {:.4f} | Comm(s) {:.4f} | Reduce(s) {:.4f} | Loss {:.4f}".format(
-                rank, epoch, np.mean(train_dur) if train_dur else float('nan'),
-                np.mean(comm_dur) if comm_dur else float('nan'),
-                np.mean(reduce_dur) if reduce_dur else float('nan'), loss.item() / max(st.part_train, 1)))
+            print(log_line(rank, epoch, train_dur, comm_dur, reduce_dur, loss.item() / max(st.part_train, 1)))
             if evaluator is not None:                                       # train.py:427-442
                 evaluator.after_epoch(st.model, epoch)
         if save_every > 0 and ((epoch + 1) % save_every == 0 or epoch + 1 == args.n_epochs):

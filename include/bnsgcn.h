@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 11
+#define BNS_ABI_VERSION 12
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -700,6 +700,15 @@ int bns_part_cluster_edges(int64_t n, const int64_t *indptr, const int32_t *cid,
                            const int64_t *ce, int64_t ecap, uint64_t seed, int32_t *target, int64_t *gain, void *stream);
 int bns_part_weights_i64(int64_t n, const int32_t *label, const int64_t *nw, int64_t n_labels, int64_t *out,
                          void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 12: interval stamps inside a captured CUDA graph (train.GraphedEpoch(timed=True), the --cuda-graph log line).
+ * bns_stamp_globaltimer: one single-thread kernel on `stream` that stores the GPU's %globaltimer (nanoseconds) to dst
+ *     (device, 8-byte aligned).  Two stamps on one stream bracket the work enqueued between them, as two CUDA events
+ *     would; unlike events they may sit inside a captured graph and are rewritten at the same address by every replay.
+ *     Differences are only meaningful between stamps of one GPU.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_stamp_globaltimer(uint64_t *dst /*device*/, void *stream);
 
 #ifdef __cplusplus
 }
