@@ -22,15 +22,29 @@ only, and applies the same rules:
 * ``n_class`` is ``label.max() + 1``, or the label width for multi-label data (``utils.py:62-65``).
 
 Malformed input is refused with ``DataFileError`` naming the file, before anything is built from it.  DGL's ``.bin``
-and OGB's ``processed/`` caches are not read.  ogbn-papers100M is refused: its 111 M nodes and 57 GB of features do not
-fit the whole-graph partitioner (``make_local_partition`` generates its shape per rank instead).
+and OGB's ``processed/`` caches are not read.
+
+ogbn-papers100M (111 M nodes, 1.6 B edges, 57 GB of features) is not read whole: ``load_files`` refuses it.
+``read_papers100m`` checks its files and holds only the node tables; the edges and feature rows are read as streams,
+in chunks, by the partition step that writes them into the store (``store.papers100m_partition``):
+
+    ogbn-papers100m ogbn_papers100M/raw/data.npz         edge_index int64 [2, E] (row 0 source, row 1 destination),
+                                                         node_feat [N, F] (float; widened to f32), num_nodes_list [1]
+                    ogbn_papers100M/raw/node-label.npz   node_label [N] or [N, 1], float, NaN where a node has none
+                    ogbn_papers100M/split/time/{train,valid,test}.csv.gz                        (one id per line)
+
+* The same self-loop rule; multi-edges stay; no inverse edges are added (OGB's ``add_inverse_edge`` is off for it).
+* Labels are ``view(-1).long()``; an unlabelled (NaN) node is stored as ``-1``, and no split may hold one.
+  ``n_class`` is ``label.max() + 1``.  Other keys in the archives (``node_year``, ...) are ignored.
 """
 from __future__ import annotations
 
+import dataclasses
 import gzip
 import json
 import os
-from typing import Optional
+import zipfile
+from typing import Iterator, Optional, Tuple
 
 import numpy as np
 import torch
@@ -280,10 +294,179 @@ def _read_products(root: str, device) -> FullGraph:
 _READERS = {"reddit": _read_reddit, "yelp": _read_yelp, "ogbn-products": _read_products}
 
 
+# ---- ogbn-papers100M, read as streams ------------------------------------------------------------------------------
+
+PAPERS100M = ("ogbn-papers100m", "papers100m")
+
+
+def is_papers100m(dataset: str) -> bool:
+    return dataset in PAPERS100M
+
+
+class NpzMember:
+    """One ``.npy`` member of an ``.npz`` archive (stored or deflated), read as a stream: the header is parsed once,
+    rows are read in chunks through a fresh handle, and the array is never loaded whole."""
+
+    def __init__(self, path: str, key: str):
+        self.path, self.key, self.name = path, key, key + ".npy"
+        try:
+            with zipfile.ZipFile(_need(path)) as z:
+                names = z.namelist()
+                if self.name not in names:
+                    raise DataFileError(path, f"no key {key!r} (it holds {sorted(n[:-4] for n in names)})")
+                with z.open(self.name) as f:
+                    version = np.lib.format.read_magic(f)
+                    if version == (1, 0):
+                        shape, fortran, dtype = np.lib.format.read_array_header_1_0(f)
+                    elif version == (2, 0):
+                        shape, fortran, dtype = np.lib.format.read_array_header_2_0(f)
+                    else:
+                        raise ValueError(f".npy format version {version}")
+                    self.offset = f.tell()
+        except DataFileError:
+            raise
+        except Exception as e:                              # not a zip, a corrupt member, an unreadable header
+            raise DataFileError(path, f"{key!r} is not a readable .npy member ({e})") from e
+        if dtype.hasobject:
+            raise DataFileError(path, f"{key!r} holds Python objects")
+        if fortran and len(shape) > 1:
+            raise DataFileError(path, f"{key!r} is stored in Fortran order; only C order is read")
+        self.shape, self.dtype = tuple(int(s) for s in shape), dtype
+        self.row_items = int(np.prod(self.shape[1:], dtype=np.int64))
+
+    def rows(self, chunk: int, start: int = 0, count: Optional[int] = None, flat: bool = False) -> Iterator[np.ndarray]:
+        """Rows ``[start, start + count)`` in chunks of at most ``chunk`` rows (of ``flat`` elements instead, for a
+        [2, E] array read row by row), native byte order."""
+        per = 1 if flat else self.row_items
+        total = (int(np.prod(self.shape, dtype=np.int64)) if flat else self.shape[0]) - start
+        count = total if count is None else count
+        size = self.dtype.itemsize * per
+        try:
+            with zipfile.ZipFile(self.path) as z, z.open(self.name) as f:
+                f.MAX_SEEK_READ = min(f.MAX_SEEK_READ, max(chunk * size, 1 << 16))   # a deflated member is skipped
+                f.seek(self.offset + start * size)                                   # by reading, a chunk at a time
+                done = 0
+                while done < count:
+                    k = min(chunk, count - done)
+                    buf = bytearray(k * size)                   # writable: torch.from_numpy takes it as it is
+                    got = f.readinto(buf)
+                    if got != k * size:
+                        raise DataFileError(self.path, f"{self.key!r} ends after {done + got // size} of {count} rows")
+                    a = np.frombuffer(buf, dtype=self.dtype).astype(self.dtype.newbyteorder("="), copy=False)
+                    yield a if flat else a.reshape((k,) + self.shape[1:])
+                    done += k
+        except DataFileError:
+            raise
+        except (zipfile.BadZipFile, OSError, EOFError, ValueError) as e:    # a corrupt deflate stream or CRC
+            raise DataFileError(self.path, f"{self.key!r}: {e}") from e
+
+    def read(self) -> np.ndarray:
+        """The whole array (only for node-sized members)."""
+        items = int(np.prod(self.shape, dtype=np.int64))
+        if items == 0:
+            return np.empty(self.shape, self.dtype.newbyteorder("="))
+        return next(self.rows(items, flat=True)).reshape(self.shape)
+
+
+@dataclasses.dataclass
+class PapersFiles:
+    """ogbn-papers100M's files, checked: the node tables in memory, the edges and features as streams."""
+    n: int
+    n_feat: int
+    n_edges: int
+    label: np.ndarray           # int64 [N], -1 where a node has no label
+    train: np.ndarray           # bool [N]
+    val: np.ndarray
+    test: np.ndarray
+    n_class: int
+    edge: NpzMember             # edge_index [2, E]
+    feat: NpzMember             # node_feat [N, F]
+
+    def edges(self, chunk: int) -> Iterator[Tuple[np.ndarray, np.ndarray]]:
+        """``(src, dst)`` int64 chunks of at most ``chunk`` edges, every id checked against ``[0, N)``: two handles on
+        the one member, the second advanced past the source row."""
+        e = self.n_edges
+        for src, dst in zip(self.edge.rows(chunk, 0, e, flat=True), self.edge.rows(chunk, e, e, flat=True)):
+            for a in (src, dst):
+                if a.size and (int(a.min()) < 0 or int(a.max()) >= self.n):
+                    bad = int(a[(a < 0) | (a >= self.n)][0])
+                    raise DataFileError(self.edge.path, f"edge_index: node id {bad} outside [0, {self.n})")
+            yield src.astype(np.int64, copy=False), dst.astype(np.int64, copy=False)
+
+    def features(self, chunk: int) -> Iterator[np.ndarray]:
+        """f32 ``[k, F]`` chunks of at most ``chunk`` rows, in node order."""
+        for a in self.feat.rows(chunk):
+            yield a.astype(np.float32, copy=False)
+
+
+def _papers_labels(path: str, label: np.ndarray, n: int, splits) -> Tuple[np.ndarray, int]:
+    if label.shape not in ((n,), (n, 1)):
+        raise DataFileError(path, f"node_label has shape {label.shape}, not [{n}] or [{n}, 1]")
+    label = label.reshape(-1)
+    if np.issubdtype(label.dtype, np.integer):
+        known = np.ones(n, dtype=bool)
+        out = label.astype(np.int64)
+    elif np.issubdtype(label.dtype, np.floating):
+        known = np.isfinite(label)
+        out = np.full(n, -1, dtype=np.int64)
+        out[known] = label[known].astype(np.int64)          # view(-1).long(): truncates toward zero
+    else:
+        raise DataFileError(path, f"node_label is {label.dtype}, not a number")
+    for name, ids in splits:
+        miss = ~known[ids]
+        if miss.any():
+            raise DataFileError(path, f"node {int(ids[miss][0])} of the {name} split has no label ({label[ids[miss][0]]})")
+        lab = label[ids]
+        bad = (lab != np.floor(lab)) | (lab < 0) if np.issubdtype(lab.dtype, np.floating) else lab < 0
+        if bad.any():
+            raise DataFileError(path, f"node {int(ids[bad][0])} of the {name} split has the label "
+                                      f"{lab[bad][0]}, not a class")
+    if not known.any():
+        raise DataFileError(path, "no node has a label")
+    return out, int(out.max()) + 1
+
+
+def read_papers100m(root: str) -> PapersFiles:
+    """Check ogbn-papers100M's files under ``root`` and read its node tables (count, labels, splits).  Every refusal
+    but an out-of-range edge id is raised here, before the partition step writes anything; the edge ids are checked
+    as ``PapersFiles.edges`` streams them."""
+    raw = os.path.join(root, "ogbn_papers100M", "raw")
+    split = os.path.join(root, "ogbn_papers100M", "split", "time")
+    data_path = os.path.join(raw, "data.npz")
+    nn = NpzMember(data_path, "num_nodes_list")
+    if nn.shape != (1,) or not np.issubdtype(nn.dtype, np.integer):
+        raise DataFileError(data_path, f"num_nodes_list is {nn.dtype} of shape {nn.shape}; one graph holds one count")
+    n = int(nn.read()[0])
+    _check_n(data_path, n)
+    edge = NpzMember(data_path, "edge_index")
+    if len(edge.shape) != 2 or edge.shape[0] != 2 or not np.issubdtype(edge.dtype, np.integer):
+        raise DataFileError(data_path, f"edge_index is {edge.dtype} of shape {edge.shape}, not integers [2, E]")
+    feat = NpzMember(data_path, "node_feat")
+    if len(feat.shape) != 2 or feat.shape[0] != n:
+        raise DataFileError(data_path, f"node_feat has shape {feat.shape}, not [{n}, F]")
+    if not np.issubdtype(feat.dtype, np.floating):
+        raise DataFileError(data_path, f"node_feat is {feat.dtype}, not float")
+    splits = []
+    for k in ("train", "valid", "test"):
+        p = os.path.join(split, f"{k}.csv.gz")
+        ids = _read_csv(p, np.int64, "node ids")
+        if ids.shape[0] and ids.shape[1] != 1:
+            raise DataFileError(p, f"{ids.shape[1]} columns, not one node id per line")
+        splits.append((k, _ids(p, ids.reshape(-1), n, "split ids").numpy()))
+    label_path = os.path.join(raw, "node-label.npz")
+    label, n_class = _papers_labels(label_path, NpzMember(label_path, "node_label").read(), n, splits)
+    masks = []
+    for _, ids in splits:
+        m = np.zeros(n, dtype=bool)
+        m[ids] = True
+        masks.append(m)
+    return PapersFiles(n, feat.shape[1], edge.shape[1], label, *masks, n_class, edge, feat)
+
+
 def load_files(dataset: str, data_path: str, device: Optional[torch.device] = None) -> FullGraph:
     """``dataset`` read from its published files under ``data_path``, as the ``FullGraph`` ``make_graph`` returns.
     The edges are sorted on ``device`` (default: the GPU when there is one); the CPU builds the identical graph."""
-    if dataset in ("ogbn-papers100m", "papers100m"):
+    if is_papers100m(dataset):
         raise ValueError(f"--dataset {dataset} --data-source files: not supported.  The whole-graph partitioner would "
                          "have to hold 111 M nodes and 57 GB of features on one host; papers100M needs per-rank "
                          "loading, which this build only has for the generated shape")

@@ -255,6 +255,38 @@ def refine_label_propagation(fg: FullGraph, part: torch.Tensor, n_parts: int, ob
     return part.cpu()
 
 
+def _blocks(order: torch.Tensor, n_parts: int) -> torch.Tensor:
+    """``order`` cut into ``n_parts`` blocks of sizes within one node: the owner of every node."""
+    n = order.numel()
+    part = torch.empty(n, dtype=torch.int64)
+    part[order] = (torch.arange(n, dtype=torch.int64) * n_parts) // n
+    return part
+
+
+def random_parts(n: int, n_parts: int, seed: int) -> torch.Tensor:
+    """``--partition-method random``: the owner of every node of an ``n``-node graph, int64 ``[n]``, balanced to one
+    node.  It needs only the node count, so the streaming partition step (``store.papers100m_partition``) calls it
+    too."""
+    if n_parts == 1:
+        return torch.zeros(n, dtype=torch.int64)
+    return _blocks(torch.randperm(n, generator=torch.Generator().manual_seed(seed + 7919)), n_parts)
+
+
+def relabel_ids(part: torch.Tensor, n_parts: int, device: Optional[torch.device] = None):
+    """``(order, new_id, ranges)`` of ``relabel``: new id -> old id, old id -> new id, and the id range of every part
+    (parts in order, each keeping its nodes' old order).  ``order`` and ``new_id`` live on ``device`` (default: the
+    host); every device gives the same ids."""
+    dev = torch.device(device) if device is not None else torch.device("cpu")
+    part = part.to(dev)
+    n = part.numel()
+    order = torch.argsort(part, stable=True)
+    new_id = torch.empty(n, dtype=torch.int64, device=dev)
+    new_id[order] = torch.arange(n, dtype=torch.int64, device=dev)
+    ranges = torch.zeros(n_parts + 1, dtype=torch.int64)
+    ranges[1:] = torch.cumsum(torch.bincount(part, minlength=n_parts).cpu(), 0)
+    return order, new_id, ranges
+
+
 def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective: str = "vol", device=None,
                  balance: str = "nodes") -> torch.Tensor:
     """Owner of every node, int64 ``[N]``: ``random`` balanced to ±1 node, ``metis`` (stand-in) and ``multilevel`` (the
@@ -265,8 +297,7 @@ def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective:
     if n_parts == 1:
         return torch.zeros(n, dtype=torch.int64)
     if method == "random":
-        gen = torch.Generator().manual_seed(seed + 7919)
-        order = torch.randperm(n, generator=gen)
+        order = None
     elif method == "multilevel":                      # the GPU partitioner (data/multilevel.py)
         from .multilevel import multilevel_partition
         return multilevel_partition(fg, n_parts, objective, seed, device, balance)[0]
@@ -277,8 +308,7 @@ def assign_parts(fg: FullGraph, n_parts: int, method: str, seed: int, objective:
         order = torch.from_numpy(np.ascontiguousarray(reverse_cuthill_mckee(a, symmetric_mode=True)).astype(np.int64))
     else:
         raise ValueError(f"unknown partition method {method!r}")
-    part = torch.empty(n, dtype=torch.int64)
-    part[order] = (torch.arange(n, dtype=torch.int64) * n_parts) // n
+    part = random_parts(n, n_parts, seed) if order is None else _blocks(order, n_parts)
     ehi = None
     if balance == "edges":                            # the same blocks with their in-edges evened out by swaps
         deg = fg.in_degrees()
@@ -297,12 +327,7 @@ def relabel(fg: FullGraph, part: torch.Tensor, n_parts: int, device: Optional[to
     if device is None:
         device = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
     n = fg.n_nodes
-    order = torch.argsort(part, stable=True)              # new id -> old id
-    new_id = torch.empty(n, dtype=torch.int64)
-    new_id[order] = torch.arange(n, dtype=torch.int64)
-    counts = torch.bincount(part, minlength=n_parts)
-    ranges = torch.zeros(n_parts + 1, dtype=torch.int64)
-    ranges[1:] = torch.cumsum(counts, 0)
+    order, new_id, ranges = relabel_ids(part, n_parts)
     nid = new_id.to(device)
     dst = nid[fg.dst().to(device)]
     src = nid[fg.src.to(device)]

@@ -27,9 +27,10 @@ from typing import Dict, Optional, Tuple
 import numpy as np
 import torch
 
-from .partition import NID, GraphPartitionBook, LocalGraph, Partition, induced_subgraph, partition_graph
-from .files import data_source, load_graph
-from .synthetic import FullGraph
+from .partition import (NID, GraphPartitionBook, LocalGraph, Partition, induced_subgraph, partition_graph, random_parts,
+                        relabel_ids)
+from .files import data_source, is_papers100m, load_graph, read_papers100m
+from .synthetic import FullGraph, make_local_partition
 
 FORMAT_VERSION = 1
 _BOOL_KEYS = ("inner_node", "train_mask", "val_mask", "test_mask")
@@ -110,12 +111,20 @@ def _write_parts(parts, graph_dir: str, part_config: str, cfg: dict) -> None:
     os.replace(tmp, part_config)
 
 
-def _config_head(args, parts) -> dict:
+def _head(args, ranges: torch.Tensor, n_edges: int) -> dict:
     return {"format_version": FORMAT_VERSION, "graph_name": args.graph_name, "data_source": data_source(args),
             "num_parts": args.n_partitions, "part_method": args.partition_method, "inductive": bool(args.inductive),
             "balance": partition_balance(args),
-            "node_map": [int(x) for x in parts[0].gpb.ranges.tolist()],
-            "num_nodes": int(parts[0].gpb.ranges[-1]), "num_edges": int(sum(p.graph.num_edges() for p in parts))}
+            "node_map": [int(x) for x in ranges.tolist()], "num_nodes": int(ranges[-1]), "num_edges": int(n_edges)}
+
+
+def _config_head(args, parts) -> dict:
+    return _head(args, parts[0].gpb.ranges, sum(p.graph.num_edges() for p in parts))
+
+
+def _write_meta(graph_dir: str, n_feat: int, n_class: int, n_train: int) -> None:
+    with open(os.path.join(graph_dir, 'meta.json'), 'w') as f:
+        json.dump({'n_feat': n_feat, 'n_class': n_class, 'n_train': n_train}, f)
 
 
 def wants_eval_partitions(args) -> bool:
@@ -167,7 +176,10 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
     files with ``--data-source files``), partition it unless the part config already exists, always (re)write
     ``meta.json``.  Returns the part-config path.  Nothing is written before the graph is built and checked.
     With ``--eval --parallel-eval --inductive`` the two evaluation sets (``val/``, ``test/``: ``eval_partitions``) are
-    written too, each unless its own config exists, from the same ``FullGraph``."""
+    written too, each unless its own config exists, from the same ``FullGraph``.
+    ogbn-papers100M (``--dataset ogbn-papers100m``) is never built whole: ``papers100m_partition`` writes its store."""
+    if fg is None and is_papers100m(args.dataset):
+        return papers100m_partition(args, device)
     graph_dir, part_config = _dirs(args)
     if os.path.exists(part_config):
         with open(part_config) as f:
@@ -201,9 +213,238 @@ def graph_partition(args, fg: Optional[FullGraph] = None, device: Optional[torch
         cfg["inductive"], cfg["eval_graph"] = False, which     # a partition of the whole evaluation graph
         _write_parts(parts, eval_dir, eval_config, cfg)
         del parts
-    with open(os.path.join(graph_dir, 'meta.json'), 'w') as f:
-        json.dump({'n_feat': n_feat, 'n_class': n_class, 'n_train': n_train}, f)
+    _write_meta(graph_dir, n_feat, n_class, n_train)
     return part_config
+
+
+# ---- ogbn-papers100M: the store written without the whole graph ---------------------------------------------------
+
+PAPERS_CHUNK = 1 << 21          # edges, or feature rows, read per step: 32 MB of edge ids, 1 GB of 128-wide f32 rows
+
+
+def papers100m_refusals(args) -> list:
+    """Every reason ``args`` cannot train ogbn-papers100M, which is only ever partitioned by streaming (empty: none)."""
+    why = []
+    if args.partition_method != 'random':
+        why.append(f"--partition-method {args.partition_method} partitions the whole graph; only random streams")
+    if partition_balance(args) == 'edges':
+        why.append("--partition-balance edges swaps nodes by in-degree, which would need the degrees before the "
+                   "relabelling pass")
+    if args.inductive:
+        why.append("--inductive needs the train | val subgraph and a whole-graph evaluation set (the reference runs "
+                   "papers100M transductively)")
+    if getattr(args, 'eval', False) and not getattr(args, 'parallel_eval', False):
+        why.append("--eval without --parallel-eval evaluates on rank 0's whole graph; pass --parallel-eval or --no-eval")
+    return why
+
+
+def check_papers100m(args) -> None:
+    """Raise ``ValueError`` naming every reason of ``papers100m_refusals`` (nothing for the other datasets)."""
+    why = papers100m_refusals(args) if is_papers100m(args.dataset) else []
+    if why:
+        raise ValueError(f"--dataset {args.dataset}: " + "; ".join(why))
+
+
+def _finish(graph_dir: str, part_config: str, cfg: dict, meta) -> None:
+    """``meta.json``, then the part config through a temporary file: a store without a config is incomplete."""
+    _write_meta(graph_dir, *meta)
+    tmp = part_config + ".tmp"
+    with open(tmp, 'w') as f:
+        json.dump(cfg, f, indent=1)
+    os.replace(tmp, part_config)
+
+
+def _generated_papers(args, graph_dir: str, part_config: str, device) -> None:
+    """The generated papers100M shape: part r is ``make_local_partition`` of rank r, one part at a time."""
+    entries, n_edges, p = {}, 0, None
+    for r in range(args.n_partitions):
+        p = make_local_partition("papers100m", r, args.n_partitions, seed=getattr(args, 'graph_seed', 0),
+                                 device=device, scale=getattr(args, 'graph_scale', 1.0))
+        entries[f"part-{r}"] = save_partition(p, graph_dir)
+        n_edges += p.graph.num_edges()
+    cfg = _head(args, p.gpb.ranges, n_edges)
+    cfg.update(entries)
+    _finish(graph_dir, part_config, cfg, (p.meta["n_feat"], p.meta["n_class"], p.meta["n_train"]))
+
+
+def _spill_edges(pf, new_id, ranges, spills, dev, chunk: int):
+    """The edge pass: drop self-loops, map both ends to new ids, count the in- and out-degrees, and append every
+    (destination, source) pair, as int64, to the spill file of its destination's part."""
+    n, n_parts = pf.n, len(spills)
+    in_cnt = torch.zeros(n, dtype=torch.int64, device=dev)
+    out_cnt = torch.zeros(n, dtype=torch.int64, device=dev)
+    ranges_d = ranges.to(dev)
+    for src, dst in pf.edges(chunk):
+        s, d = torch.from_numpy(src).to(dev), torch.from_numpy(dst).to(dev)
+        keep = s != d
+        s, d = new_id[s[keep]], new_id[d[keep]]
+        ones = torch.ones(s.numel(), dtype=torch.int64, device=dev)
+        out_cnt.index_add_(0, s, ones)
+        in_cnt.index_add_(0, d, ones)
+        pairs = torch.stack([d, s], 1)
+        if n_parts > 1:
+            owner = torch.searchsorted(ranges_d, d, right=True) - 1
+            pairs = pairs[torch.argsort(owner, stable=True)]
+            counts = torch.bincount(owner, minlength=n_parts).tolist()
+        else:
+            counts = [pairs.shape[0]]
+        pairs = pairs.cpu().numpy()
+        at = 0
+        for f, c in zip(spills, counts):
+            if c:
+                f.write(memoryview(pairs[at:at + c]))
+                at += c
+    return in_cnt.cpu(), out_cnt.cpu()
+
+
+def _streamed_part(pf, r: int, ranges, order, in_cnt, out_cnt, spill_path: str, part_dir: str, dev):
+    """Part ``r`` from its spill file, written as ``save_partition`` writes ``extract_partition``'s piece; the feature
+    file is created at its size with its header, and filled later by ``_stream_features``."""
+    n = pf.n
+    start, end = int(ranges[r]), int(ranges[r + 1])
+    n_in = end - start
+    pairs = torch.from_numpy(np.fromfile(spill_path, dtype=np.int64).reshape(-1, 2)).to(dev)
+    loops = torch.arange(start, end, dtype=torch.int64, device=dev)
+    dst, src = torch.cat([pairs[:, 0], loops]), torch.cat([pairs[:, 1], loops])
+    del pairs
+    perm = torch.argsort(dst * n + src)                    # relabel's sort; equal keys are equal pairs
+    dst, src = dst[perm], src[perm]
+    del perm
+    indptr = torch.zeros(n_in + 1, dtype=torch.int64, device=dev)
+    indptr[1:] = torch.cumsum(torch.bincount(dst - start, minlength=n_in), 0)
+    del dst
+    inner = (src >= start) & (src < end)
+    halo = torch.unique(src[~inner])                       # as extract_partition
+    local = torch.where(inner, src - start, n_in + torch.searchsorted(halo, src))
+    del src, inner
+    n_halo = int(halo.numel())
+    if n_in + n_halo < 2 ** 31:
+        local = local.to(torch.int32)
+    gid = torch.cat([loops, halo])
+    part_id = torch.searchsorted(ranges.to(dev), gid, right=True) - 1
+    inner_node = torch.zeros(gid.numel(), dtype=torch.bool)
+    inner_node[:n_in] = True
+    old = order[start:end].cpu().numpy()
+    os.makedirs(part_dir, exist_ok=True)
+    arrays: Dict[str, object] = {}
+    arrays["indptr"] = _save_array(os.path.join(part_dir, "indptr.npy"), indptr)
+    arrays["indices"] = _save_array(os.path.join(part_dir, "indices.npy"), local)
+    n_edges = int(local.numel())
+    del indptr, local
+    feat_path = os.path.join(part_dir, "node_feat.npy")
+    m = np.lib.format.open_memmap(feat_path, mode="w+", dtype=np.float32, shape=(n_in, pf.n_feat))
+    del m
+    nd = {NID: gid, "part_id": part_id, "inner_node": inner_node, "feat": None,
+          "label": torch.from_numpy(pf.label[old]), "in_deg": in_cnt[start:end] + 1, "out_deg": out_cnt[start:end] + 1,
+          "train_mask": torch.from_numpy(pf.train[old]), "val_mask": torch.from_numpy(pf.val[old]),
+          "test_mask": torch.from_numpy(pf.test[old])}
+    for k, v in nd.items():
+        arrays["node/" + k] = ({"dtype": "float32", "shape": [n_in, pf.n_feat]} if v is None else
+                               _save_array(os.path.join(part_dir, f"node_{k}.npy"), v))
+    return {"dir": os.path.basename(part_dir), "n_in": n_in, "n_halo": n_halo, "n_edges": n_edges, "arrays": arrays}
+
+
+def _stream_features(pf, part: torch.Tensor, n_in, graph_dir: str, chunk: int) -> None:
+    """Every feature row to its part's file (``n_in``: the row count of each).  ``relabel`` keeps each part's nodes in
+    their old order, so each part's rows arrive in file order: every file is appended to, after its header."""
+    n_parts = len(n_in)
+    files = []
+    try:
+        for r in range(n_parts):
+            path = os.path.join(graph_dir, f"part{r}", "node_feat.npy")
+            f = open(path, "r+b")
+            files.append(f)
+            f.seek(os.path.getsize(path) - n_in[r] * pf.n_feat * 4)
+        part = part.numpy()
+        at = 0
+        for rows in pf.features(chunk):
+            k = rows.shape[0]
+            owner = part[at:at + k]
+            at += k
+            if n_parts == 1:
+                files[0].write(memoryview(rows))
+                continue
+            rows = rows[np.argsort(owner, kind="stable")]
+            bounds = np.cumsum(np.bincount(owner, minlength=n_parts)).tolist()
+            for r in range(n_parts):
+                lo = bounds[r - 1] if r else 0
+                if bounds[r] > lo:
+                    files[r].write(memoryview(rows[lo:bounds[r]]))
+    finally:
+        for f in files:
+            f.close()
+
+
+def papers100m_partition(args, device: Optional[torch.device] = None, chunk: int = PAPERS_CHUNK) -> str:
+    """``graph_partition`` for ogbn-papers100M: the store ``partition_graph(fg, P, 'random')`` + ``_write_parts`` would
+    write, byte for byte, without ever holding the whole graph.  Returns the part-config path; a store whose config
+    exists is kept as it is.
+
+    * ``--data-source files``: the checked node tables (``files.read_papers100m``), the owners ``random_parts`` and
+      the ids ``relabel_ids`` give; one pass over the edges (``chunk`` at a time, on ``device``: default the GPU
+      when there is one) counts the degrees and spills every edge to its destination's part under a temporary
+      directory in the store; then each part is sorted and written in turn; then the feature rows are streamed to
+      their parts, ``chunk`` rows at a time.  Host memory: the node tables (a few length-N arrays), one part's
+      largest array, and a few chunks -- nothing proportional to E or to N x F.
+    * ``--data-source synthetic``: part r is ``make_local_partition('papers100m', r, P, seed=args.graph_seed,
+      scale=args.graph_scale)``, the generator ``bench.py`` uses (its ``out_deg`` is its ``in_deg``, and ``n_train``
+      comes from the shape's fraction).
+    The part config is written last; a failure removes the spill directory, and the store directory when this call
+    created it."""
+    import shutil
+    import tempfile
+    check_papers100m(args)
+    graph_dir, part_config = _dirs(args)
+    if os.path.exists(part_config):
+        with open(part_config) as f:
+            cfg = json.load(f)
+        _check_source(cfg, args, part_config)
+        _check_balance(cfg, args, part_config)
+        return part_config
+    if device is None:
+        device = torch.device("cuda") if torch.cuda.is_available() else torch.device("cpu")
+    dev = torch.device(device)
+    pf = read_papers100m(args.data_path) if data_source(args) == "files" else None
+    created = not os.path.isdir(graph_dir)
+    os.makedirs(graph_dir, exist_ok=True)
+    spill_dir = None
+    try:
+        if pf is None:
+            _generated_papers(args, graph_dir, part_config, dev)
+            return part_config
+        n_parts = args.n_partitions
+        part = random_parts(pf.n, n_parts, getattr(args, 'graph_seed', 0))
+        order, new_id, ranges = relabel_ids(part, n_parts, dev)
+        spill_dir = tempfile.mkdtemp(prefix=".spill-", dir=graph_dir)
+        paths = [os.path.join(spill_dir, f"part{r}.bin") for r in range(n_parts)]
+        spills = [open(p, "wb") for p in paths]
+        try:
+            in_cnt, out_cnt = _spill_edges(pf, new_id, ranges, spills, dev, chunk)
+        finally:
+            for f in spills:
+                f.close()
+        del new_id
+        order = order.cpu()
+        cfg = _head(args, ranges, 0)
+        for r in range(n_parts):
+            cfg[f"part-{r}"] = _streamed_part(pf, r, ranges, order, in_cnt, out_cnt, paths[r],
+                                              os.path.join(graph_dir, f"part{r}"), dev)
+            os.remove(paths[r])
+        cfg["num_edges"] = sum(cfg[f"part-{r}"]["n_edges"] for r in range(n_parts))
+        del order, in_cnt, out_cnt
+        _stream_features(pf, part, [cfg[f"part-{r}"]["n_in"] for r in range(n_parts)], graph_dir, chunk)
+        _finish(graph_dir, part_config, cfg, (pf.n_feat, pf.n_class, int(pf.train.sum())))
+        return part_config
+    except BaseException:
+        if created:
+            shutil.rmtree(graph_dir, ignore_errors=True)
+        else:                                              # a store directory without a config holds no complete part
+            for r in range(args.n_partitions):
+                shutil.rmtree(os.path.join(graph_dir, f"part{r}"), ignore_errors=True)
+        raise
+    finally:
+        if spill_dir is not None:
+            shutil.rmtree(spill_dir, ignore_errors=True)
 
 
 def _load_array(path: str, mmap: bool) -> torch.Tensor:

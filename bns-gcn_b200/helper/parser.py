@@ -5,9 +5,12 @@ import argparse
 
 # (flag, type or None for a switch, default, extra argparse keywords)
 _REFERENCE_FLAGS = [
-    ("dataset", str, "reddit", dict(help="synthetic shape to generate: reddit | ogbn-products | yelp | synthetic-10k | "
-                                         "small | tiny; with --data-source files, the dataset to read: reddit | "
-                                         "ogbn-products | yelp")),
+    ("dataset", str, "reddit", dict(help="synthetic shape to generate: reddit | ogbn-products | yelp | "
+                                         "ogbn-papers100m | synthetic-10k | small | tiny; with --data-source files, the "
+                                         "dataset to read: reddit | ogbn-products | yelp | ogbn-papers100m.  "
+                                         "ogbn-papers100m (also papers100m) is partitioned by streaming, one part at a "
+                                         "time: only with --partition-method random, --partition-balance nodes, "
+                                         "transductive, and --parallel-eval or --no-eval")),
     ("data-path", str, "./dataset/", {}),
     ("part-path", str, "./partition/", {}),
     ("graph-name", str, "", {}),
@@ -73,9 +76,9 @@ def build_parser():
                              "and of the full graph, which the partition step writes beside the training parts")
     parser.add_argument(*_spellings("data-source"), default="synthetic", choices=["synthetic", "files"],
                         help="NEW: where the graph comes from.  synthetic generates the --dataset shape from a seed.  "
-                             "files reads reddit, yelp or ogbn-products from the files DGL / OGB leave under "
-                             "--data-path (reddit/, yelp/, ogbn_products/raw and split/); the store's default graph "
-                             "name then carries a 'files' token")
+                             "files reads reddit, yelp, ogbn-products or ogbn-papers100m from the files DGL / OGB "
+                             "leave under --data-path (reddit/, yelp/, ogbn_products/ and ogbn_papers100M/ raw and "
+                             "split/); the store's default graph name then carries a 'files' token")
     parser.add_argument(*_spellings("agg-dtype"), default="f32", choices=["f32", "bf16", "fp8"],
                         help="NEW: element type of the rows the wide (hidden-width) aggregation passes gather.  bf16 "
                              "rounds them to bf16 (nearest even) before each pass -- h_u forward, the transposed "

@@ -2,7 +2,12 @@
 ``--data-source files``; nothing is downloaded), partition it into the on-disk store (``data/store.py``:
 ``graph_partition`` unless ``--skip-partition``), start one process per partition / GPU; each loads its part
 (``load_partition``; with ``--eval --parallel-eval --inductive`` also its parts of the two evaluation graphs,
-``load_eval_partition``) and runs ``train.run``.
+``load_eval_partition``) and runs ``train.run``.  ogbn-papers100M is never built whole: its store is written by
+streaming (``store.papers100m_partition``), and the configurations that would need its whole graph are refused at
+launch (``store.check_papers100m``).
+
+    python -m bns_gcn_b200.main --dataset ogbn-papers100m --data-source files --data-path ./dataset/ \
+        --n-partitions 8 --partition-method random --use-pp --parallel-eval
 
     python -m bns_gcn_b200.main --dataset reddit --n-partitions 4 --model graphsage --n-layers 3 --n-hidden 256 \
         --sampling-rate 0.1 --use-pp --partition-method random --n-epochs 50 --no-eval
@@ -17,8 +22,8 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from .data.store import (EVAL_GRAPHS, default_graph_name, graph_partition, load_eval_partition, load_partition,
-                         wants_eval_partitions)
+from .data.store import (EVAL_GRAPHS, check_papers100m, default_graph_name, graph_partition, load_eval_partition,
+                         load_partition, wants_eval_partitions)
 from .helper.parser import create_parser
 
 
@@ -51,6 +56,7 @@ def init_processes(rank, size, args):
 
 def main(argv=None):
     args = create_parser(argv)
+    check_papers100m(args)                                  # before anything is read or written
     if args.fix_seed is False:
         if args.parts_per_node < args.n_partitions:
             warnings.warn('Please enable `--fix-seed` for multi-node training.')

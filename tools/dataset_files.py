@@ -80,6 +80,26 @@ def write_products(fg, root: str) -> str:
 WRITERS = {"reddit": write_reddit, "yelp": write_yelp, "ogbn-products": write_products}
 
 
+def write_papers100m(fg, root: str, compressed: bool = False) -> str:
+    """ogbn-papers100M's raw layout (``data.read_papers100m``): every edge of ``fg`` as stored, self-loops and
+    duplicates included (row = source), in CSR order; labels as float32 with NaN where ``fg.label`` is negative;
+    ``compressed`` deflates the two archives.  Not in ``WRITERS``: ``load_files`` does not read this layout, the
+    streaming partition step does."""
+    raw = os.path.join(root, "ogbn_papers100M", "raw")
+    split = os.path.join(root, "ogbn_papers100M", "split", "time")
+    os.makedirs(raw, exist_ok=True)
+    os.makedirs(split, exist_ok=True)
+    save = np.savez_compressed if compressed else np.savez
+    save(os.path.join(raw, "data.npz"), edge_index=np.stack([fg.src.numpy(), fg.dst().numpy()]),
+         node_feat=fg.feat.numpy(), num_nodes_list=np.array([fg.n_nodes], dtype=np.int64))
+    label = fg.label.numpy().astype(np.float32)
+    label[fg.label.numpy() < 0] = np.nan
+    save(os.path.join(raw, "node-label.npz"), node_label=label.reshape(-1, 1))
+    for name, m in (("train", fg.train_mask), ("valid", fg.val_mask), ("test", fg.test_mask)):
+        _write_csv(os.path.join(split, f"{name}.csv.gz"), np.nonzero(m.numpy())[0], "%d")
+    return os.path.join(root, "ogbn_papers100M")
+
+
 def standard_scaled(fg):
     """``fg`` with its features standardised as the Yelp reader does (``StandardScaler`` fit on the training rows)."""
     import dataclasses
