@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 12
+ABI_VERSION = 13
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -204,6 +204,22 @@ SIGNATURES = {
     "bns_part_weights_i64": (c_int, [c_int64, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     # ---- ABI 12 ----
     "bns_stamp_globaltimer": (c_int, [c_void_p, c_void_p]),
+    # ---- ABI 13 ----
+    "bns_gatv2_scores_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
+                                     c_int64, c_void_p, c_int64, c_void_p, c_float, c_float, c_uint64, c_uint64, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "bns_gatv2_bwd_workspace_bytes": (c_size_t, [c_int64, c_int32, c_int32]),
+    "bns_gatv2_softmax_bwd_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32,
+                                          c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_float, c_float, c_uint64,
+                                          c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64,
+                                          c_void_p, c_void_p, c_size_t, c_void_p]),
+    "bns_gatv2_colsum_f32": (c_int, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_int64, c_void_p, c_int64, c_void_p,
+                                     c_float, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "bns_gatv2_infer_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int32, c_int32, c_float,
+                                    c_void_p, c_int64, c_void_p]),
+    "bns_gatv2_infer_block_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int32, c_int32,
+                                          c_float, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_int64,
+                                          c_void_p]),
 }
 
 

@@ -467,3 +467,173 @@ def gat_infer_block(a: ops.DeviceGraph, ft: Optional[torch.Tensor], el: Optional
                                           acc.stride(0), 1 if first else 0, 1 if last else 0, ops._ptr(bias),
                                           ops._ptr(rst), rst.stride(0) if rst is not None else HF,
                                           torch.cuda.current_stream(a.device).cuda_stream), "bns_gat_infer_block_f32")
+
+
+_GATV2_WS = {}
+
+
+class Gatv2Attention(torch.autograd.Function):
+    """The attention of ``dgl.nn.GATv2Conv`` (``share_weights=False``) for all heads:
+
+        s_uv = sum_f attn[h, f] * leaky_relu(z_src[u, h, f] + z_dst[v, h, f])
+        rst_v = sum_u attn_drop(edge_softmax(s))_uv * z_src[u]
+
+    over the inner entries and this epoch's sampled halo entries, as ``GatAttention``.  ``zs [n_u, H * Fp]``,
+    ``zd [n_in, H * Fp]``, ``attn [1, H, Fp]`` (per-head widths padded to ``Fp``, pad columns zero) -> ``[n_in, H * Fp]``;
+    gradients for all three.
+
+    Stages (include/bnsgcn.h, ABI 13): ``bns_gatv2_scores_f32`` (F-wide scores -> probabilities + dropped attention per
+    entry) -> ``bns_spmm_weighted_f32`` / ``bns_spmm_compact_f32`` per head; backward ``bns_sddmm_dot_f32`` ->
+    ``bns_gatv2_softmax_bwd_f32`` (d s, d z_dst, d attn) -> ``bns_spmm_weighted_f32`` on the transposes +
+    ``bns_gatv2_colsum_f32`` (d z_src)."""
+
+    @staticmethod
+    def forward(ctx, zs, zd, attn, g: PartitionGraph, H: int, Fp: int, slope: float, p: float, seed: int):
+        from ._lib import check, lib
+        zs, zd = zs.contiguous(), zd.contiguous()
+        av = attn.reshape(-1).contiguous()
+        n_in, dev = g.n_in, zs.device
+        c = g.compact if (g.a_out is not None and zs.shape[0] > n_in) else None
+        if c is None and g.a_out is not None and g.a_out.nnz and zs.shape[0] > n_in:
+            raise RuntimeError("Gatv2Attention: halo rows were passed but the partition graph has no compaction "
+                               "(refresh_compaction)")
+        if c is not None and c.cpos is None:
+            raise RuntimeError("Gatv2Attention: the partition graph was compacted without positions (want_positions)")
+        rst = torch.empty(n_in, H * Fp, dtype=torch.float32, device=dev)
+        p_in = torch.empty(max(g.a_in.nnz, 1), H, dtype=torch.float32, device=dev)
+        p_out = torch.empty(max(g.a_out.nnz, 1), H, dtype=torch.float32, device=dev) if c is not None else None
+        w_in = torch.empty_like(p_in) if p > 0 else None
+        w_out = torch.empty_like(p_out) if p > 0 and p_out is not None else None
+        wc = torch.empty_like(p_out) if p_out is not None else None
+        off, off_dev = ops.RNG["offset"], ops.RNG["offset_dev"]
+        head = (g.a_in._h, None if c is None else g.a_out._h, None if c is None else c.cidx.data_ptr(),
+                None if c is None else c.chunk_cnt.data_ptr(), None if c is None else c.cpos.data_ptr(), n_in, H, Fp)
+        tail = (zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0), av.data_ptr(), float(slope), float(p),
+                seed & (2 ** 64 - 1), off & (2 ** 64 - 1), ops._ptr(off_dev))
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):
+            check(lib.bns_gatv2_scores_f32(*head, *tail, p_in.data_ptr(), ops._ptr(p_out), ops._ptr(w_in),
+                                           ops._ptr(w_out), ops._ptr(wc), st), "bns_gatv2_scores_f32")
+        for h in range(H):
+            cols = slice(h * Fp, (h + 1) * Fp)
+            ops.spmm_weighted(g.a_in, zs[:n_in, cols], rst[:, cols], p_in if w_in is None else w_in, h)
+            if c is not None:
+                ops.spmm_compact(c, zs[n_in:, cols], rst[:, cols], accumulate=True, weights=wc, head=h)
+        ctx.g, ctx.c, ctx.head, ctx.tail, ctx.cfg = g, c, head, tail, (H, Fp, slope, attn.shape)
+        saved = [zs, zd, av, p_in] + ([p_out] if p_out is not None else [])
+        if w_in is not None:
+            saved += [w_in] + ([w_out] if w_out is not None else [])
+        ctx.n_w = 0 if w_in is None else (2 if w_out is not None else 1)
+        ctx.save_for_backward(*saved)
+        return rst
+
+    @staticmethod
+    def backward(ctx, d_rst):
+        from ._lib import check, lib
+        g, c = ctx.g, ctx.c
+        H, Fp, slope, shape = ctx.cfg
+        zs, zd, av, p_in, *rest = ctx.saved_tensors
+        p_out = rest.pop(0) if c is not None else None
+        d_rst = d_rst.contiguous()
+        dev, n_in, n_u = zs.device, g.n_in, zs.shape[0]
+        de_in = torch.empty_like(p_in)
+        de_out = torch.empty_like(p_out) if p_out is not None else None
+        w_in, w_out = p_in, p_out
+        if ctx.n_w:
+            w_in = rest.pop(0)
+            w_out = rest.pop(0) if ctx.n_w == 2 else None
+        for h in range(H):                                     # d a'_uv = <d rst_v, z_src[u]>
+            cols = slice(h * Fp, (h + 1) * Fp)
+            ops.sddmm_dot(g.a_in, d_rst[:, cols], zs[:n_in, cols], out=de_in[:, h])
+            if c is not None:
+                ops.sddmm_dot(g.a_out, d_rst[:, cols], zs[n_in:, cols], col_map=g.slot, n_direct=0, out=de_out[:, h])
+        d_zd = torch.empty(n_in, H * Fp, dtype=torch.float32, device=dev)
+        d_attn = torch.empty(H * Fp, dtype=torch.float32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):                           # the workspace's size follows this device's SM count
+            need = lib.bns_gatv2_bwd_workspace_bytes(n_in, H, Fp)
+            key = (dev, need, st)
+            ws = _GATV2_WS.get(key)
+            if ws is None:
+                ws = _GATV2_WS[key] = torch.empty(max(need, 16), dtype=torch.uint8, device=dev)
+            check(lib.bns_gatv2_softmax_bwd_f32(*ctx.head, *ctx.tail, p_in.data_ptr(), ops._ptr(p_out), de_in.data_ptr(),
+                                                ops._ptr(de_out), d_zd.data_ptr(), d_zd.stride(0), d_attn.data_ptr(),
+                                                ws.data_ptr(), ws.numel(), st), "bns_gatv2_softmax_bwd_f32")
+        d_zs = torch.empty(n_u, H * Fp, dtype=torch.float32, device=dev)
+        for h in range(H):                                     # A'^T d rst
+            cols = slice(h * Fp, (h + 1) * Fp)
+            ops.spmm_weighted(g.a_in_t, d_rst[:, cols], d_zs[:n_in, cols], w_in, h, through_perm=True)
+            if c is not None:
+                ops.spmm_weighted(g.a_out_t, d_rst[:, cols], d_zs[n_in:, cols], w_out, h, through_perm=True,
+                                  row_map=g.slot)
+        zargs = (zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0), av.data_ptr(), float(slope))
+        with torch.cuda.device(dev):                           # + the score's share of d z_src
+            check(lib.bns_gatv2_colsum_f32(g.a_in_t._h, de_in.data_ptr(), H, Fp, *zargs, None, 0, d_zs.data_ptr(),
+                                           d_zs.stride(0), st), "bns_gatv2_colsum_f32")
+            if c is not None:
+                check(lib.bns_gatv2_colsum_f32(g.a_out_t._h, de_out.data_ptr(), H, Fp, *zargs, g.slot.data_ptr(), n_in,
+                                               d_zs.data_ptr(), d_zs.stride(0), st), "bns_gatv2_colsum_f32")
+        return d_zs, d_zd, d_attn.view(shape), None, None, None, None, None, None
+
+
+def _gatv2_check(who: str, a: ops.DeviceGraph, H: int, Fp: int, tensors) -> None:
+    """Refuses, before any launch, what the GATv2 inference kernels do not take: ``tensors`` are ``(t, name, shape)``
+    with ``t`` None to skip."""
+    from ._lib import BnsError
+    why = gat_unsupported(H, Fp)
+    if why is not None or Fp % 4:
+        raise BnsError(f"{who}: {why or f'padded width {Fp} is not a multiple of 4'}")
+    for t, name, shape in tensors:
+        if t is None:
+            continue
+        ops._req(t, torch.float32, name)
+        if t.device != a.device:
+            raise BnsError(f"{who}: {name} is on {t.device}, the graph on {a.device}")
+        if tuple(t.shape) != tuple(shape) or t.stride(-1) != 1 or (t.dim() == 2 and name in ("m", "l")
+                                                                   and not t.is_contiguous()):
+            raise BnsError(f"{who}: {name} must be {list(shape)} with unit column stride, got {tuple(t.shape)}")
+
+
+def gatv2_infer(a: ops.DeviceGraph, zs: torch.Tensor, zd: torch.Tensor, attn: torch.Tensor, H: int, Fp: int,
+                slope: float) -> torch.Tensor:
+    """The evaluation forward of ``dgl.nn.GATv2Conv``'s attention on a homogeneous graph ``a`` (``bns_gatv2_infer_f32``):
+
+        rst[v] = sum_{u -> v} softmax_u(sum_f attn[h, f] leaky_relu(zs[u, h, f] + zd[v, h, f])) * zs[u, h, :]
+
+    ``zs [a.n_cols, H * Fp]``, ``zd [a.n_rows, H * Fp]`` (head-major, ``Fp`` a multiple of 4, pad columns zero),
+    ``attn`` with ``H * Fp`` elements -> ``[a.n_rows, H * Fp]``.  No dropout, no gradient."""
+    from ._lib import check, lib
+    HF = H * Fp
+    av = attn.reshape(-1).contiguous()
+    _gatv2_check("gatv2_infer", a, H, Fp, ((zs, "zs", (a.n_cols, HF)), (zd, "zd", (a.n_rows, HF)), (av, "attn", (HF,))))
+    rst = torch.empty(a.n_rows, HF, dtype=torch.float32, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.bns_gatv2_infer_f32(a._h, zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0), av.data_ptr(), H, Fp,
+                                      float(slope), rst.data_ptr(), rst.stride(0),
+                                      torch.cuda.current_stream(a.device).cuda_stream), "bns_gatv2_infer_f32")
+    return rst
+
+
+def gatv2_infer_block(a: ops.DeviceGraph, zs: Optional[torch.Tensor], zd: torch.Tensor, attn: torch.Tensor, H: int,
+                      Fp: int, slope: float, m: torch.Tensor, l: torch.Tensor, acc: torch.Tensor, first: bool,
+                      last: bool, rst: Optional[torch.Tensor] = None) -> None:
+    """One column block of ``gatv2_infer`` (``bns_gatv2_infer_block_f32``), the online-softmax state ``m``, ``l``
+    ``[a.n_rows, H]`` and ``acc [a.n_rows, H * Fp]`` carried as in ``gat_infer_block``; ``last`` writes ``acc / l`` to
+    ``rst`` (may be ``acc``).  ``zs [a.n_cols, H * Fp]`` are this block's source rows (None when it has no entries)."""
+    from ._lib import BnsError, check, lib
+    HF = H * Fp
+    if a.nnz and zs is None:
+        raise BnsError("gatv2_infer_block: a block with entries needs zs")
+    if last and rst is None:
+        raise BnsError("gatv2_infer_block: the last block needs rst")
+    av = attn.reshape(-1).contiguous()
+    _gatv2_check("gatv2_infer_block", a, H, Fp, ((zs, "zs", (a.n_cols, HF)), (zd, "zd", (a.n_rows, HF)),
+                                                 (av, "attn", (HF,)), (m, "m", (a.n_rows, H)), (l, "l", (a.n_rows, H)),
+                                                 (acc, "acc", (a.n_rows, HF)), (rst, "rst", (a.n_rows, HF))))
+    with torch.cuda.device(a.device):
+        check(lib.bns_gatv2_infer_block_f32(a._h, ops._ptr(zs), zs.stride(0) if zs is not None else HF, zd.data_ptr(),
+                                            zd.stride(0), av.data_ptr(), H, Fp, float(slope), m.data_ptr(), l.data_ptr(),
+                                            acc.data_ptr(), acc.stride(0), 1 if first else 0, 1 if last else 0,
+                                            ops._ptr(rst), rst.stride(0) if rst is not None else HF,
+                                            torch.cuda.current_stream(a.device).cuda_stream),
+              "bns_gatv2_infer_block_f32")

@@ -14,7 +14,9 @@ _REFERENCE_FLAGS = [
     ("data-path", str, "./dataset/", {}),
     ("part-path", str, "./partition/", {}),
     ("graph-name", str, "", {}),
-    ("model", str, "graphsage", {}),
+    ("model", str, "graphsage", dict(help="graphsage | gcn | gat | gatv2.  gatv2 (NEW) is GAT with dynamic attention "
+                                          "(GATv2Conv: the score attn . leaky_relu(z_src[u] + z_dst[v]) per head), on the "
+                                          "same layer stack, heads, norms and limits as gat")),
     ("dropout", float, 0.5, {}),
     ("lr", float, 1e-2, {}),
     ("sampling-rate", float, 1, {}),

@@ -150,8 +150,8 @@ class GATConv(nn.Module):
         return acc.view(-1, H, Fp)[..., :Fo]
 
 
-def _refuse_zero_in_degree(graph) -> None:
+def _refuse_zero_in_degree(graph, layer: str = "GATConv") -> None:
     if graph.has_zero_in_degree():
-        # dgl.nn.GATConv(allow_zero_in_degree=False) refuses such a graph (DGLError)
-        raise RuntimeError("GATConv: there are 0-in-degree nodes in the graph, their output would be invalid; "
+        # dgl.nn.GATConv / GATv2Conv(allow_zero_in_degree=False) refuse such a graph (DGLError)
+        raise RuntimeError(f"{layer}: there are 0-in-degree nodes in the graph, their output would be invalid; "
                            "add self-loops")

@@ -129,12 +129,16 @@ class GraphSAGE(GNNBase):
 
 class GAT(GNNBase):
     """module/model.py:96-132: attention layers take the ``(source rows, destination rows)`` pair, heads are averaged,
-    dropout sits inside the attention layers (and before the closing linear layers only)."""
+    dropout sits inside the attention layers (and before the closing linear layers only).  ``conv`` is the attention
+    layer's class, built as ``conv(in, out, heads, dropout, dropout)``: ``GATConv`` (the default) or ``GATv2Conv``
+    (``--model gatv2``)."""
 
-    def __init__(self, layer_size, activation, use_pp, heads=1, dropout=0.5, norm='layer', train_size=None, n_linear=0):
+    def __init__(self, layer_size, activation, use_pp, heads=1, dropout=0.5, norm='layer', train_size=None, n_linear=0,
+                 conv=None):
         super().__init__(layer_size, activation, use_pp, dropout, norm, n_linear)
-        from .gat import GATConv
-        self._populate(layer_size, lambda i, a, b: GATConv(a, b, heads, dropout, dropout), norm, train_size)
+        if conv is None:
+            from .gat import GATConv as conv
+        self._populate(layer_size, lambda i, a, b: conv(a, b, heads, dropout, dropout), norm, train_size)
         for i, layer in enumerate(self.layers):
             layer._layer_index = i              # salts the Philox stream of the layer's attention dropout
 

@@ -233,7 +233,7 @@ def precompute(part: PartitionGraph, graph, node_dict, boundary, model, gpb, pos
             # fn.mean divides by the number of messages = the full in-degree (every in-edge is present here)
             mean = PartitionAggregate.apply(h_u, g, 1.0 / node_dict['in_deg'].float(), None, None, None)
             return torch.cat([feat, mean[:, :n_feat]], dim=1)
-        elif model == 'gat':
+        elif model in ('gat', 'gatv2'):
             return h_u[:, :n_feat]
         raise Exception
 
@@ -292,6 +292,10 @@ def create_model(layer_size, args):
                          train_size=args.n_train, n_linear=args.n_linear)
     elif args.model == 'gat':
         return GAT(layer_size, F.relu, use_pp=True, heads=args.heads, norm=args.norm, dropout=args.dropout)
+    elif args.model == 'gatv2':
+        from .module.gatv2 import GATv2Conv
+        return GAT(layer_size, F.relu, use_pp=True, heads=args.heads, norm=args.norm, dropout=args.dropout,
+                   train_size=args.n_train, n_linear=args.n_linear, conv=GATv2Conv)
     raise NotImplementedError(args.model)
 
 
@@ -450,7 +454,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     node_dict = dict(node_dict)
     in_graph, out_graph = get_in_out_graph(graph, node_dict, dev, getattr(args, 'chunk_nnz', 0))
     part = PartitionGraph(graph.n_in, graph.n_halo, in_graph, out_graph, dev)
-    part.want_positions = args.model == 'gat'          # the fused attention keeps per-entry values at CSR positions
+    part.want_positions = args.model in ('gat', 'gatv2')   # the attention keeps per-entry values at CSR positions
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
     agg = check_agg_dtype(args, layer_size, dev)
@@ -569,7 +573,7 @@ def _forward_logits(st: TrainState, epoch: int, selected: Optional[list] = None)
         return st.model(g, st.feat, st.in_norm, st.out_norm)
     elif args.model == 'graphsage':
         return st.model(g, st.feat, st.in_norm)
-    elif args.model == 'gat':
+    elif args.model in ('gat', 'gatv2'):
         return st.model(g, construct_feat(g.num_nodes('_V'), st.feat, st.pos, one_hops))        # train.py:401-402
     raise NotImplementedError
 

@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 12
+#define BNS_ABI_VERSION 13
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -709,6 +709,47 @@ int bns_part_weights_i64(int64_t n, const int32_t *label, const int64_t *nw, int
  *     Differences are only meaningful between stamps of one GPU.
  * ----------------------------------------------------------------------------------------------*/
 int bns_stamp_globaltimer(uint64_t *dst /*device*/, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 13: GATv2Conv's dynamic attention (--model gatv2, csrc/gatv2.cuh).  z_src [n_u, heads * Fp], z_dst [n_in, heads * Fp]
+ * and attn [heads * Fp] are head-major with the per-head width padded to Fp (a multiple of 4, pad columns zero), 16-byte
+ * aligned rows; 1 <= heads <= 8 and heads * Fp <= 1024.  Per entry u -> v and head h
+ *     s_uv = sum_f attn[h, f] * leaky_relu(z_src[u, h, f] + z_dst[v, h, f], slope).
+ * bns_gatv2_scores_f32: bns_gat_scores_f32 with these scores: the same graph arguments, P / W / W_out_compact outputs and
+ *     dropout mask (one Philox4x32-10 call per entry and 4 heads).  The aggregation A' z_src is bns_spmm_weighted_f32 /
+ *     bns_spmm_compact_f32 and d a' is bns_sddmm_dot_f32, as for GAT.
+ * bns_gatv2_softmax_bwd_f32: dE holds d a' at the original positions; writes d s = P (d P - sum_u P d P) in place
+ *     (d P = d a' * mask / (1 - p)), d_zd [n_in, heads * Fp] (row stride ldd) = sum_u d s_uv attn * lrelu'(z_src[u] +
+ *     z_dst[v]) and d_attn [heads * Fp] = sum over entries of d s_uv lrelu(z_src[u] + z_dst[v]) from one partial per warp
+ *     summed in a fixed order (ws: bns_gatv2_bwd_workspace_bytes(n_in, heads, Fp) bytes, 16-byte aligned).
+ * bns_gatv2_colsum_f32: on a transpose gT (bns_graph_transpose) of a_in, or of a_out with row_map = slot and out_base =
+ *     n_in: d_zs[out_base + orow(r)] += sum over the entries k of row r of dS[perm[k], h] attn * lrelu'(z_src[out_base +
+ *     orow(r)] + z_dst[gT.indices[k]]) (rows with row_map -1 skipped).  Accumulates onto A'^T d rst.
+ * bns_gatv2_infer_f32: the evaluation forward on a homogeneous graph: rst = sum_u softmax_u(s_uv) z_src[u], one pass per
+ *     row, nothing stored per entry.  bns_gatv2_infer_block_f32: the same over column blocks, the state m, l [n_rows,
+ *     heads] and acc [n_rows, heads * Fp] carried between launches as in bns_gat_infer_block_f32 (no bias).
+ * Every kernel sums in an order fixed by the inputs: two launches give bit-identical results.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_gatv2_scores_f32(const bns_graph_t *a_in, const bns_graph_t *a_out, const int32_t *cidx, const int32_t *chunk_cnt,
+                         const int32_t *cpos, int64_t x_halo_base, int32_t heads, int32_t Fp, const float *zs, int64_t ldzs,
+                         const float *zd, int64_t ldzd, const float *attn, float slope, float p_drop, uint64_t seed,
+                         uint64_t offset, const uint64_t *offset_dev, float *P_in, float *P_out, float *W_in, float *W_out,
+                         float *W_out_compact, void *stream);
+size_t bns_gatv2_bwd_workspace_bytes(int64_t n_rows, int32_t heads, int32_t Fp);
+int bns_gatv2_softmax_bwd_f32(const bns_graph_t *a_in, const bns_graph_t *a_out, const int32_t *cidx,
+                              const int32_t *chunk_cnt, const int32_t *cpos, int64_t x_halo_base, int32_t heads, int32_t Fp,
+                              const float *zs, int64_t ldzs, const float *zd, int64_t ldzd, const float *attn, float slope,
+                              float p_drop, uint64_t seed, uint64_t offset, const uint64_t *offset_dev, const float *P_in,
+                              const float *P_out, float *dE_in, float *dE_out, float *d_zd, int64_t ldd, float *d_attn,
+                              void *ws, size_t ws_bytes, void *stream);
+int bns_gatv2_colsum_f32(const bns_graph_t *gT, const float *dS, int32_t heads, int32_t Fp, const float *zs, int64_t ldzs,
+                         const float *zd, int64_t ldzd, const float *attn, float slope, const int32_t *row_map,
+                         int64_t out_base, float *d_zs, int64_t ldd, void *stream);
+int bns_gatv2_infer_f32(const bns_graph_t *g, const float *zs, int64_t ldzs, const float *zd, int64_t ldzd,
+                        const float *attn, int32_t heads, int32_t Fp, float slope, float *rst, int64_t ldr, void *stream);
+int bns_gatv2_infer_block_f32(const bns_graph_t *g, const float *zs, int64_t ldzs, const float *zd, int64_t ldzd,
+                              const float *attn, int32_t heads, int32_t Fp, float slope, float *m, float *l, float *acc,
+                              int64_t ldacc, int first, int last, float *rst, int64_t ldr, void *stream);
 
 #ifdef __cplusplus
 }
