@@ -637,3 +637,114 @@ def gatv2_infer_block(a: ops.DeviceGraph, zs: Optional[torch.Tensor], zd: torch.
                                             ops._ptr(rst), rst.stride(0) if rst is not None else HF,
                                             torch.cuda.current_stream(a.device).cuda_stream),
               "bns_gatv2_infer_block_f32")
+
+
+SAGE_MAX_WIDTH = 1024
+
+
+class SageMax(torch.autograd.Function):
+    """The max-pooling aggregation of ``dgl.nn.SAGEConv(in, out, 'pool')`` after its ``fc_pool``:
+
+        z = relu(y),   m[v, f] = max over the inner entries and this epoch's sampled halo entries u -> v of z[u, f]
+
+    (0 for a row without entries).  ``y [n_u, Fp]`` (``Fp`` a multiple of 4, at most 1024) -> ``m [n_in, Fp]``.  The
+    forward (``bns_sage_max_f32``) records each column's winner, the first entry in walk order whose z is the max, at
+    its CSR position (the partition graph's compaction with positions, so a multi-edge is credited once); the backward
+    (``bns_sage_max_bwd_f32`` on the static transposes) sends ``d m`` to the winners only, times ``relu'(y)``."""
+
+    @staticmethod
+    def forward(ctx, y, g: PartitionGraph):
+        from ._lib import check, lib
+        n_in, dev, Fp = g.n_in, y.device, y.shape[1]
+        z = torch.relu(y).contiguous()
+        c = g.compact if (g.a_out is not None and z.shape[0] > n_in) else None
+        if c is None and g.a_out is not None and g.a_out.nnz and z.shape[0] > n_in:
+            raise RuntimeError("SageMax: halo rows were passed but the partition graph has no compaction "
+                               "(refresh_compaction)")
+        if c is not None and c.cpos is None:
+            raise RuntimeError("SageMax: the partition graph was compacted without positions (want_positions)")
+        m = torch.empty(n_in, Fp, dtype=torch.float32, device=dev)
+        win = torch.empty(n_in, Fp, dtype=torch.int32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):
+            check(lib.bns_sage_max_f32(g.a_in._h, None if c is None else g.a_out._h,
+                                       None if c is None else c.cidx.data_ptr(),
+                                       None if c is None else c.chunk_cnt.data_ptr(),
+                                       None if c is None else c.cpos.data_ptr(), n_in, Fp, z.data_ptr(), z.stride(0),
+                                       m.data_ptr(), win.data_ptr(), st), "bns_sage_max_f32")
+        ctx.g, ctx.halo = g, c is not None
+        ctx.save_for_backward(z, win)
+        return m
+
+    @staticmethod
+    def backward(ctx, dm):
+        from ._lib import check, lib
+        g = ctx.g
+        z, win = ctx.saved_tensors
+        dm = dm.contiguous()
+        dev, n_in, Fp = z.device, g.n_in, z.shape[1]
+        dy = torch.empty_like(z)
+        if not ctx.halo and z.shape[0] > n_in:
+            dy[n_in:].zero_()                                  # halo rows without halo entries
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):
+            check(lib.bns_sage_max_bwd_f32(g.a_in_t._h, 0, None, 0, Fp, win.data_ptr(), dm.data_ptr(), z.data_ptr(),
+                                           z.stride(0), dy.data_ptr(), st), "bns_sage_max_bwd_f32")
+            if ctx.halo:
+                check(lib.bns_sage_max_bwd_f32(g.a_out_t._h, g.a_in.nnz, g.slot.data_ptr(), n_in, Fp, win.data_ptr(),
+                                               dm.data_ptr(), z.data_ptr(), z.stride(0), dy.data_ptr(), st),
+                      "bns_sage_max_bwd_f32")
+        return dy, None
+
+
+def _sage_check(who: str, a: ops.DeviceGraph, tensors) -> None:
+    """Refuses, before any launch, what the max kernels do not take: ``tensors`` are ``(t, name, shape, dtype)`` with
+    ``t`` None to skip."""
+    from ._lib import BnsError
+    for t, name, shape, dtype in tensors:
+        if t is None:
+            continue
+        ops._req(t, dtype, name)
+        if t.device != a.device:
+            raise BnsError(f"{who}: {name} is on {t.device}, the graph on {a.device}")
+        if tuple(t.shape) != tuple(shape) or not t.is_contiguous():
+            raise BnsError(f"{who}: {name} must be a contiguous {list(shape)}, got {tuple(t.shape)}")
+        if t.dim() == 2 and (t.shape[1] % 4 or t.shape[1] > SAGE_MAX_WIDTH):
+            raise BnsError(f"{who}: width {t.shape[1]} is not a multiple of 4 up to {SAGE_MAX_WIDTH}")
+
+
+def sage_max_infer(a: ops.DeviceGraph, z: torch.Tensor) -> torch.Tensor:
+    """The evaluation forward of the max-pooling aggregation on a homogeneous graph ``a`` (``bns_sage_max_infer_f32``):
+    ``m[v] = max over u -> v of z[u]`` per column, 0 for a row without entries.  ``z [a.n_cols, Fp]`` -> ``[a.n_rows,
+    Fp]``.  No gradient."""
+    from ._lib import check, lib
+    Fp = z.shape[1] if z.dim() == 2 else -1
+    _sage_check("sage_max_infer", a, ((z, "z", (a.n_cols, Fp), torch.float32),))
+    out = torch.empty(a.n_rows, Fp, dtype=torch.float32, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.bns_sage_max_infer_f32(a._h, Fp, z.data_ptr(), z.stride(0), out.data_ptr(),
+                                         torch.cuda.current_stream(a.device).cuda_stream), "bns_sage_max_infer_f32")
+    return out
+
+
+def sage_max_infer_block(a: ops.DeviceGraph, z: Optional[torch.Tensor], m: torch.Tensor, seen: torch.Tensor,
+                         first: bool, last: bool, out: Optional[torch.Tensor] = None) -> None:
+    """One column block of ``sage_max_infer`` (``bns_sage_max_infer_block_f32``): the rows' running max ``m [a.n_rows,
+    Fp]`` and ``seen [a.n_rows]`` (int32) are carried from the previous block (``first``: from empty); ``last`` writes
+    the max, or 0 for a row that had no entry in any block, to ``out`` (may be ``m``).  ``z [a.n_cols, Fp]``: this
+    block's source rows (None when it has no entries)."""
+    from ._lib import BnsError, check, lib
+    Fp = m.shape[1] if m.dim() == 2 else -1
+    if a.nnz and z is None:
+        raise BnsError("sage_max_infer_block: a block with entries needs z")
+    if last and out is None:
+        raise BnsError("sage_max_infer_block: the last block needs out")
+    _sage_check("sage_max_infer_block", a, ((z, "z", (a.n_cols, Fp), torch.float32),
+                                            (m, "m", (a.n_rows, Fp), torch.float32),
+                                            (seen, "seen", (a.n_rows,), torch.int32),
+                                            (out, "out", (a.n_rows, Fp), torch.float32)))
+    with torch.cuda.device(a.device):
+        check(lib.bns_sage_max_infer_block_f32(a._h, Fp, ops._ptr(z), z.stride(0) if z is not None else Fp, m.data_ptr(),
+                                               seen.data_ptr(), 1 if first else 0, 1 if last else 0, ops._ptr(out),
+                                               torch.cuda.current_stream(a.device).cuda_stream),
+              "bns_sage_max_infer_block_f32")

@@ -14,9 +14,12 @@ _REFERENCE_FLAGS = [
     ("data-path", str, "./dataset/", {}),
     ("part-path", str, "./partition/", {}),
     ("graph-name", str, "", {}),
-    ("model", str, "graphsage", dict(help="graphsage | gcn | gat | gatv2.  gatv2 (NEW) is GAT with dynamic attention "
-                                          "(GATv2Conv: the score attn . leaky_relu(z_src[u] + z_dst[v]) per head), on the "
-                                          "same layer stack, heads, norms and limits as gat")),
+    ("model", str, "graphsage", dict(help="graphsage | gcn | gat | gatv2 | graphsage-pool.  gatv2 (NEW) is GAT with "
+                                          "dynamic attention (GATv2Conv: the score attn . leaky_relu(z_src[u] + z_dst[v]) "
+                                          "per head), on the same layer stack, heads, norms and limits as gat.  "
+                                          "graphsage-pool (NEW) is GraphSAGE with the max-pooling aggregator (SAGEConv "
+                                          "'pool': a max over the sampled neighbours of relu(fc_pool(h)), exchanged rows "
+                                          "unscaled); --heads is ignored")),
     ("dropout", float, 0.5, {}),
     ("lr", float, 1e-2, {}),
     ("sampling-rate", float, 1, {}),

@@ -109,6 +109,17 @@ def get_send_size(boundary, prob):
     return res, ratio
 
 
+def exchange_ratio(model, ratio):
+    """The ratios the exchanged rows (and their returned gradients) are divided by.  Dividing by the sampled share keeps
+    a SUM over the sampled neighbours unbiased, and nothing else: a max over them takes the rows unscaled, so
+    ``graphsage-pool`` gets 1.0 for every peer (the reference's TODO in ``get_send_size``).  Every other model keeps
+    ``get_send_size``'s ratios, GAT included."""
+    if model != 'graphsage-pool':
+        return ratio
+    rank, _ = _rank_size()
+    return [0 if i == rank else 1.0 for i in range(len(ratio))]
+
+
 def get_recv_size(node_dict, prob):
     """train.py:122-131."""
     rank, size = _rank_size()
@@ -233,7 +244,7 @@ def precompute(part: PartitionGraph, graph, node_dict, boundary, model, gpb, pos
             # fn.mean divides by the number of messages = the full in-degree (every in-edge is present here)
             mean = PartitionAggregate.apply(h_u, g, 1.0 / node_dict['in_deg'].float(), None, None, None)
             return torch.cat([feat, mean[:, :n_feat]], dim=1)
-        elif model in ('gat', 'gatv2'):
+        elif model in ('gat', 'gatv2', 'graphsage-pool'):
             return h_u[:, :n_feat]
         raise Exception
 
@@ -296,6 +307,10 @@ def create_model(layer_size, args):
         from .module.gatv2 import GATv2Conv
         return GAT(layer_size, F.relu, use_pp=True, heads=args.heads, norm=args.norm, dropout=args.dropout,
                    train_size=args.n_train, n_linear=args.n_linear, conv=GATv2Conv)
+    elif args.model == 'graphsage-pool':
+        from .module.sage_pool import SAGEPoolConv
+        return GAT(layer_size, F.relu, use_pp=True, norm=args.norm, dropout=args.dropout, train_size=args.n_train,
+                   n_linear=args.n_linear, conv=lambda n_in, n_out, _heads, drop, _: SAGEPoolConv(n_in, n_out, drop))
     raise NotImplementedError(args.model)
 
 
@@ -454,7 +469,8 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     node_dict = dict(node_dict)
     in_graph, out_graph = get_in_out_graph(graph, node_dict, dev, getattr(args, 'chunk_nnz', 0))
     part = PartitionGraph(graph.n_in, graph.n_halo, in_graph, out_graph, dev)
-    part.want_positions = args.model in ('gat', 'gatv2')   # the attention keeps per-entry values at CSR positions
+    # the attention keeps per-entry values at CSR positions; the max records its winners by position
+    part.want_positions = args.model in ('gat', 'gatv2', 'graphsage-pool')
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
     agg = check_agg_dtype(args, layer_size, dev)
@@ -490,9 +506,12 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     part_train = int(node_dict['train_mask'].int().sum().item())
     pos = get_pos(node_dict, gpb)
     send_size, ratio = get_send_size(boundary, args.sampling_rate)
+    ratio = exchange_ratio(args.model, ratio)
     recv_size = get_recv_size(node_dict, args.sampling_rate)
+    # graphsage-pool's layer 0 always takes the stored halo rows: --use-pp does not change it
+    use_pp = args.use_pp or args.model == 'graphsage-pool'
     ctx.buffer.init_buffer(in_graph.n_rows, ratio, send_size, recv_size,
-                           layer_size[:args.n_layers - args.n_linear], use_pp=args.use_pp, backend=args.backend,
+                           layer_size[:args.n_layers - args.n_linear], use_pp=use_pp, backend=args.backend,
                            device=dev, comm_dtype=comm_dtype)
     if size > 1 and ctx.buffer._get()._p2p is not None:
         # slot map + the inverse maps of the gradient scatter in ONE allocation (one memset + one kernel per epoch)
@@ -501,7 +520,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
         part.slot = maps[:n_slot]
         ctx.buffer._get().set_maps(maps, n_slot, pos)
     out_deg_all = collect_out_degree(node_dict, boundary)                   # train.py:350
-    if args.use_pp:
+    if use_pp:
         halo_bytes = graph.n_halo * node_dict['feat'].shape[1] * 4
         stream = getattr(args, 'streaming_precompute', None)
         if stream is None:                  # automatic: when all the halo rows together would not fit comfortably
@@ -573,7 +592,7 @@ def _forward_logits(st: TrainState, epoch: int, selected: Optional[list] = None)
         return st.model(g, st.feat, st.in_norm, st.out_norm)
     elif args.model == 'graphsage':
         return st.model(g, st.feat, st.in_norm)
-    elif args.model in ('gat', 'gatv2'):
+    elif args.model in ('gat', 'gatv2', 'graphsage-pool'):
         return st.model(g, construct_feat(g.num_nodes('_V'), st.feat, st.pos, one_hops))        # train.py:401-402
     raise NotImplementedError
 

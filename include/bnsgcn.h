@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 13
+#define BNS_ABI_VERSION 14
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -750,6 +750,34 @@ int bns_gatv2_infer_f32(const bns_graph_t *g, const float *zs, int64_t ldzs, con
 int bns_gatv2_infer_block_f32(const bns_graph_t *g, const float *zs, int64_t ldzs, const float *zd, int64_t ldzd,
                               const float *attn, int32_t heads, int32_t Fp, float slope, float *m, float *l, float *acc,
                               int64_t ldacc, int first, int last, float *rst, int64_t ldr, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 14: GraphSAGE's max-pooling aggregator (--model graphsage-pool, csrc/sage_pool.cuh).  z [n_u, F] (row stride ldz)
+ * holds relu(fc_pool(x)), finite, with F a multiple of 4 and at most 1024 (pad columns zero), 16-byte aligned rows;
+ * m, win, dm and d_y are contiguous [rows, F].  Per destination row v and column f, m[v, f] = max over the entries
+ * u -> v of z[u, f], 0 for a row without entries; -0 is stored as +0, so m does not depend on the order of the entries.
+ * bns_sage_max_f32: over the inner entries (a_in) and this epoch's sampled halo entries (a_out through the compaction
+ *     cidx / chunk_cnt / cpos, with positions, as bns_gat_scores_f32): m [n_in, F] and win [n_in, F], the position of
+ *     the first entry in that walk order whose z equals the max (a_in position, or nnz_in + a_out position for a halo
+ *     entry; -1 for a row without entries).  Refuses nnz_in + nnz_out > INT32_MAX.
+ * bns_sage_max_bwd_f32: on a transpose gT (bns_graph_transpose) of a_in with pos_base = 0, or of a_out with pos_base =
+ *     nnz_in, row_map = slot and out_base = n_in: d_y[out_base + orow(r)] = (z[...] > 0) * sum over the entries k of
+ *     row r, in gT's order, of dm[gT.indices[k], f] where win[gT.indices[k], f] == pos_base + perm[k] (rows with
+ *     row_map -1 skipped; a row without a winning entry gets 0).  No float atomics.
+ * bns_sage_max_infer_f32: m over every entry of a homogeneous graph, no winner.  bns_sage_max_infer_block_f32: the same
+ *     over column blocks, the running max m [n_rows, F] and seen [n_rows] (int32) carried between launches (first: from
+ *     empty; a launch that is not last stores them; last writes the max, or 0 for a row never seen, to out, which may
+ *     be m).  The result equals the single pass bit for bit for any split of the columns.
+ * Two launches on the same inputs give bit-identical results.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_sage_max_f32(const bns_graph_t *a_in, const bns_graph_t *a_out, const int32_t *cidx, const int32_t *chunk_cnt,
+                     const int32_t *cpos, int64_t x_halo_base, int32_t F, const float *z, int64_t ldz, float *m,
+                     int32_t *win, void *stream);
+int bns_sage_max_bwd_f32(const bns_graph_t *gT, int64_t pos_base, const int32_t *row_map, int64_t out_base, int32_t F,
+                         const int32_t *win, const float *dm, const float *z, int64_t ldz, float *d_y, void *stream);
+int bns_sage_max_infer_f32(const bns_graph_t *g, int32_t F, const float *z, int64_t ldz, float *out, void *stream);
+int bns_sage_max_infer_block_f32(const bns_graph_t *g, int32_t F, const float *z, int64_t ldz, float *m, int32_t *seen,
+                                 int first, int last, float *out, void *stream);
 
 #ifdef __cplusplus
 }
