@@ -13,7 +13,7 @@ from ctypes import POINTER, Structure, c_char_p, c_float, c_int, c_int32, c_int6
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "libbnsgcn.so")
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 P2P_HANDLE_BYTES = 64
 COMM_ID_BYTES = 128
 
@@ -228,6 +228,18 @@ SIGNATURES = {
     "bns_sage_max_infer_f32": (c_int, [c_void_p, c_int32, c_void_p, c_int64, c_void_p, c_void_p]),
     "bns_sage_max_infer_block_f32": (c_int, [c_void_p, c_int32, c_void_p, c_int64, c_void_p, c_void_p, c_int, c_int,
                                              c_void_p, c_void_p]),
+    # ---- ABI 15 ----
+    "bns_tconv_scores_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_void_p,
+                                     c_int64, c_void_p, c_int64, c_float, c_float, c_uint64, c_uint64, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "bns_tconv_softmax_bwd_f32": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32,
+                                          c_void_p, c_int64, c_void_p, c_int64, c_float, c_float, c_uint64, c_uint64,
+                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p]),
+    "bns_tconv_infer_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int32, c_int32,
+                                    c_float, c_void_p, c_int64, c_void_p]),
+    "bns_tconv_infer_block_f32": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_int32,
+                                          c_int32, c_float, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p,
+                                          c_int64, c_void_p]),
 }
 
 

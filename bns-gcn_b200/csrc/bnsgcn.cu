@@ -2354,6 +2354,7 @@ extern "C" int bns_p2p_wait_flag(bns_p2p_t *p, int32_t flag_index, uint64_t flag
 #include "gat.cuh"
 #include "gatv2.cuh"
 #include "sage_pool.cuh"
+#include "transformer.cuh"
 #include "comm.cuh"
 
 // =================================================================================================

@@ -203,11 +203,12 @@ def eval_input(args, g, feat: torch.Tensor) -> torch.Tensor:
     in-neighbours]`` and GCN's ``D_in^-1/2 A D_out^-1/2 x`` over the inner rows; GAT (its layer 0 always takes the
     stored rows, ``train.create_model``) the inner rows followed by every halo row.  Degrees are those of ``g``'s own
     graph; the halo rows come through ``g``'s exchange (collective)."""
-    if not (args.use_pp or args.model in ('gat', 'gatv2', 'graphsage-pool')):
+    from .train import ATTENTION_STACK
+    if not (args.use_pp or args.model in ATTENTION_STACK):
         return feat
     n_in, n_feat = feat.shape
     with torch.no_grad():
-        if args.model in ('gat', 'gatv2', 'graphsage-pool'):
+        if args.model in ATTENTION_STACK:
             h = torch.empty(n_in + g.n_halo, n_feat, dtype=feat.dtype, device=feat.device)
             h[:n_in] = feat
             for j, _, xr in g.peer_rows(feat.contiguous()):

@@ -748,3 +748,152 @@ def sage_max_infer_block(a: ops.DeviceGraph, z: Optional[torch.Tensor], m: torch
                                                seen.data_ptr(), 1 if first else 0, 1 if last else 0, ops._ptr(out),
                                                torch.cuda.current_stream(a.device).cuda_stream),
               "bns_sage_max_infer_block_f32")
+
+
+class TconvAttention(torch.autograd.Function):
+    """The scaled dot-product attention of the graph transformer layer (``torch_geometric.nn.TransformerConv``) for all
+    heads:
+
+        s_uv = scale * <q_v, k_u>,   rst_v = sum_u attn_drop(edge_softmax(s))_uv * v_u
+
+    over the inner entries and this epoch's sampled halo entries, as ``Gatv2Attention``.  ``q [n_in, H * Fp]`` and
+    ``kv [n_u, 2 * H * Fp]``, the key rows in its first ``H * Fp`` columns and the value rows in the rest (per-head
+    widths padded to ``Fp``, pad columns zero) -> ``[n_in, H * Fp]``; gradients for both.
+
+    Stages (include/bnsgcn.h, ABI 15): ``bns_tconv_scores_f32`` (scores -> probabilities + dropped attention per entry)
+    -> ``bns_spmm_weighted_f32`` / ``bns_spmm_compact_f32`` per head on the value columns; backward
+    ``bns_sddmm_dot_f32`` -> ``bns_tconv_softmax_bwd_f32`` (d s, d q) -> ``bns_spmm_weighted_f32`` on the transposes
+    (d v with the attention, d k with d s)."""
+
+    @staticmethod
+    def forward(ctx, q, kv, g: PartitionGraph, H: int, Fp: int, scale: float, p: float, seed: int):
+        from ._lib import check, lib
+        q, kv = q.contiguous(), kv.contiguous()
+        HF = H * Fp
+        n_in, dev = g.n_in, kv.device
+        if q.shape != (n_in, HF) or kv.dim() != 2 or kv.shape[1] != 2 * HF:
+            raise RuntimeError(f"TconvAttention: q must be [{n_in}, {HF}] and kv [*, {2 * HF}], got {tuple(q.shape)} "
+                               f"and {tuple(kv.shape)}")
+        c = g.compact if (g.a_out is not None and kv.shape[0] > n_in) else None
+        if c is None and g.a_out is not None and g.a_out.nnz and kv.shape[0] > n_in:
+            raise RuntimeError("TconvAttention: halo rows were passed but the partition graph has no compaction "
+                               "(refresh_compaction)")
+        if c is not None and c.cpos is None:
+            raise RuntimeError("TconvAttention: the partition graph was compacted without positions (want_positions)")
+        rst = torch.empty(n_in, HF, dtype=torch.float32, device=dev)
+        p_in = torch.empty(max(g.a_in.nnz, 1), H, dtype=torch.float32, device=dev)
+        p_out = torch.empty(max(g.a_out.nnz, 1), H, dtype=torch.float32, device=dev) if c is not None else None
+        w_in = torch.empty_like(p_in) if p > 0 else None
+        w_out = torch.empty_like(p_out) if p > 0 and p_out is not None else None
+        wc = torch.empty_like(p_out) if p_out is not None else None
+        off, off_dev = ops.RNG["offset"], ops.RNG["offset_dev"]
+        head = (g.a_in._h, None if c is None else g.a_out._h, None if c is None else c.cidx.data_ptr(),
+                None if c is None else c.chunk_cnt.data_ptr(), None if c is None else c.cpos.data_ptr(), n_in, H, Fp)
+        tail = (q.data_ptr(), q.stride(0), kv.data_ptr(), kv.stride(0), float(scale), float(p), seed & (2 ** 64 - 1),
+                off & (2 ** 64 - 1), ops._ptr(off_dev))
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):
+            check(lib.bns_tconv_scores_f32(*head, *tail, p_in.data_ptr(), ops._ptr(p_out), ops._ptr(w_in),
+                                           ops._ptr(w_out), ops._ptr(wc), st), "bns_tconv_scores_f32")
+        for h in range(H):
+            cols, vcols = slice(h * Fp, (h + 1) * Fp), slice(HF + h * Fp, HF + (h + 1) * Fp)
+            ops.spmm_weighted(g.a_in, kv[:n_in, vcols], rst[:, cols], p_in if w_in is None else w_in, h)
+            if c is not None:
+                ops.spmm_compact(c, kv[n_in:, vcols], rst[:, cols], accumulate=True, weights=wc, head=h)
+        ctx.g, ctx.c, ctx.head, ctx.tail, ctx.cfg = g, c, head, tail, (H, Fp)
+        saved = [q, kv, p_in] + ([p_out] if p_out is not None else [])
+        if w_in is not None:
+            saved += [w_in] + ([w_out] if w_out is not None else [])
+        ctx.n_w = 0 if w_in is None else (2 if w_out is not None else 1)
+        ctx.save_for_backward(*saved)
+        return rst
+
+    @staticmethod
+    def backward(ctx, d_rst):
+        from ._lib import check, lib
+        g, c = ctx.g, ctx.c
+        H, Fp = ctx.cfg
+        HF = H * Fp
+        q, kv, p_in, *rest = ctx.saved_tensors
+        p_out = rest.pop(0) if c is not None else None
+        d_rst = d_rst.contiguous()
+        dev, n_in, n_u = kv.device, g.n_in, kv.shape[0]
+        de_in = torch.empty_like(p_in)
+        de_out = torch.empty_like(p_out) if p_out is not None else None
+        w_in, w_out = p_in, p_out
+        if ctx.n_w:
+            w_in = rest.pop(0)
+            w_out = rest.pop(0) if ctx.n_w == 2 else None
+        for h in range(H):                                     # d a'_uv = <d rst_v, v_u>
+            cols, vcols = slice(h * Fp, (h + 1) * Fp), slice(HF + h * Fp, HF + (h + 1) * Fp)
+            ops.sddmm_dot(g.a_in, d_rst[:, cols], kv[:n_in, vcols], out=de_in[:, h])
+            if c is not None:
+                ops.sddmm_dot(g.a_out, d_rst[:, cols], kv[n_in:, vcols], col_map=g.slot, n_direct=0, out=de_out[:, h])
+        d_q = torch.empty(n_in, HF, dtype=torch.float32, device=dev)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        with torch.cuda.device(dev):                           # d s in place of d a', and d q
+            check(lib.bns_tconv_softmax_bwd_f32(*ctx.head, *ctx.tail, p_in.data_ptr(), ops._ptr(p_out), de_in.data_ptr(),
+                                                ops._ptr(de_out), d_q.data_ptr(), d_q.stride(0), st),
+                  "bns_tconv_softmax_bwd_f32")
+        d_kv = torch.empty(n_u, 2 * HF, dtype=torch.float32, device=dev)
+        for h in range(H):                                     # d v = A'^T d rst, d k = dS^T q
+            cols, vcols = slice(h * Fp, (h + 1) * Fp), slice(HF + h * Fp, HF + (h + 1) * Fp)
+            ops.spmm_weighted(g.a_in_t, d_rst[:, cols], d_kv[:n_in, vcols], w_in, h, through_perm=True)
+            ops.spmm_weighted(g.a_in_t, q[:, cols], d_kv[:n_in, cols], de_in, h, through_perm=True)
+            if c is not None:
+                ops.spmm_weighted(g.a_out_t, d_rst[:, cols], d_kv[n_in:, vcols], w_out, h, through_perm=True,
+                                  row_map=g.slot)
+                ops.spmm_weighted(g.a_out_t, q[:, cols], d_kv[n_in:, cols], de_out, h, through_perm=True,
+                                  row_map=g.slot)
+        return d_q, d_kv, None, None, None, None, None, None
+
+
+def _tconv_ptrs(kv: Optional[torch.Tensor], HF: int):
+    """``(k, ldk, v, ldv)`` arguments for the two halves of a ``[n, 2 * HF]`` key / value table (None: no table)."""
+    if kv is None:
+        return None, 2 * HF, None, 2 * HF
+    return kv.data_ptr(), kv.stride(0), kv.data_ptr() + 4 * HF, kv.stride(0)
+
+
+def tconv_infer(a: ops.DeviceGraph, q: torch.Tensor, kv: torch.Tensor, H: int, Fp: int, scale: float) -> torch.Tensor:
+    """The evaluation forward of the graph transformer layer's attention on a homogeneous graph ``a``
+    (``bns_tconv_infer_f32``):
+
+        rst[v] = sum_{u -> v} softmax_u(scale * <q[v, h], k[u, h]>) * v[u, h]
+
+    ``q [a.n_rows, H * Fp]``, ``kv [a.n_cols, 2 * H * Fp]`` (key columns, then value columns; head-major, ``Fp`` a
+    multiple of 4, pad columns zero) -> ``[a.n_rows, H * Fp]``.  No dropout, no gradient."""
+    from ._lib import check, lib
+    HF = H * Fp
+    _gatv2_check("tconv_infer", a, H, Fp, ((q, "q", (a.n_rows, HF)), (kv, "kv", (a.n_cols, 2 * HF))))
+    rst = torch.empty(a.n_rows, HF, dtype=torch.float32, device=a.device)
+    with torch.cuda.device(a.device):
+        check(lib.bns_tconv_infer_f32(a._h, q.data_ptr(), q.stride(0), *_tconv_ptrs(kv, HF), H, Fp, float(scale),
+                                      rst.data_ptr(), rst.stride(0), torch.cuda.current_stream(a.device).cuda_stream),
+              "bns_tconv_infer_f32")
+    return rst
+
+
+def tconv_infer_block(a: ops.DeviceGraph, q: torch.Tensor, kv: Optional[torch.Tensor], H: int, Fp: int, scale: float,
+                      m: torch.Tensor, l: torch.Tensor, acc: torch.Tensor, first: bool, last: bool,
+                      rst: Optional[torch.Tensor] = None) -> None:
+    """One column block of ``tconv_infer`` (``bns_tconv_infer_block_f32``), the online-softmax state ``m``, ``l``
+    ``[a.n_rows, H]`` and ``acc [a.n_rows, H * Fp]`` carried as in ``gatv2_infer_block``; ``last`` writes ``acc / l`` to
+    ``rst`` (may be ``acc``).  ``kv [a.n_cols, 2 * H * Fp]`` are this block's source rows (None when it has no
+    entries)."""
+    from ._lib import BnsError, check, lib
+    HF = H * Fp
+    if a.nnz and kv is None:
+        raise BnsError("tconv_infer_block: a block with entries needs kv")
+    if last and rst is None:
+        raise BnsError("tconv_infer_block: the last block needs rst")
+    _gatv2_check("tconv_infer_block", a, H, Fp, ((q, "q", (a.n_rows, HF)), (kv, "kv", (a.n_cols, 2 * HF)),
+                                                 (m, "m", (a.n_rows, H)), (l, "l", (a.n_rows, H)),
+                                                 (acc, "acc", (a.n_rows, HF)), (rst, "rst", (a.n_rows, HF))))
+    with torch.cuda.device(a.device):
+        check(lib.bns_tconv_infer_block_f32(a._h, q.data_ptr(), q.stride(0), *_tconv_ptrs(kv, HF), H, Fp, float(scale),
+                                            m.data_ptr(), l.data_ptr(), acc.data_ptr(), acc.stride(0),
+                                            1 if first else 0, 1 if last else 0, ops._ptr(rst),
+                                            rst.stride(0) if rst is not None else HF,
+                                            torch.cuda.current_stream(a.device).cuda_stream),
+              "bns_tconv_infer_block_f32")

@@ -14,12 +14,15 @@ _REFERENCE_FLAGS = [
     ("data-path", str, "./dataset/", {}),
     ("part-path", str, "./partition/", {}),
     ("graph-name", str, "", {}),
-    ("model", str, "graphsage", dict(help="graphsage | gcn | gat | gatv2 | graphsage-pool.  gatv2 (NEW) is GAT with "
+    ("model", str, "graphsage", dict(help="graphsage | gcn | gat | gatv2 | graphsage-pool | transformer.  gatv2 (NEW) is GAT with "
                                           "dynamic attention (GATv2Conv: the score attn . leaky_relu(z_src[u] + z_dst[v]) "
                                           "per head), on the same layer stack, heads, norms and limits as gat.  "
                                           "graphsage-pool (NEW) is GraphSAGE with the max-pooling aggregator (SAGEConv "
                                           "'pool': a max over the sampled neighbours of relu(fc_pool(h)), exchanged rows "
-                                          "unscaled); --heads is ignored")),
+                                          "unscaled); --heads is ignored.  transformer (NEW) is the graph transformer "
+                                          "layer (TransformerConv: scaled dot-product attention <q_v, k_u> / sqrt(C), "
+                                          "heads averaged, plus a root weight), on GAT's stack, heads, norms and "
+                                          "limits, exchanged rows unscaled")),
     ("dropout", float, 0.5, {}),
     ("lr", float, 1e-2, {}),
     ("sampling-rate", float, 1, {}),

@@ -131,7 +131,8 @@ class GAT(GNNBase):
     """module/model.py:96-132: attention layers take the ``(source rows, destination rows)`` pair, heads are averaged,
     dropout sits inside the attention layers (and before the closing linear layers only).  ``conv`` is the attention
     layer's class, built as ``conv(in, out, heads, dropout, dropout)``: ``GATConv`` (the default) or ``GATv2Conv``
-    (``--model gatv2``); ``--model graphsage-pool`` passes a factory of one-head ``SAGEPoolConv`` layers."""
+    (``--model gatv2``) or ``TransformerConv`` (``--model transformer``); ``--model graphsage-pool`` passes a
+    factory of one-head ``SAGEPoolConv`` layers."""
 
     def __init__(self, layer_size, activation, use_pp, heads=1, dropout=0.5, norm='layer', train_size=None, n_linear=0,
                  conv=None):

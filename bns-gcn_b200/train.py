@@ -109,12 +109,19 @@ def get_send_size(boundary, prob):
     return res, ratio
 
 
+# the models built on GAT's layer stack (``module.model.GAT``): layer 0 takes the stored halo rows, and the attention
+# layers keep per-entry values at the partition graph's CSR positions
+ATTENTION_STACK = ('gat', 'gatv2', 'graphsage-pool', 'transformer')
+
+
 def exchange_ratio(model, ratio):
     """The ratios the exchanged rows (and their returned gradients) are divided by.  Dividing by the sampled share keeps
     a SUM over the sampled neighbours unbiased, and nothing else: a max over them takes the rows unscaled, so
-    ``graphsage-pool`` gets 1.0 for every peer (the reference's TODO in ``get_send_size``).  Every other model keeps
-    ``get_send_size``'s ratios, GAT included."""
-    if model != 'graphsage-pool':
+    ``graphsage-pool`` gets 1.0 for every peer (the reference's TODO in ``get_send_size``).  So does ``transformer``:
+    its softmax takes a convex combination over whichever neighbours were sampled, and a sampled row divided by the
+    sampled share would inflate both its key and its value.  Every other model keeps ``get_send_size``'s ratios, GAT
+    and GATv2 included."""
+    if model not in ('graphsage-pool', 'transformer'):
         return ratio
     rank, _ = _rank_size()
     return [0 if i == rank else 1.0 for i in range(len(ratio))]
@@ -244,7 +251,7 @@ def precompute(part: PartitionGraph, graph, node_dict, boundary, model, gpb, pos
             # fn.mean divides by the number of messages = the full in-degree (every in-edge is present here)
             mean = PartitionAggregate.apply(h_u, g, 1.0 / node_dict['in_deg'].float(), None, None, None)
             return torch.cat([feat, mean[:, :n_feat]], dim=1)
-        elif model in ('gat', 'gatv2', 'graphsage-pool'):
+        elif model in ATTENTION_STACK:
             return h_u[:, :n_feat]
         raise Exception
 
@@ -311,6 +318,10 @@ def create_model(layer_size, args):
         from .module.sage_pool import SAGEPoolConv
         return GAT(layer_size, F.relu, use_pp=True, norm=args.norm, dropout=args.dropout, train_size=args.n_train,
                    n_linear=args.n_linear, conv=lambda n_in, n_out, _heads, drop, _: SAGEPoolConv(n_in, n_out, drop))
+    elif args.model == 'transformer':
+        from .module.transformer import TransformerConv
+        return GAT(layer_size, F.relu, use_pp=True, heads=args.heads, norm=args.norm, dropout=args.dropout,
+                   train_size=args.n_train, n_linear=args.n_linear, conv=TransformerConv)
     raise NotImplementedError(args.model)
 
 
@@ -470,7 +481,7 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     in_graph, out_graph = get_in_out_graph(graph, node_dict, dev, getattr(args, 'chunk_nnz', 0))
     part = PartitionGraph(graph.n_in, graph.n_halo, in_graph, out_graph, dev)
     # the attention keeps per-entry values at CSR positions; the max records its winners by position
-    part.want_positions = args.model in ('gat', 'gatv2', 'graphsage-pool')
+    part.want_positions = args.model in ATTENTION_STACK
     boundary = get_boundary({k: v.to(dev) for k, v in node_dict.items() if k in ('part_id', NID)}, gpb)
     layer_size = get_layer_size(args.n_feat, args.n_hidden, args.n_class, args.n_layers)
     agg = check_agg_dtype(args, layer_size, dev)
@@ -508,8 +519,8 @@ def setup(graph: LocalGraph, node_dict, gpb, args, device=None) -> TrainState:
     send_size, ratio = get_send_size(boundary, args.sampling_rate)
     ratio = exchange_ratio(args.model, ratio)
     recv_size = get_recv_size(node_dict, args.sampling_rate)
-    # graphsage-pool's layer 0 always takes the stored halo rows: --use-pp does not change it
-    use_pp = args.use_pp or args.model == 'graphsage-pool'
+    # graphsage-pool's and transformer's layer 0 always takes the stored halo rows: --use-pp does not change it
+    use_pp = args.use_pp or args.model in ('graphsage-pool', 'transformer')
     ctx.buffer.init_buffer(in_graph.n_rows, ratio, send_size, recv_size,
                            layer_size[:args.n_layers - args.n_linear], use_pp=use_pp, backend=args.backend,
                            device=dev, comm_dtype=comm_dtype)
@@ -592,7 +603,7 @@ def _forward_logits(st: TrainState, epoch: int, selected: Optional[list] = None)
         return st.model(g, st.feat, st.in_norm, st.out_norm)
     elif args.model == 'graphsage':
         return st.model(g, st.feat, st.in_norm)
-    elif args.model in ('gat', 'gatv2', 'graphsage-pool'):
+    elif args.model in ATTENTION_STACK:
         return st.model(g, construct_feat(g.num_nodes('_V'), st.feat, st.pos, one_hops))        # train.py:401-402
     raise NotImplementedError
 

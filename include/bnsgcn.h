@@ -36,7 +36,7 @@ extern "C" {
 #define BNS_E_WORKSPACE  (-3)   /* workspace too small */
 #define BNS_E_UNSUPPORTED (-4)
 
-#define BNS_ABI_VERSION 14
+#define BNS_ABI_VERSION 15
 
 typedef struct bns_graph bns_graph_t;   /* opaque: a static CSR matrix resident in HBM */
 typedef struct bns_p2p   bns_p2p_t;     /* opaque: peer-mapped exchange slabs of one rank */
@@ -778,6 +778,40 @@ int bns_sage_max_bwd_f32(const bns_graph_t *gT, int64_t pos_base, const int32_t 
 int bns_sage_max_infer_f32(const bns_graph_t *g, int32_t F, const float *z, int64_t ldz, float *out, void *stream);
 int bns_sage_max_infer_block_f32(const bns_graph_t *g, int32_t F, const float *z, int64_t ldz, float *m, int32_t *seen,
                                  int first, int last, float *out, void *stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * ABI 15: the graph transformer layer's scaled dot-product attention (--model transformer, csrc/transformer.cuh).
+ * q [n_in, heads * Fp], k and v [n_u, heads * Fp] are head-major with the per-head width padded to Fp (a multiple of 4,
+ * pad columns zero), 16-byte aligned rows with their own row strides (k and v may be the two halves of one
+ * [n_u, 2 * heads * Fp] table); 1 <= heads <= 8 and heads * Fp <= 1024; scale finite and positive.  Per entry u -> v
+ * and head h
+ *     s_uv = scale * <q[v, h, :], k[u, h, :]>.
+ * bns_tconv_scores_f32: bns_gatv2_scores_f32 with these scores: the same graph arguments, P / W / W_out_compact outputs
+ *     and dropout mask (GAT's Philox stream and entry numbering).  The aggregation A' v is bns_spmm_weighted_f32 /
+ *     bns_spmm_compact_f32 and d a' = <d rst_v, v[u]> is bns_sddmm_dot_f32.
+ * bns_tconv_softmax_bwd_f32: dE holds d a' at the original positions; writes d s = scale P (g - sum_u P g) in place
+ *     (g = d a' * mask / (1 - p)) and d_q [n_in, heads * Fp] (row stride ldd) = sum_u d s_uv k[u], one warp per row, no
+ *     atomics.  d k = sum_v d s_uv q[v] and d v = A'^T d rst are bns_spmm_weighted_f32 on the transposes.
+ * bns_tconv_infer_f32: the evaluation forward on a homogeneous graph: rst = sum_u softmax_u(s_uv) v[u], one pass per
+ *     row, nothing stored per entry.  bns_tconv_infer_block_f32: the same over column blocks, the state m, l [n_rows,
+ *     heads] and acc [n_rows, heads * Fp] carried between launches as in bns_gatv2_infer_block_f32.
+ * Every kernel sums in an order fixed by the inputs: two launches give bit-identical results.
+ * ----------------------------------------------------------------------------------------------*/
+int bns_tconv_scores_f32(const bns_graph_t *a_in, const bns_graph_t *a_out, const int32_t *cidx, const int32_t *chunk_cnt,
+                         const int32_t *cpos, int64_t x_halo_base, int32_t heads, int32_t Fp, const float *q, int64_t ldq,
+                         const float *k, int64_t ldk, float scale, float p_drop, uint64_t seed, uint64_t offset,
+                         const uint64_t *offset_dev, float *P_in, float *P_out, float *W_in, float *W_out,
+                         float *W_out_compact, void *stream);
+int bns_tconv_softmax_bwd_f32(const bns_graph_t *a_in, const bns_graph_t *a_out, const int32_t *cidx,
+                              const int32_t *chunk_cnt, const int32_t *cpos, int64_t x_halo_base, int32_t heads, int32_t Fp,
+                              const float *q, int64_t ldq, const float *k, int64_t ldk, float scale, float p_drop,
+                              uint64_t seed, uint64_t offset, const uint64_t *offset_dev, const float *P_in,
+                              const float *P_out, float *dE_in, float *dE_out, float *d_q, int64_t ldd, void *stream);
+int bns_tconv_infer_f32(const bns_graph_t *g, const float *q, int64_t ldq, const float *k, int64_t ldk, const float *v,
+                        int64_t ldv, int32_t heads, int32_t Fp, float scale, float *rst, int64_t ldr, void *stream);
+int bns_tconv_infer_block_f32(const bns_graph_t *g, const float *q, int64_t ldq, const float *k, int64_t ldk,
+                              const float *v, int64_t ldv, int32_t heads, int32_t Fp, float scale, float *m, float *l,
+                              float *acc, int64_t ldacc, int first, int last, float *rst, int64_t ldr, void *stream);
 
 #ifdef __cplusplus
 }
